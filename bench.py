@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py - headline benchmark of the UniVTG hot path on B200 (contract in the task statement).
+"""bench.py - headline benchmark of the UniVTG hot path on H100.
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--workload NAME]
 
@@ -26,6 +26,7 @@ import time
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
+import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
 from univtg_b200 import synth  # noqa: E402
@@ -51,7 +52,8 @@ def load_peaks():
         z = json.load(open(p))
         return dict(hbm_gbs=z["hbm_gbs"], tflops_burst=z["bf16_tflops"], tflops_sustained=z["bf16_tflops_sustained"],
                     source="measured (MEASURED_PEAKS.json)")
-    return dict(hbm_gbs=6650.0, tflops_burst=1590.0, tflops_sustained=1400.0, source="fallback (B200_PROFILING.md)")
+    # NVIDIA H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense BF16 / FP16 - not reached, a ceiling for the ratio
+    return dict(hbm_gbs=3350.0, tflops_burst=989.0, tflops_sustained=989.0, source="H100 SXM data sheet")
 
 
 class ClockSampler:
@@ -100,7 +102,7 @@ class ClockSampler:
 
 
 def gemm_flops_forward(cfg):
-    """Algorithmic FLOPs of everything the tcgen05 GEMM kernel executes in one forward (projectors, QKV/out/FFN, conv 1-2)."""
+    """Algorithmic FLOPs of everything the tensor-core GEMM kernel executes in one forward (projectors, QKV/out/FFN, conv 1-2)."""
     d, ff, N = cfg["hidden_dim"], cfg["dim_feedforward"], cfg["enc_layers"]
     B, Lv, Lt = cfg["batch"], cfg["l_vid"], cfg["l_txt"]
     L = Lv + Lt
@@ -119,7 +121,7 @@ def workload_config(workload, wl, cfg, n_gpus):
             "t_feat_dim": cfg["t_feat_dim"],
             "step": ("forward + criterion + backward + clip_grad_norm(0.1) + AdamW, input_dropout 0.5, droppath 0.1"
                      if wl["mode"] == "train" else "inference forward"),
-            "l2_policy": "rotating input batches larger than the 126 MB L2 in total"}
+            "l2_policy": "rotating input batches larger than the 50 MB L2 in total"}
 
 
 def oracle_step_fn(cfg, mode, batch, device="cpu", dtype=None, autocast=None):
@@ -155,7 +157,7 @@ def oracle_step_fn(cfg, mode, batch, device="cpu", dtype=None, autocast=None):
 
 
 def gpu_eager_baseline(cfg, wl, dev, steps=10):
-    """The "second bar" of SURVEY.md section 8(d) / BASELINE.md section 3: the reference's fp32 PyTorch path run on the SAME B200
+    """The "second bar" of SURVEY.md section 8(d) / BASELINE.md section 3: the reference's fp32 PyTorch path run on the SAME GPU
     through torch eager (cuBLAS / ATen kernels) - here the oracle port of that path (oracle/univtg_oracle.py is device-agnostic
     tensor algebra; the reference itself cannot travel to the GPU box).  Three precisions: strict fp32, TF32 matmuls, bf16 autocast.
     A baseline beside the product, never part of it."""
@@ -502,6 +504,31 @@ def emit_json_line(line):
     print(json.dumps(line), flush=True)
 
 
+DUMP_CAP_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, last):
+    """The arrays the timed path returned in its last step, as float32 .npy files (every model output and, when training, every
+    loss term and the weighted total).  At most DUMP_CAP_BYTES in all: when the outputs are larger, every array of more than 64 Ki
+    elements is replaced by a fixed, seeded sample of its flattened elements (the same elements for the same shapes) so that the
+    large arrays share what the small ones leave of the cap; two builds still compare element for element."""
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {k: v for k, v in last["out"].items() if torch.is_tensor(v) and v.is_floating_point()}
+    arrays.update({f"loss_{k}": v for k, v in last.get("losses", {}).items()})
+    if "total" in last:
+        arrays["loss_total"] = last["total"]
+    arrays = {k: v.detach().float().cpu().numpy() for k, v in arrays.items()}
+    large = 4 * sum(a.size for a in arrays.values() if a.size > 65536)
+    small = 4 * sum(a.size for a in arrays.values() if a.size <= 65536)
+    scale = min(1.0, (DUMP_CAP_BYTES - small) / large) if large else 1.0
+    for k, a in arrays.items():
+        keep = int(a.size * scale) if a.size > 65536 else a.size
+        if keep < a.size:
+            idx = np.sort(np.random.default_rng(0).choice(a.size, size=keep, replace=False))
+            a = a.reshape(-1)[idx]
+        np.save(os.path.join(out_dir, f"{k}.npy"), a)
+
+
 def main():
     _quiet_stdout()
     ap = argparse.ArgumentParser()
@@ -522,15 +549,21 @@ def main():
     ap.add_argument("--static-loss-scale", action="store_true", help="fixed fp16 loss scale (no overflow flag read-back)")
     ap.add_argument("--no-zero-after-step", action="store_true",
                     help="zero the flat gradient buffer in front of the backward instead of on a side stream behind the optimizer step")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step computed (model outputs, losses) as DIR/<name>.npy "
+                         "(float32); inputs are seeded, so two builds can be compared output for output")
     ap.add_argument("--no-extras", action="store_true",
                     help="skip the extra legs of the default line (cfg4_train / cfg5_fwd sub-results, GPU torch-eager baseline)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3)
+    torch.manual_seed(0)  # the dropout / DropPath draws follow torch's generator: same arguments -> same computation
     wl = WORKLOADS[args.workload]
     cfg = synth.CONFIGS[wl["cfg"]]
     train = wl["mode"] == "train"
 
     if args.impl == "reference":
+        if args.dump_outputs:
+            ap.error("--dump-outputs writes the outputs of the CUDA path; --impl reference only times the CPU arm")
         run_reference_arm(args, wl, cfg)
         return
 
@@ -579,7 +612,7 @@ def main():
         model.eval()
         model.use_cuda_graphs = bool(args.graphs)  # the 41 launches of a forward replayed from one CUDA graph per shape
 
-    # Rotating set of distinct input batches whose total size exceeds the 126 MB L2 (no L2-resident inputs between steps).
+    # Rotating set of distinct input batches whose total size exceeds the 50 MB L2 (no L2-resident inputs between steps).
     per_batch = B * (Lv * cfg["v_feat_dim"] + Lt * cfg["t_feat_dim"] + Lv + Lt) * 4
     n_rot = max(2, int(160e6 // per_batch) + 1)
     host_batches, host_targets = [], []
@@ -599,6 +632,8 @@ def main():
             dist.barrier()
             torch.cuda.synchronize()
 
+    last = {}  # what the most recent step handed back to its caller (--dump-outputs)
+
     def train_step(inputs, targets):
         out = model(**inputs)
         ld = crit(out, targets)
@@ -606,13 +641,16 @@ def main():
         opt.zero_grad(set_to_none=True)
         total.backward()
         opt.step()  # clip_grad_norm_(0.1) (reference --grad_clip 0.1) + AdamW
+        last.update(out=out, losses=ld, total=total)
         return total
 
     def device_step(i):
         if train:
             return train_step(dev_batches[i % n_rot], dev_targets[i % n_rot])
         with torch.no_grad():
-            return model(**dev_batches[i % n_rot])
+            out = model(**dev_batches[i % n_rot])
+        last.update(out=out)
+        return out
 
     # ------------------------------------------------ device-resident timing ------------------------------------------------
     for i in range(args.warmup):
@@ -631,6 +669,8 @@ def main():
     sync_all()
     ms_total = e0.elapsed_time(e1)
     gpu_launches = int(lib.univtg_launch_count()) - launches0  # kernels of THIS library launched inside the timed region
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last)
     # host side of the same loop: how long the CPU needs to ENQUEUE a step (5 steps = ~600 launches stay below the driver's launch
     # queue depth, so the host is not throttled by the GPU here).  enqueue time ~ ms_per_step means the step is host-bound.
     sync_all()
@@ -908,7 +948,7 @@ def main():
                                else "forward (CUDA-graph replay)")),
                 "parallelism": (f"dp{n_gpus}: shard by sample; flat fp32 gradient buffer NCCL all-reduced (AVG) in backward-stage slices on a side stream" if train
                                 else f"replicas x{n_gpus} (shard by sample, no collective)"),
-                "l2_policy": f"{n_rot} rotating input batches ({n_rot * per_batch / 1e6:.0f} MB > 126 MB L2)",
+                "l2_policy": f"{n_rot} rotating input batches ({n_rot * per_batch / 1e6:.0f} MB > 50 MB L2)",
                 "clips_per_s": value * Lv},
             "e2e": {"value": e2e_value, "unit": "pairs/s", "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h,
                     "ms_per_step": ms_e2e / args.steps},
@@ -918,10 +958,11 @@ def main():
             "clocks": clocks,
             "tflops_algorithmic": total_flops / (step_ms * 1e-3) / 1e12,
             "encoder_tflops_pct_of_sustained_peak": 100.0 * enc_flops / (step_ms * 1e-3) / 1e12 / peaks["tflops_sustained"],
-            "roofline": {"kernel": "gemm_tcgen05_kernel", "bound": "tensor", "achieved": achieved_tf,
+            "roofline": {"kernel": "gemm_wgmma_kernel", "bound": "tensor", "achieved": achieved_tf,
                          "peak": peaks["tflops_sustained"], "unit": "TFLOP/s", "frac": achieved_tf / peaks["tflops_sustained"],
                          "traffic": gemm_traffic_bytes(),
-                         "traffic_source": "static: mean DRAM read+write bytes per launch over the 58 GEMM launches of one train step in the committed ncu --set full capture (profiles/gemm_traffic.json), not measured in this run",
+                         "traffic_source": ("static: mean DRAM read+write bytes per launch of an ncu --set full capture (profiles/gemm_traffic.json), "
+                                            "not measured in this run") if gemm_traffic_bytes() is not None else "not measured",
                          "peak_source": peaks["source"] + ", sustained (kernel timed inside a step)",
                          "scope": ("every launch of the kernel in the train step: forward + dgrad + wgrad (CUDA events around each launch)" if train
                                    else "forward launches of the kernel (CUDA events between launches)"),

@@ -1,5 +1,5 @@
 /*
- * univtg_b200 — C ABI of the B200-native UniVTG hot path (cross-modal encoder + heads).
+ * univtg_b200 — C ABI of the H100-native UniVTG hot path (cross-modal encoder + heads).
  *
  * Drop-in boundary: the reference reaches this path through ONE Python plugin call,
  *     importlib.import_module('model.' + opt.model_id).build_model(opt) -> (model, criterion)
@@ -126,7 +126,7 @@ int univtg_droppath_scales(const univtg_rng* rng, int32_t n_sites, int32_t batch
 /* Backward of the last univtg_forward_train on (plan, train_ws).  g_*: upstream gradients of pred_logits [B,Lv,1],
  * pred_spans [B,Lv,2], vid_mem_proj [B,Lv,d], txt_mem_proj [B,1,d] (NULL = zero).  grads: HOST array of device pointers,
  * one ZERO-FILLED fp32 tensor per parameter in univtg_pack_weights order and in the parameter's own layout.
- * grad_scale: power-of-two loss scale S > 0.  Gradient GEMM operands share the plan's 16-bit format (one tcgen05.mma takes
+ * grad_scale: power-of-two loss scale S > 0.  Gradient GEMM operands share the plan's 16-bit format (one wgmma takes
  * A and B in one format); with fp16 operands the intermediate gradients are carried multiplied by S so they do not
  * underflow, and every parameter gradient is multiplied by 1/S where it is written (the results are unscaled).  Use 1 for
  * bf16 plans. */
@@ -171,7 +171,7 @@ int64_t univtg_launch_count(void);
 
 /* Optional per-launch CUDA-event timeline of univtg_forward (bench / profiling only; adds event records to the stream).
  * read_profile returns the number of launches of the last forward and fills ms[i] / kinds[i]
- * (kind 0 = bandwidth-bound row kernel, 1 = tcgen05 GEMM, 2 = attention); it synchronises on the last event. */
+ * (kind 0 = bandwidth-bound row kernel, 1 = tensor-core GEMM, 2 = attention); it synchronises on the last event. */
 int univtg_plan_set_profiling(univtg_plan* plan, int32_t enable);
 int univtg_plan_read_profile(univtg_plan* plan, float* ms, int32_t* kinds, int32_t cap);
 
@@ -184,24 +184,19 @@ int univtg_plan_read_profile(univtg_plan* plan, float* ms, int32_t* kinds, int32
 int univtg_op_gemm(const void* a, const void* b, int32_t M, int32_t N, int32_t K, int32_t a_mn, int32_t b_mn, int32_t fmt,
                    int32_t bn, int32_t ksplit, const float* bias, int32_t act, float alpha, float* out32, void* out16,
                    void* stream);
-/* Same GEMM launched as 2-CTA clusters: vertically adjacent tiles share their B tile through TMA multicast (half the
- * L2 -> SM traffic of B).  bn multiple of 32 (of 128 when b_mn). */
+/* Same GEMM launched as 2-CTA clusters: vertically adjacent tiles share a K-major B tile through TMA multicast (half the
+ * L2 -> SM traffic of B).  bn multiple of 32; b_mn must be 0 (an MN-major B is rejected with an error). */
 int univtg_op_gemm_cluster(const void* a, const void* b, int32_t M, int32_t N, int32_t K, int32_t a_mn, int32_t b_mn,
                            int32_t fmt, int32_t bn, int32_t ksplit, const float* bias, int32_t act, float alpha, float* out32,
                            void* out16, void* stream);
-/* Profiling aid: when `buf` (device, >= 148*8 uint64) is non-NULL every following GEMM launch stamps %globaltimer per CTA:
- * [0] entry, [1] setup done, [2] all TMA issued, [3] first stage landed, [4] last MMA issued, [5] accumulator ready,
+/* Profiling aid: when `buf` (device, >= num_SMs*8 uint64) is non-NULL every following GEMM launch stamps %globaltimer per CTA:
+ * [0] entry, [1] setup done, [2] all TMA issued, [3] first stage landed, [4] last MMA of the first tile retired, [5] unused,
  * [6] epilogue done, [7] exit.  Pass NULL to switch it off. */
 int univtg_debug_gemm_timeline(void* buf);
 /* Host-only: the tile width / split-K factor the GEMM launcher's cost model picks for a grouped launch (num <= 4 problems of
  * M x N with kblocks 64-wide k-blocks each; step 16 for K-major B, 64 for MN-major B).  Testing / tuning aid. */
 int univtg_debug_choose_tile(const int32_t* Ms, const int32_t* Ns, const int32_t* kblocks, int32_t num, int32_t num_sms, int32_t step,
                              int32_t max_split, int32_t* bn, int32_t* ksplit);
-/* tcgen05.ld rate probe with the GEMM epilogue's access pattern: out_ns[block] = ns per 16-column step.  Profiling aid only. */
-int univtg_debug_tmem_ld_rate(int32_t iters, int32_t mode, int32_t blocks, float* out_ns, float* sink, void* stream);
-/* tcgen05.mma issue-rate probe (M=128, N=n, K=16 from resident smem): out_ns[block] = ns per MMA.  Profiling aid only. */
-int univtg_debug_mma_rate(int32_t n, int32_t iters, int32_t per_commit, int32_t kstep_bytes, int32_t blocks, float* out_ns,
-                          void* stream);
 /* Parameter update of the reference's training loop (main/train_vlp_ddp.py:66-68 = main/train_mr.py:64-66; optimizer built at
  * main/config.py:350 as torch.optim.AdamW(lr, weight_decay)) over ONE flat fp32 buffer of n floats (n % 4 == 0, 16-byte
  * aligned; the plugin lays every parameter and its gradient out at the same offsets):
@@ -261,13 +256,13 @@ int univtg_op_layernorm(const float* in, int32_t rows, int32_t d, const float* g
                         int32_t fmt, float* out32, void* out16, int32_t ld16, void* stream);
 /* Attention core.  qkv: [B*L, 3d] 16-bit, column blocks Q | K | V (heads are dh-wide sub-blocks), d = H*dh; scores are
  * scaled by 1/sqrt(dh); key_mask [B,L] f32 (1 = valid key); out [B*L,d] 16-bit; lse [B,H,L] f32 or NULL.
- * impl: 0 = tcgen05 (dh in {64,128}), 1 = SIMT (any dh). */
+ * impl: 0 = tensor cores (wgmma, dh in {64,128}), 1 = SIMT (any dh). */
 int univtg_op_attention(const void* qkv, const float* key_mask, void* out, float* lse, int32_t B, int32_t L, int32_t H,
                         int32_t dh, int32_t fmt, int32_t impl, void* stream);
 
 /* Attention core backward.  qkv as above; dO [B*L,d] 16-bit gradient of `out`; O = forward output (16-bit, fmt_act);
  * (same 16-bit format as qkv); lse from the forward; delta_ws [B,H,L] f32 scratch; dqkv32 [B*L,3d] f32 receives
- * dQ | dK | dV.  impl: 0 tcgen05, 1 SIMT. */
+ * dQ | dK | dV.  impl: 0 tensor cores (wgmma), 1 SIMT. */
 int univtg_op_attention_bwd(const void* qkv, const void* dO, const void* O, const float* key_mask, const float* lse,
                             float* delta_ws, float* dqkv32, int32_t B, int32_t L, int32_t H, int32_t dh, int32_t fmt_act,
                             int32_t impl, void* stream);

@@ -8,11 +8,11 @@ __graft_entry__.smoke() and bench.py's cpu_baseline / --impl reference legs may 
 (univtg_b200/) must never import, call or fall back to anything under oracle/.
 
 Parity pinning: the reference ships no tests or golden vectors for this path (SURVEY.md section 4/8c: "parity unpinned"
-by its own tests).  The oracle is therefore pinned against the LIVE reference (`/root/reference/model/univtg.py`
-imported in the build container) by tests/test_oracle_vs_reference.py, and against the fixtures that
-tests/golden/make_golden.py generated from that live reference (tests/golden/*.npz).
+by its own tests).  The oracle is therefore pinned against outputs of the reference (`model/univtg.py`),
+stored in tests/golden/reference_pins.npz, by tests/test_oracle_vs_reference.py, and against the fixtures that
+tests/golden/make_golden.py generated from the reference (tests/golden/*.npz).
 
-Reference lines each function follows (paths relative to /root/reference):
+Reference lines each function follows (paths relative to the UniVTG repository root):
   layer_norm / linear_layer   model/univtg.py:384-406 (LinearLayer), torch nn.LayerNorm (eps 1e-5, biased variance)
   sine_position               model/position_encoding.py:60-83
   multi_head_attention        torch F.multi_head_attention_forward as called at model/transformer_encoder_droppath.py:118

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""Generate tests/golden/*.npz by running the UNMODIFIED reference (/root/reference/model/univtg.py) on CPU fp32.
+"""Generate tests/golden/*.npz by running the UNMODIFIED reference (model/univtg.py of a showlab/UniVTG checkout) on CPU fp32.
 
-Run in the build container only (the GPU box has no /root/reference):  python tests/golden/make_golden.py
+Usage:  python tests/golden/make_golden.py <path to a showlab/UniVTG checkout>
 Weights and synthetic inputs are regenerated from seeds by univtg_b200.synth, so a fixture stores only the seeds, the
 outputs, the five losses and per-parameter gradient summaries.  cfg1 additionally stores the reference's demo features
 (tmp/vid.npz, tmp/txt.npz) pre-processed as main_gradio.py:58-80 does.
@@ -14,7 +14,8 @@ import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, ROOT)
-sys.path.insert(0, "/root/reference")
+REF = os.path.abspath(sys.argv[1])
+sys.path.insert(0, REF)
 
 from univtg_b200 import synth  # noqa: E402
 from model.univtg import build_model  # noqa: E402  (the reference)
@@ -25,8 +26,8 @@ OUT_KEYS = ("pred_logits", "pred_spans", "saliency_scores", "vid_mem_proj", "txt
 
 def demo_inputs():
     """Reference demo inputs, as main_gradio.load_data prepares them."""
-    vid = np.load("/root/reference/tmp/vid.npz")["features"].astype(np.float32)
-    txt = np.load("/root/reference/tmp/txt.npz")["features"].astype(np.float32)
+    vid = np.load(os.path.join(REF, "tmp", "vid.npz"))["features"].astype(np.float32)
+    txt = np.load(os.path.join(REF, "tmp", "txt.npz"))["features"].astype(np.float32)
     vid = torch.from_numpy(vid)
     txt = torch.from_numpy(txt)
     vid = vid / (vid.norm(dim=-1, keepdim=True) + 1e-5)  # utils/basic_utils.py:97-99

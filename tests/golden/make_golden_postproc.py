@@ -1,13 +1,13 @@
 #!/usr/bin/env python
-"""Writes tests/golden/postproc_nms.json: inputs and outputs of the LIVE reference `utils.temporal_nms.temporal_nms`
-(/root/reference, build container only) on seeded random windows, so the oracle's restatement stays pinned on machines where
-the reference is absent.  Usage: PYTHONPATH=/root/reference python tests/golden/make_golden_postproc.py"""
+"""Writes tests/golden/postproc_nms.json: inputs and outputs of the reference `utils.temporal_nms.temporal_nms` on seeded random
+windows, so the oracle's restatement stays pinned without the reference.
+Usage: python tests/golden/make_golden_postproc.py <path to a showlab/UniVTG checkout>"""
 import json
 import os
 import random
 import sys
 
-sys.path.insert(0, "/root/reference")
+sys.path.insert(0, os.path.abspath(sys.argv[1]))
 from utils.temporal_nms import temporal_nms  # noqa: E402
 
 rng = random.Random(7)

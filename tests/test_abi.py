@@ -51,7 +51,7 @@ def test_tile_cost_model_choices_are_legal_and_sensible():
 
     lib = _lib.load_library()
 
-    def choose(problems, step, max_split, sms=148):
+    def choose(problems, step, max_split, sms=132):
         n = len(problems)
         Ms = (ctypes.c_int32 * n)(*[p[0] for p in problems])
         Ns = (ctypes.c_int32 * n)(*[p[1] for p in problems])
@@ -68,15 +68,15 @@ def test_tile_cost_model_choices_are_legal_and_sensible():
         assert 64 <= bn <= 256 and bn % step == 0
         assert 1 <= ks <= max_split and (ks & (ks - 1)) == 0
         assert ks == 1 or all(ks * 4 <= (p[2] + 63) // 64 for p in problems)
-    # N = 1024 over 27 row tiles: a single round exists (<= 148 tiles) and must be chosen
+    # N = 1024 over 27 row tiles: a single round exists (<= 132 tiles on H100) and must be chosen
     bn, ks = choose([(M, d, d)], 16, 1)
-    assert ((M + 127) // 128) * ((d + bn - 1) // bn) <= 148 and ks == 1
+    assert ((M + 127) // 128) * ((d + bn - 1) // bn) <= 132 and ks == 1
     # weight gradient d x d with K = 3424: 32 output tiles -> split-K so that most SMs work
     bn, ks = choose([(d, d, M)], 64, 16)
-    assert bn == 256 and ks >= 2 and 8 * 4 * ks <= 148
+    assert bn == 256 and ks >= 2 and 8 * 4 * ks <= 132
     # bad arguments are rejected
     z = ctypes.c_int32(0)
-    assert lib.univtg_debug_choose_tile(None, None, None, 1, 148, 16, 1, ctypes.byref(z), ctypes.byref(z)) != 0
+    assert lib.univtg_debug_choose_tile(None, None, None, 1, 132, 16, 1, ctypes.byref(z), ctypes.byref(z)) != 0
 
 
 def test_product_entry_points_fail_loudly_without_cuda():

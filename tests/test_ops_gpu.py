@@ -1,6 +1,6 @@
 """Operator-level parity of the CUDA kernels against plain PyTorch fp32 references of the same op (the correctness cases of
-tools/gpu_selftest.py, run in-process): tcgen05 GEMM (K-/MN-major operands, ragged shapes, split-K, CTA pairs, epilogues),
-LayerNorm rows, attention forward and backward (tcgen05 and SIMT paths; L = 107, 128, 182, 300, 1277)."""
+tools/gpu_selftest.py, run in-process): wgmma GEMM (K-/MN-major operands, ragged shapes, split-K, 2-CTA clusters, epilogues),
+LayerNorm rows, attention forward and backward (wgmma and SIMT paths; L = 107, 128, 182, 300, 1277)."""
 import importlib.util
 import os
 

@@ -1,23 +1,30 @@
-"""Pin the oracle against the LIVE reference (only where /root/reference exists, i.e. the build container)."""
-import sys
+"""Pin the oracle, the decode restatement and the plugin boundary against the original UniVTG code: its outputs for these
+inputs are stored in tests/golden/reference_pins.npz (written by tests/golden/make_golden_pins.py from an unmodified checkout)."""
+import json
+import os
 
+import numpy as np
 import pytest
 import torch
 
-from tests.conftest import REFERENCE, has_reference
+from tests.helpers import GOLDEN
 from univtg_b200 import synth
 
-pytestmark = pytest.mark.skipif(not has_reference(), reason="/root/reference not present on this box")
+_PINS = None
 
 
-def _ref_model(cfg, sd, **over):
-    if REFERENCE not in sys.path:
-        sys.path.insert(0, REFERENCE)
-    from model.univtg import build_model  # the unmodified reference
+def pins():
+    """(arrays, meta): reference outputs by name, and the structured values (losses, key lists, decoded rows)."""
+    global _PINS
+    if _PINS is None:
+        z = dict(np.load(os.path.join(GOLDEN, "reference_pins.npz")))
+        _PINS = ({k: torch.from_numpy(v) for k, v in z.items() if k != "meta"}, json.loads(z["meta"].tobytes().decode()))
+    return _PINS
 
-    model, crit = build_model(synth.reference_args(cfg, **over))
-    model.load_state_dict(sd, strict=True)
-    return model, crit
+
+def _ref_outputs(prefix):
+    arrays, _ = pins()
+    return {k.split("/", 1)[1]: v for k, v in arrays.items() if k.startswith(prefix + "/")}
 
 
 @pytest.mark.parametrize("cfg_name,ragged,batch", [("tiny", True, None), ("tiny", False, 5), ("cfg1", True, 3)])
@@ -26,13 +33,10 @@ def test_forward_and_losses(cfg_name, ragged, batch):
 
     cfg = synth.CONFIGS[cfg_name]
     sd = synth.make_state_dict(cfg, seed=123)
-    model, crit = _ref_model(cfg, sd)
-    model.eval()
     inp = synth.make_inputs(cfg, seed=7, ragged=ragged, batch=batch)
     tgt = synth.make_targets(inp, seed=8)
-    with torch.no_grad():
-        ref = model(**inp)
-        ref_loss = crit(ref, tgt)
+    ref = _ref_outputs(f"fwd_{cfg_name}_{ragged}_{batch}")
+    ref_loss = pins()[1][f"fwd_{cfg_name}_{ragged}_{batch}/losses"]
     out = O.forward(sd, cfg, **inp)
     for k in ("pred_logits", "pred_spans", "saliency_scores", "vid_mem_proj", "txt_mem_proj"):
         torch.testing.assert_close(out[k], ref[k].double(), rtol=2e-5, atol=2e-5)
@@ -48,12 +52,9 @@ def test_bool_masks_of_the_highlight_path_give_the_same_outputs():
 
     cfg = synth.CONFIGS["tiny"]
     sd = synth.make_state_dict(cfg, seed=11)
-    model, _ = _ref_model(cfg, sd)
-    model.eval()
     inp = synth.make_inputs(cfg, seed=3, ragged=True, batch=4)
     as_bool = dict(inp, src_vid_mask=inp["src_vid_mask"].bool(), src_txt_mask=inp["src_txt_mask"].bool())
-    with torch.no_grad():
-        ref_f, ref_b = model(**inp), model(**as_bool)
+    ref_f, ref_b = _ref_outputs("bool_float"), _ref_outputs("bool_bool")
     out = O.forward(sd, cfg, **as_bool)
     for k in ("pred_logits", "pred_spans", "saliency_scores", "vid_mem_proj", "txt_mem_proj"):
         torch.testing.assert_close(ref_b[k], ref_f[k], rtol=0, atol=0)
@@ -67,12 +68,9 @@ def test_droppath_scales_match_reference_train_mode():
 
     cfg = synth.CONFIGS["tiny"]
     sd = synth.make_state_dict(cfg, seed=5)
-    model, _ = _ref_model(cfg, sd, droppath=0.3, input_dropout=0.0)
-    model.train()
     inp = synth.make_inputs(cfg, seed=9, ragged=True, batch=6)
     B = inp["src_vid"].shape[0]
-    torch.manual_seed(77)
-    ref = model(**inp)
+    ref = _ref_outputs("droppath")  # the reference's train-mode output after torch.manual_seed(77)
     torch.manual_seed(77)
     keep = 0.7
     scales = torch.stack([torch.floor(keep + torch.rand((B, 1, 1))).flatten() / keep for _ in range(2 * cfg["enc_layers"])])
@@ -84,9 +82,9 @@ def test_droppath_scales_match_reference_train_mode():
 def test_state_dict_keys_and_shapes_match_reference():
     for name in ("tiny", "cfg1"):
         cfg = synth.CONFIGS[name]
-        model, _ = _ref_model(cfg, synth.make_state_dict(cfg))
-        ref = {k: tuple(v.shape) for k, v in model.state_dict().items()}
+        ref = {k: tuple(v) for k, v in pins()[1][f"state_dict/{name}"]}
         assert list(ref.items()) == list(synth.state_dict_shapes(cfg).items())
+        assert set(synth.make_state_dict(cfg)) == set(ref)
 
 
 def test_input_dropout_masks_match_reference_train_mode():
@@ -98,14 +96,11 @@ def test_input_dropout_masks_match_reference_train_mode():
 
     cfg = synth.CONFIGS["tiny"]
     sd = synth.make_state_dict(cfg, seed=5)
-    model, crit = _ref_model(cfg, sd, droppath=0.0, input_dropout=0.5)
-    model.train()
     inp = synth.make_inputs(cfg, seed=9, ragged=True, batch=6)
     tgt = synth.make_targets(inp, seed=10)
     B, Lv, Lt, d = inp["src_vid"].shape[0], inp["src_vid"].shape[1], inp["src_txt"].shape[1], cfg["hidden_dim"]
-    torch.manual_seed(31)
-    ref = model(**inp)
-    ref_loss = crit(ref, tgt)
+    ref = _ref_outputs("input_dropout")  # the reference's train-mode output after torch.manual_seed(31)
+    ref_loss = pins()[1]["input_dropout/losses"]
     torch.manual_seed(31)
     shapes = [(B, Lv, cfg["v_feat_dim"]), (B, Lv, d), (B, Lt, cfg["t_feat_dim"]), (B, Lt, d)]
     masks = [torch.nn.functional.dropout(torch.ones(s), 0.5, True) for s in shapes]
@@ -123,17 +118,16 @@ def test_hl_loss_list_matches_reference():
     from oracle import univtg_oracle as O
 
     cfg = synth.CONFIGS["tiny"]
+    from univtg_b200 import build_model
+
     sd = synth.make_state_dict(cfg, seed=5)
-    model, crit = _ref_model(cfg, sd, dset_type="hl")
-    assert crit.losses == ["labels", "saliency"]
-    model.eval()
+    assert pins()[1]["hl/crit_losses"] == ["labels", "saliency"]
+    assert build_model(synth.reference_args(cfg, device="cpu", dset_type="hl"))[1].losses == ["labels", "saliency"]
     inp = synth.make_inputs(cfg, seed=9, ragged=True, batch=6)
     full = synth.make_targets(inp, seed=10)
     tgt = {"saliency_scores": full["saliency_scores"], "saliency_pos_labels": full["saliency_pos_labels"],
            "timestamp_mask": full["timestamp_mask"], "timestamp_window": 1 * (full["saliency_scores"] > 0)}
-    with torch.no_grad():
-        ref = model(**inp)
-        ref_loss = crit(ref, tgt)
+    ref_loss = pins()[1]["hl/losses"]
     assert sorted(ref_loss) == ["loss_f", "loss_s_inter", "loss_s_intra"]
     loss = O.criterion(O.forward(sd, cfg, **inp), tgt, losses=("labels", "saliency"))
     assert sorted(loss) == sorted(ref_loss)
@@ -141,40 +135,8 @@ def test_hl_loss_list_matches_reference():
         assert abs(float(loss[k]) - float(v)) < 5e-6 * max(1.0, abs(float(v))), k
 
 
-def _stub_dataset_deps():
-    """main.dataset imports h5py and nncore at module level but the MR evaluation loop never calls into them (SURVEY 8c)."""
-    import types
-
-    if "h5py" not in sys.modules:
-        sys.modules["h5py"] = types.ModuleType("h5py")
-    if "nncore" not in sys.modules:
-        nn_ = types.ModuleType("nncore")
-        ds = types.ModuleType("nncore.dataset")
-
-        class _Registry:
-            def register(self, *a, **k):
-                return lambda c: c
-
-        ds.DATASETS = _Registry()
-        par = types.ModuleType("nncore.parallel")
-        par.DataContainer = object
-        nn_.dataset, nn_.parallel = ds, par
-        sys.modules.update({"nncore": nn_, "nncore.dataset": ds, "nncore.parallel": par})
-    if REFERENCE not in sys.path:
-        sys.path.insert(0, REFERENCE)
-
-
-@pytest.mark.parametrize("sort", [True, False])
-def test_decode_restatement_matches_compute_mr_results(sort):
-    """Pins oracle/postproc_oracle.decode_mr + saliency_lists to the reference's own evaluation loop: compute_mr_results
-    (main/inference_mr.py:86-193) is executed here with a stub model / loader that replay fixed outputs."""
-    from argparse import Namespace
-
-    from oracle import postproc_oracle as PO
-
-    _stub_dataset_deps()
-    import main.inference_mr as M
-
+def decode_case():
+    """Fixed model outputs replayed through the evaluation loop: (outputs, timestamps, video mask, durations, B, Lt)."""
     g = torch.Generator().manual_seed(1234)
     B, Lv, Lt = 5, 23, 7
     lens = [23, 9, 17, 1, 12]
@@ -189,71 +151,38 @@ def test_decode_restatement_matches_compute_mr_results(sort):
     ts = ((torch.arange(Lv, dtype=torch.float32) + 0.5) / Lv)[None, :, None].expand(B, Lv, 2).contiguous()
     durs = [150.0, 33.3, 126.0, 2.0, 150.0]
     outputs = {"pred_logits": pred_logits, "pred_spans": pred_spans, "saliency_scores": sal}
+    return outputs, ts, vmask, durs, B, Lt
 
-    class FakeModel:
-        def eval(self):
-            return self
 
-        def __call__(self, **kw):
-            return {k: v.clone() for k, v in outputs.items()}
+@pytest.mark.parametrize("sort", [True, False])
+def test_decode_restatement_matches_compute_mr_results(sort):
+    """Pins oracle/postproc_oracle.decode_mr + saliency_lists to the reference's own evaluation loop: what compute_mr_results
+    (main/inference_mr.py:86-193) returned when a stub model / loader replayed these outputs."""
+    from oracle import postproc_oracle as PO
 
-    meta = [{"qid": i, "query": "q", "vid": "v", "duration": durs[i]} for i in range(B)]
-    batch = {"query_feat": (torch.zeros(B, Lt, 4), torch.ones(B, Lt)), "video_feat": (torch.zeros(B, Lv, 4), vmask),
-             "timestamp": (ts, vmask), "timestamp_window": (torch.zeros(B, Lv),), "span_labels_nn": (torch.zeros(B, Lv, 2),)}
-    opt = Namespace(device="cpu", pin_memory=False, span_loss_type="l1", model_id="univtg", eval_mode=None,
-                    no_sort_results=not sort, debug=False, round_multiple=0, clip_length=2)
-    res, _ = M.compute_mr_results(FakeModel(), [(meta, batch)], opt)
-    rows = PO.decode_mr(pred_logits, pred_spans, ts, vmask, durs, sort=sort)
-    sal_lists = PO.saliency_lists(sal, vmask)
+    outputs, ts, vmask, durs, B, _ = decode_case()
+    res = pins()[1][f"decode/{sort}"]
+    rows = PO.decode_mr(outputs["pred_logits"], outputs["pred_spans"], ts, vmask, durs, sort=sort)
+    sal_lists = PO.saliency_lists(outputs["saliency_scores"], vmask)
     assert len(res) == B
     for b in range(B):
-        assert res[b]["pred_relevant_windows"] == rows[b], b
-        assert res[b]["pred_saliency_scores"] == sal_lists[b], b
+        assert [list(r) for r in rows[b]] == res[b]["pred_relevant_windows"], b
+        assert list(sal_lists[b]) == res[b]["pred_saliency_scores"], b
 
 
-def test_reference_setup_model_builds_the_plugin(tmp_path):
+def test_plugin_matches_what_reference_setup_model_builds():
     """Boundary (SURVEY 8b): main.config.setup_model does importlib.import_module('model.' + opt.model_id).build_model(opt)
-    (main/config.py:341-342).  With the one-line shim of INTEGRATION.md on sys.path as model/univtg_b200.py the reference's own
-    factory builds (model, criterion, optimizer, lr_scheduler); AdamW sees the same parameter names / order / shapes as for
-    --model_id univtg, and a checkpoint saved from the reference model loads strict=True after `module.` stripping."""
-    import importlib
+    (main/config.py:341-342) and builds AdamW over every trainable parameter, the WarmupStepLR scheduler and the criterion.
+    The plugin built from the same args exposes the same parameter names / order / shapes, so the optimizer and scheduler the
+    reference builds around it are the ones it built for --model_id univtg."""
+    from univtg_b200 import build_model
 
-    _stub_dataset_deps()
-    # the reference's `model` is a namespace package (no __init__.py): a second model/ directory on sys.path joins it, which is
-    # how the one-file shim is tried out without touching /root/reference (a maintainer drops the file into model/ instead)
-    shim = tmp_path / "model"
-    shim.mkdir()
-    (shim / "univtg_b200.py").write_text("from univtg_b200.plugin import build_model  # noqa: F401\n")
-    sys.path.append(str(tmp_path))
-    importlib.invalidate_caches()
-    try:
-        cfgmod = importlib.import_module("main.config")
-        cfg = synth.CONFIGS["tiny"]
-        class _CpuDevice(str):  # the reference reads opt.device both as torch.device(opt.device) (model/univtg.py:410) and as
-            def __int__(self):  # int(opt.device) >= 0 (main/config.py:344; the CLI passes 0 = cuda, which this box lacks)
-                return -1
-
-        extra = dict(device=_CpuDevice("cpu"), gpu_id=0, lr=1e-4, wd=1e-4, lr_warmup=[10], lr_drop=400, lr_gamma=0.1, resume=None, resume_all=False)
-        built = {}
-        for mid in ("univtg", "univtg_b200"):
-            opt = synth.reference_args(cfg, model_id=mid, **extra)
-            torch.manual_seed(0)
-            built[mid] = cfgmod.setup_model(opt)
-        (m_ref, c_ref, o_ref, s_ref), (m_new, c_new, o_new, s_new) = built["univtg"], built["univtg_b200"]
-        assert type(m_new).__module__ == "univtg_b200.plugin"
-        assert type(s_new).__name__ == type(s_ref).__name__ == "WarmupStepLR"
-        names_ref = [(n, tuple(p.shape)) for n, p in m_ref.named_parameters() if p.requires_grad]
-        names_new = [(n, tuple(p.shape)) for n, p in m_new.named_parameters() if p.requires_grad]
-        assert names_ref == names_new
-        assert [tuple(p.shape) for p in o_ref.param_groups[0]["params"]] == [tuple(p.shape) for p in o_new.param_groups[0]["params"]]
-        assert c_new.weight_dict == c_ref.weight_dict and c_new.losses == c_ref.losses
-        # checkpoint written by the reference training loop (DDP prefixes every key with 'module.', train_vlp_ddp.py:157-164)
-        ckpt = tmp_path / "ckpt.pt"
-        torch.save({"model": {"module." + k: v for k, v in m_ref.state_dict().items()}, "epoch": 3}, ckpt)
-        opt = synth.reference_args(cfg, model_id="univtg_b200", **dict(extra, resume=str(ckpt)))
-        m_loaded = cfgmod.setup_model(opt)[0]
-        for (k1, v1), (k2, v2) in zip(m_ref.state_dict().items(), m_loaded.state_dict().items()):
-            assert k1 == k2 and torch.equal(v1, v2)
-    finally:
-        sys.path.remove(str(tmp_path))
-        sys.modules.pop("model.univtg_b200", None)
+    ref = pins()[1]["setup_model"]
+    cfg = synth.CONFIGS["tiny"]
+    torch.manual_seed(0)
+    model, crit = build_model(synth.reference_args(cfg, device="cpu", model_id="univtg_b200"))
+    names = [[n, list(p.shape)] for n, p in model.named_parameters() if p.requires_grad]
+    assert names == ref["named_parameters"]
+    assert [s for _, s in names] == ref["optimizer_shapes"]
+    assert ref["optimizer"] == "AdamW" and ref["scheduler"] == "WarmupStepLR"
+    assert {k: float(v) for k, v in crit.weight_dict.items()} == ref["weight_dict"] and list(crit.losses) == ref["losses"]

@@ -7,7 +7,6 @@ import sys
 import pytest
 import torch
 
-from tests.conftest import REFERENCE, has_reference
 from tests.helpers import GOLDEN
 
 
@@ -27,23 +26,24 @@ def test_oracle_nms_matches_reference_fixtures():
         assert got == c["expected"], (c["nms_thd"], c["max_after_nms"], len(c["rows"]))
 
 
-@pytest.mark.skipif(not has_reference(), reason="/root/reference not present on this box")
 def test_oracle_nms_matches_live_reference_random():
-    if REFERENCE not in sys.path:
-        sys.path.insert(0, REFERENCE)
-    from utils.temporal_nms import temporal_nms as ref_nms
-
+    """300 seeded random window sets through the reference utils.temporal_nms.temporal_nms (stored in
+    tests/golden/reference_pins.npz by tests/golden/make_golden_pins.py)."""
     from oracle import postproc_oracle as P
+    from tests.test_oracle_vs_reference import pins
 
+    cases = pins()[1]["nms_random"]
     rng = random.Random(3)
-    for _ in range(300):
+    assert len(cases) == 300
+    for c in cases:
         n = rng.choice([0, 1, 2, 5, 10, 40])
         rows = []
         for _ in range(n):
             st = round(rng.uniform(0, 100), 4)
             rows.append([st, round(st + rng.choice([0.0, rng.uniform(0, 50)]), 4), round(rng.choice([0.0, rng.random()]), 4)])
         thd, ma = rng.choice([0.1, 0.5, 0.7, 0.9]), rng.choice([1, 3, 10, 100])
-        assert P.temporal_nms([list(r) for r in rows], thd, ma) == ref_nms([list(r) for r in rows], thd, ma)
+        assert (rows, thd, ma) == (c["rows"], c["nms_thd"], c["max_after_nms"])
+        assert [list(r) for r in P.temporal_nms([list(r) for r in rows], thd, ma)] == c["expected"]
 
 
 def _random_batch(B, Lv, seed, ties=True):

@@ -8,7 +8,7 @@ from univtg_b200 import build_model, synth
 
 pytestmark = pytest.mark.gpu
 WD = {"loss_b": 10.0, "loss_g": 1.0, "loss_f": 10.0, "loss_s_intra": 0.1, "loss_s_inter": 0.1}
-CFG = dict(synth.CONFIGS["tiny"], nheads=2)  # d = 256, dh = 128: tcgen05 attention, oracle finishes in well under a second
+CFG = dict(synth.CONFIGS["tiny"], nheads=2)  # d = 256, dh = 128: wgmma attention, oracle finishes in well under a second
 
 
 def _model(**over):

@@ -1,4 +1,4 @@
-"""univtg_b200 - B200-native (sm_100a) implementation of the UniVTG cross-modal encoder + heads hot path.
+"""univtg_b200 - H100-native (sm_90a) implementation of the UniVTG cross-modal encoder + heads hot path.
 
 Public surface mirrors the reference plugin boundary (reference main/config.py:341-342, model/univtg.py:409-450):
 

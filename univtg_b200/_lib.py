@@ -92,8 +92,6 @@ SIGNATURES = {
                                        c_float, c_void_p, c_void_p, c_void_p]),
     "univtg_debug_gemm_timeline": (c_int, [c_void_p]),
     "univtg_debug_choose_tile": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
-    "univtg_debug_tmem_ld_rate": (c_int, [c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
-    "univtg_debug_mma_rate": (c_int, [c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     "univtg_op_layernorm": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_float, c_int, c_void_p, c_void_p, c_int,
                                     c_void_p]),
     "univtg_op_attention": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int,
@@ -109,7 +107,7 @@ def load_library():
         return _lib
     if not os.path.exists(LIB_PATH):
         raise RuntimeError(
-            f"{LIB_PATH} not found: build it with `python __graft_entry__.py` (nvcc, sm_100a). "
+            f"{LIB_PATH} not found: build it with `python __graft_entry__.py` (nvcc, sm_90a). "
             "univtg_b200 has no CPU or PyTorch fallback.")
     lib = ctypes.CDLL(LIB_PATH)
     for name, (res, args) in SIGNATURES.items():

@@ -228,7 +228,7 @@ int univtg_plan_create(const univtg_config* cfg, const univtg_shape* shape, cons
   int dev = 0;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&P->num_sms, cudaDevAttrMultiProcessorCount, dev);
-  if (P->num_sms <= 0) P->num_sms = 148;
+  if (P->num_sms <= 0) P->num_sms = 132;
   const int d = cfg->hidden_dim, ff = cfg->dim_feedforward;
   P->B = shape->batch;
   P->Lv = shape->l_vid;
@@ -675,6 +675,10 @@ static int op_gemm_impl(const void* a, const void* b, int32_t M, int32_t N, int3
     set_error("univtg_op_gemm: bad argument");
     return 1;
   }
+  if (cluster == 2 && b_mn) {
+    set_error("univtg_op_gemm_cluster: cluster launches need a K-major B operand (b_mn = 0)");
+    return 1;
+  }
   GemmGroup g;
   memset(&g, 0, sizeof(g));
   g.num = 1;
@@ -699,7 +703,7 @@ static int op_gemm_impl(const void* a, const void* b, int32_t M, int32_t N, int3
     rc |= make_tmap_2d(&p.tm_b, b, (uint64_t)N, (uint64_t)K, (uint64_t)K, (uint32_t)(cluster == 2 ? bn / 2 : bn), 64);
     p.b_box_rows = cluster == 2 ? bn / 2 : bn;
   } else {
-    rc |= make_tmap_b_mn(p, b, (uint64_t)K, (uint64_t)N, (uint64_t)N, bn, cluster != 2);
+    rc |= make_tmap_b_mn(p, b, (uint64_t)K, (uint64_t)N, (uint64_t)N, bn);
     p.cb = OperandCoord{0, 1, 0, 0, 0, 0, 0, 1};
   }
   if (rc) return rc;
@@ -710,7 +714,7 @@ static int op_gemm_impl(const void* a, const void* b, int32_t M, int32_t N, int3
   p.ld32 = N;
   p.out16 = reinterpret_cast<uint16_t*>(out16);
   p.ld16 = N;
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 0;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   return launch_gemm_group(g, bn, sms, (cudaStream_t)stream);
@@ -726,17 +730,6 @@ int univtg_op_gemm_cluster(const void* a, const void* b, int32_t M, int32_t N, i
                            int32_t fmt, int32_t bn, int32_t ksplit, const float* bias, int32_t act, float alpha, float* out32,
                            void* out16, void* stream) {
   return op_gemm_impl(a, b, M, N, K, a_mn, b_mn, fmt, bn, ksplit, bias, act, alpha, out32, out16, 2, stream);
-}
-
-int univtg_debug_mma_rate(int32_t n, int32_t iters, int32_t per_commit, int32_t kstep_bytes, int32_t blocks, float* out_ns,
-                          void* stream) {
-  // kstep_bytes: bit 30 selects an MN-major A operand, bit 29 an MN-major B operand (probe-only encoding)
-  return uv::debug_mma_rate(n, iters, per_commit, kstep_bytes & 0xffff, blocks, out_ns, reinterpret_cast<cudaStream_t>(stream),
-                            (kstep_bytes >> 30) & 1, (kstep_bytes >> 29) & 1);
-}
-
-int univtg_debug_tmem_ld_rate(int32_t iters, int32_t mode, int32_t blocks, float* out_ns, float* sink, void* stream) {
-  return uv::debug_tmem_ld_rate(iters, mode, blocks, out_ns, sink, reinterpret_cast<cudaStream_t>(stream));
 }
 
 int univtg_debug_choose_tile(const int32_t* Ms, const int32_t* Ns, const int32_t* kblocks, int32_t num, int32_t num_sms, int32_t step,

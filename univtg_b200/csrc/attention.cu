@@ -2,218 +2,190 @@
 // call site model/transformer_encoder_droppath.py:118):
 //     S = (Q K^T) / sqrt(dh) + key-padding(-inf);  P = softmax_j(S);  O = P V
 // Q, K, V are the three d-wide column blocks of one [B*L, 3d] 16-bit matrix written by the in-projection GEMM.
-// Flash-style: S and P never touch HBM.  tcgen05 path (dh in {64,128}):
-//   CTA = one (batch, head, 128-query tile); loop over 128-key tiles with online softmax.
-//   warp 0 lane 0 : TMA producer + tcgen05.mma issuer (S = Q K^T into TMEM cols [0,128); O_j = P V into [128,128+dh))
-//   warps 1..4    : softmax (thread = query row): tcgen05.ld S -> mask/max/exp2 -> P (16-bit) into the 128B-swizzled
-//                   K-major smem tile that K occupied -> tcgen05.ld O_j -> rescale-accumulate in registers -> store.
+// Flash-style: S and P never touch HBM.  wgmma path (dh in {64,128}):
+//   CTA = one (batch, head, 128-query tile), two warpgroups of 64 query rows each; loop over 128-key tiles (K / V double-buffered
+//   through TMA) with online softmax:
+//     S  = Q K^T : wgmma m64n128, A = Q and B = K from 128B-swizzled K-major smem tiles, fp32 accumulators in registers
+//     P  = exp2(scaled S - running max), converted in registers to 16-bit wgmma A fragments (the m64n128 accumulator layout
+//          is the A-fragment layout of the next product, so P never leaves the registers)
+//     O  = alpha O + P V : wgmma m64 x dh, A = P (registers), B = V (MN-major smem tile, dh contiguous)
 // A SIMT kernel covers other head sizes (e.g. dh = 32 of the d=256 demo config).
 #include <math.h>
 
 #include "kernels.h"
 #include "ptx.cuh"
 #include "rowops.h"
+#include "wgmma.cuh"
 
 namespace uv {
 
 template <int DH>
 struct AttnCfg {
   static constexpr int kQBytes = 128 * DH * 2;   // DH/64 boxes of [128 rows x 64]
-  static constexpr int kKBytes = 128 * DH * 2;   // K tile; re-used for P: 2 boxes of [128 rows x 64] = 32 KB
-  static constexpr int kKPBytes = (kKBytes > 32768) ? kKBytes : 32768;
-  static constexpr int kVBytes = 128 * DH * 2;   // DH/64 boxes of [128 kv rows x 64]: MN-major B operand of P V
-  static constexpr int kSmemBytes = 1024 + kQBytes + kKPBytes + kVBytes + 128 * 4 + 128;
-  static constexpr uint32_t kTmemCols = 256;     // S: 128 cols, O: DH cols
+  static constexpr int kKVBytes = 128 * DH * 2;  // one K or V tile, same boxes
+  static constexpr int kSmemBytes = 1024 + kQBytes + 4 * kKVBytes + 2 * 128 * 4 + 64;
 };
 
-template <int DH>
-__global__ void __launch_bounds__(160, 2) attention_tcgen05_kernel(const __grid_constant__ AttnArgs a) {
+__device__ __forceinline__ float quad_max(float v) {
+  v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1));
+  return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 2));
+}
+__device__ __forceinline__ float quad_sum(float v) {
+  v += __shfl_xor_sync(0xffffffffu, v, 1);
+  return v + __shfl_xor_sync(0xffffffffu, v, 2);
+}
+
+template <int DH, int BF>
+__global__ void __launch_bounds__(256, 1) attention_wgmma_kernel(const __grid_constant__ AttnArgs a) {
   using Cfg = AttnCfg<DH>;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw_addr = smem_u32(smem_raw);
   uint8_t* smem = smem_raw + ((1024u - (raw_addr & 1023u)) & 1023u);
   uint8_t* sQ = smem;
-  uint8_t* sKP = sQ + Cfg::kQBytes;
-  uint8_t* sV = sKP + Cfg::kKPBytes;
-  float* s_bias = reinterpret_cast<float*>(sV + Cfg::kVBytes);  // [128] 0 or -inf per key of the current tile
-  uint64_t* bars = reinterpret_cast<uint64_t*>(s_bias + 128);
+  uint8_t* sK = sQ + Cfg::kQBytes;          // [2] K tiles
+  uint8_t* sV = sK + 2 * Cfg::kKVBytes;     // [2] V tiles
+  float* s_bias = reinterpret_cast<float*>(sV + 2 * Cfg::kKVBytes);  // [2][128] 0 or -inf per key of the tile
+  uint64_t* bars = reinterpret_cast<uint64_t*>(s_bias + 2 * 128);
   uint64_t* q_full = bars + 0;
-  uint64_t* k_full = bars + 1;
-  uint64_t* v_full = bars + 2;
-  uint64_t* s_full = bars + 3;
-  uint64_t* p_full = bars + 4;
-  uint64_t* o_full = bars + 5;
-  uint32_t* tmem_holder = reinterpret_cast<uint32_t*>(bars + 6);
+  uint64_t* kv_full = bars + 1;  // [2]
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7;               // query rows [64 wg, 64 wg + 64) of the tile
+  const int tid = threadIdx.x & 127;
+  const int fr = 16 * (tid >> 5) + (lane >> 2);  // accumulator rows fr, fr + 8; columns 8 i + fc, + 1
+  const int fc = 2 * (lane & 3);
   const int q0 = blockIdx.x * 128;
   const int h = blockIdx.y;
   const int b = blockIdx.z;
   const int L = a.L;
   const int num_kv = (L + 127) / 128;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&a.tm_qkv);
     mbar_init(q_full, 1);
-    mbar_init(k_full, 1);
-    mbar_init(v_full, 1);
-    mbar_init(s_full, 1);
-    mbar_init(p_full, 4);
-    mbar_init(o_full, 1);
+    mbar_init(&kv_full[0], 1);
+    mbar_init(&kv_full[1], 1);
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc<Cfg::kTmemCols>(tmem_holder);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  // Only now (this CTA owns its TMEM columns) may the next grid be scheduled: a dependent CTA that grabbed TMEM first and
-  // then blocked in griddepcontrol.wait could starve a CTA of this grid sharing its SM.
   pdl_launch_dependents();
-  pdl_wait();  // barriers + TMEM are set up; from here on the kernel reads what the previous kernels wrote
-  const uint32_t tmem_base = *tmem_holder;
-  const uint32_t tmem_s = tmem_base;
-  const uint32_t tmem_o = tmem_base + 128;
+  pdl_wait();  // barriers are set up; from here on the kernel reads what the previous kernels wrote
 
-  if (warp == 0) {
-    if (lane == 0) {
-      const uint32_t idesc_s = make_idesc_f16(128, 128, a.fmt, 0, 0);
-      const uint32_t idesc_o = make_idesc_f16(128, DH, a.fmt, 0, 1);  // B = V is MN-major (dh contiguous)
-      mbar_arrive_expect_tx(q_full, Cfg::kQBytes);
+  auto load_kv = [&](int j) {
+    const int s = j & 1;
+    mbar_arrive_expect_tx(&kv_full[s], 2 * Cfg::kKVBytes);
 #pragma unroll
-      for (int kb = 0; kb < DH / 64; ++kb) tma_load_2d(sQ + kb * 16384, &a.tm_qkv, q_full, h * DH + kb * 64, b * L + q0);
-      for (int j = 0; j < num_kv; ++j) {
-        const uint32_t ph = j & 1;
-        if (j > 0) mbar_wait(o_full, ph ^ 1);  // previous PV retired: K/P and V buffers are free
-        mbar_arrive_expect_tx(k_full, Cfg::kKBytes);
-#pragma unroll
-        for (int kb = 0; kb < DH / 64; ++kb)
-          tma_load_2d(sKP + kb * 16384, &a.tm_qkv, k_full, a.d + h * DH + kb * 64, b * L + j * 128);
-        mbar_arrive_expect_tx(v_full, Cfg::kVBytes);
-#pragma unroll
-        for (int vb = 0; vb < DH / 64; ++vb)
-          tma_load_2d(sV + vb * 16384, &a.tm_qkv, v_full, 2 * a.d + h * DH + vb * 64, b * L + j * 128);
-        if (j == 0) mbar_wait(q_full, 0);
-        mbar_wait(k_full, ph);
-        tc_fence_after();
-#pragma unroll
-        for (int ks = 0; ks < DH / 16; ++ks) {
-          const uint32_t off = (ks / 4) * 16384 + (ks % 4) * 32;
-          umma_f16_ss(tmem_s, make_smem_desc_sw128(smem_u32(sQ) + off, 16, 1024),
-                      make_smem_desc_sw128(smem_u32(sKP) + off, 16, 1024), idesc_s, ks > 0 ? 1u : 0u);
-        }
-        umma_commit(s_full);
-        mbar_wait(p_full, ph);
-        mbar_wait(v_full, ph);
-        tc_fence_after();
-#pragma unroll
-        for (int ks = 0; ks < 8; ++ks) {
-          const uint32_t offp = (ks / 4) * 16384 + (ks % 4) * 32;
-          // V tile: 64-wide dh blocks of [128 kv rows x 128 B]; 16 kv rows = two 1024 B swizzle atoms
-          umma_f16_ss(tmem_o, make_smem_desc_sw128(smem_u32(sKP) + offp, 16, 1024),
-                      make_smem_desc_sw128(smem_u32(sV) + ks * 2048, 16384, 1024), idesc_o, ks > 0 ? 1u : 0u);
-        }
-        umma_commit(o_full);
-      }
+    for (int kb = 0; kb < DH / 64; ++kb) {
+      tma_load_2d(sK + s * Cfg::kKVBytes + kb * 16384, &a.tm_qkv, &kv_full[s], a.d + h * DH + kb * 64, b * L + j * 128);
+      tma_load_2d(sV + s * Cfg::kKVBytes + kb * 16384, &a.tm_qkv, &kv_full[s], 2 * a.d + h * DH + kb * 64, b * L + j * 128);
     }
-  } else {
-    // ======================================= softmax warps =======================================
-    const int wq = warp & 3;            // TMEM lane quarter
-    const int row = wq * 32 + lane;     // query row inside the tile
-    const int tid = threadIdx.x - 32;   // 0..127
-    const uint32_t lane_addr = (uint32_t)(wq * 32) << 16;
-    const float kLog2e = 1.4426950408889634f * a.scale;  // scores are scaled by 1/sqrt(dh) inside the exponent
-    float m_run = -INFINITY, l_run = 0.f;
-    float acc[DH];
+  };
+  if (threadIdx.x == 0) {
+    mbar_arrive_expect_tx(q_full, Cfg::kQBytes);
 #pragma unroll
-    for (int c = 0; c < DH; ++c) acc[c] = 0.f;
-
-    for (int j = 0; j < num_kv; ++j) {
-      const uint32_t ph = j & 1;
-      {
-        const int key = j * 128 + tid;
-        float bias = -INFINITY;
-        if (key < L && a.key_mask[(size_t)b * L + key] != 0.f) bias = 0.f;
-        s_bias[tid] = bias;
-      }
-      asm volatile("bar.sync 1, 128;" ::: "memory");  // softmax warps only
-      mbar_wait(s_full, ph);
-      tc_fence_after();
-      // pass A: row max
-      float mx = -INFINITY;
-#pragma unroll
-      for (int c = 0; c < 4; ++c) {
-        uint32_t r[32];
-        tmem_ld_32x32b_x32(tmem_s + lane_addr + c * 32, r);
-        tmem_ld_wait();
-#pragma unroll
-        for (int i = 0; i < 32; ++i) mx = fmaxf(mx, __uint_as_float(r[i]) * kLog2e + s_bias[c * 32 + i]);
-      }
-      const float m_new = fmaxf(m_run, mx);  // running max of scaled scores in log2 units
-      const float m_use = (m_new == -INFINITY) ? 0.f : m_new;
-      const float alpha = exp2f(m_run - m_use);  // m_run = -inf -> 0
-      // pass B: probabilities -> 16-bit P tile (A operand of the PV product), K-major SW128
-      float psum = 0.f;
-#pragma unroll
-      for (int c = 0; c < 4; ++c) {
-        uint32_t r[32];
-        tmem_ld_32x32b_x32(tmem_s + lane_addr + c * 32, r);
-        tmem_ld_wait();
-        uint32_t pk[16];
-#pragma unroll
-        for (int i = 0; i < 32; i += 2) {
-          const float p0 = exp2f(__uint_as_float(r[i]) * kLog2e + s_bias[c * 32 + i] - m_use);
-          const float p1 = exp2f(__uint_as_float(r[i + 1]) * kLog2e + s_bias[c * 32 + i + 1] - m_use);
-          psum += p0 + p1;
-          pk[i / 2] = cvt16x2(p0, p1, a.fmt);
-        }
-        // keys c*32 .. c*32+31 -> box (c/2), 16-byte chunks ((c%2)*4 + q), q = 0..3, XOR-swizzled with row%8
-        uint8_t* rowp = sKP + (c / 2) * 16384 + row * 128;
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          const int chunk = ((c & 1) * 4 + q) ^ (row & 7);
-          *reinterpret_cast<uint4*>(rowp + chunk * 16) = make_uint4(pk[q * 4], pk[q * 4 + 1], pk[q * 4 + 2], pk[q * 4 + 3]);
-        }
-      }
-      l_run = l_run * alpha + psum;
-      m_run = m_new;
-      fence_proxy_async_smem();  // generic-proxy smem writes -> visible to the tensor core (async proxy)
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(p_full);
-      // O_j
-      mbar_wait(o_full, ph);
-      tc_fence_after();
-#pragma unroll
-      for (int c = 0; c < DH / 32; ++c) {
-        uint32_t r[32];
-        tmem_ld_32x32b_x32(tmem_o + lane_addr + c * 32, r);
-        tmem_ld_wait();
-#pragma unroll
-        for (int i = 0; i < 32; ++i) acc[c * 32 + i] = acc[c * 32 + i] * alpha + __uint_as_float(r[i]);
-      }
-      tc_fence_before();
-    }
-    const int qi = q0 + row;
-    if (qi < L) {
-      const float inv = 1.f / l_run;
-      uint16_t* dst = a.out + ((size_t)b * L + qi) * a.d + h * DH;
-#pragma unroll
-      for (int c = 0; c < DH; c += 8) {
-        uint4 v;
-        v.x = cvt16x2(acc[c] * inv, acc[c + 1] * inv, a.fmt);
-        v.y = cvt16x2(acc[c + 2] * inv, acc[c + 3] * inv, a.fmt);
-        v.z = cvt16x2(acc[c + 4] * inv, acc[c + 5] * inv, a.fmt);
-        v.w = cvt16x2(acc[c + 6] * inv, acc[c + 7] * inv, a.fmt);
-        *reinterpret_cast<uint4*>(dst + c) = v;
-      }
-      if (a.lse) a.lse[((size_t)b * a.H + h) * L + qi] = m_run * 0.6931471805599453f + logf(l_run);
-    }
+    for (int kb = 0; kb < DH / 64; ++kb) tma_load_2d(sQ + kb * 16384, &a.tm_qkv, q_full, h * DH + kb * 64, b * L + q0);
+    load_kv(0);
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc<Cfg::kTmemCols>(tmem_base);
+
+  const float kLog2e = 1.4426950408889634f * a.scale;  // scores are scaled by 1/sqrt(dh) inside the exponent
+  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};  // l_run: this thread's columns only (quad-summed at the end)
+  float o[DH / 2];
+#pragma unroll
+  for (int i = 0; i < DH / 2; ++i) o[i] = 0.f;
+
+  for (int j = 0; j < num_kv; ++j) {
+    const int s = j & 1;
+    __syncthreads();  // every wgmma of tile j-1 has retired: its K / V buffers and bias row may be overwritten
+    if (threadIdx.x == 0 && j + 1 < num_kv) load_kv(j + 1);
+    if (threadIdx.x < 128) {
+      const int key = j * 128 + threadIdx.x;
+      s_bias[s * 128 + threadIdx.x] = (key < L && a.key_mask[(size_t)b * L + key] != 0.f) ? 0.f : -INFINITY;
+    }
+    __syncthreads();
+    if (j == 0) mbar_wait(q_full, 0);
+    mbar_wait(&kv_full[s], (j >> 1) & 1);
+    const uint32_t kbase = smem_u32(sK + s * Cfg::kKVBytes), vbase = smem_u32(sV + s * Cfg::kKVBytes);
+
+    float sacc[64];
+    wgmma_fence();
+#pragma unroll
+    for (int ks = 0; ks < DH / 16; ++ks) {
+      const uint32_t off = (ks / 4) * 16384 + (ks % 4) * 32;
+      WG<128, BF>::template ss<0, 0>(sacc, make_smem_desc_sw128(smem_u32(sQ) + wg * 8192 + off, 16, 1024),
+                                     make_smem_desc_sw128(kbase + off, 16, 1024), ks > 0 ? 1u : 0u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+#pragma unroll
+    for (int i = 0; i < 64; ++i) reg_fence(sacc[i]);
+
+    // online softmax over this tile's 128 keys (log2 units)
+    const float* bias = s_bias + s * 128;
+    float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+    for (int i = 0; i < 16; ++i) {
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const float x = sacc[4 * i + e] * kLog2e + bias[8 * i + fc + (e & 1)];
+        sacc[4 * i + e] = x;
+        mx[e >> 1] = fmaxf(mx[e >> 1], x);
+      }
+    }
+    float alpha[2], m_use[2];
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      const float m_new = fmaxf(m_run[r], quad_max(mx[r]));
+      m_use[r] = (m_new == -INFINITY) ? 0.f : m_new;
+      alpha[r] = exp2f(m_run[r] - m_use[r]);  // m_run = -inf -> 0
+      m_run[r] = m_new;
+    }
+    float psum[2] = {0.f, 0.f};
+    uint32_t pf[8][4];  // P as wgmma A fragments: k-chunk kc = keys [16 kc, 16 kc + 16)
+#pragma unroll
+    for (int kc = 0; kc < 8; ++kc) {
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {
+        const int r = q & 1;  // fragment register q: row fr (+8 for odd q), keys 16 kc + 8 (q >> 1) + fc, + 1
+        const float p0 = exp2f(sacc[8 * kc + 2 * q] - m_use[r]);
+        const float p1 = exp2f(sacc[8 * kc + 2 * q + 1] - m_use[r]);
+        psum[r] += p0 + p1;
+        pf[kc][q] = cvt16x2(p0, p1, BF);
+      }
+    }
+#pragma unroll
+    for (int r = 0; r < 2; ++r) l_run[r] = l_run[r] * alpha[r] + psum[r];
+#pragma unroll
+    for (int i = 0; i < DH / 8; ++i) {
+      o[4 * i] *= alpha[0];
+      o[4 * i + 1] *= alpha[0];
+      o[4 * i + 2] *= alpha[1];
+      o[4 * i + 3] *= alpha[1];
+    }
+    wgmma_fence();
+#pragma unroll
+    for (int kc = 0; kc < 8; ++kc)  // V tile: 64-wide dh blocks of [128 kv rows x 128 B]; 16 kv rows = two 1024 B swizzle atoms
+      WG<DH, BF>::template rs<1>(o, pf[kc], make_smem_desc_sw128(vbase + kc * 2048, 16384, 1024), 1u);
+    wgmma_commit();
+    wgmma_wait<0>();
+#pragma unroll
+    for (int i = 0; i < DH / 2; ++i) reg_fence(o[i]);
+#pragma unroll
+    for (int kc = 0; kc < 8; ++kc)
+#pragma unroll
+      for (int q = 0; q < 4; ++q) reg_fence(pf[kc][q]);
+  }
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    const int qi = q0 + wg * 64 + fr + 8 * r;
+    const float l = quad_sum(l_run[r]);
+    if (qi < L) {
+      const float inv = 1.f / l;
+      uint16_t* dst = a.out + ((size_t)b * L + qi) * a.d + h * DH + fc;
+#pragma unroll
+      for (int i = 0; i < DH / 8; ++i)
+        *reinterpret_cast<uint32_t*>(dst + 8 * i) = cvt16x2(o[4 * i + 2 * r] * inv, o[4 * i + 2 * r + 1] * inv, BF);
+      if (a.lse && (lane & 3) == 0) a.lse[((size_t)b * a.H + h) * L + qi] = m_run[r] * 0.6931471805599453f + logf(l);
+    }
   }
 }
 
@@ -273,13 +245,13 @@ __global__ void __launch_bounds__(128) attention_simt_kernel(const AttnSimtArgs 
   if (lane == 0 && a.lse) a.lse[((size_t)b * a.H + h) * a.L + i] = mx + logf(sum);
 }
 
-template <int DH>
+template <int DH, int BF>
 static int launch_tc(const AttnArgs& a, cudaStream_t stream) {
   using Cfg = AttnCfg<DH>;
   static bool attr_set = false;
   if (!attr_set) {
     cudaError_t e =
-        cudaFuncSetAttribute(attention_tcgen05_kernel<DH>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes);
+        cudaFuncSetAttribute(attention_wgmma_kernel<DH, BF>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes);
     if (e != cudaSuccess) {
       set_error("cudaFuncSetAttribute(attention): %s", cudaGetErrorString(e));
       return (int)e;
@@ -287,7 +259,7 @@ static int launch_tc(const AttnArgs& a, cudaStream_t stream) {
     attr_set = true;
   }
   dim3 grid((a.L + 127) / 128, a.H, a.B);
-  launch_k(attention_tcgen05_kernel<DH>, dim3(grid), dim3(160), Cfg::kSmemBytes, stream, a);
+  launch_k(attention_wgmma_kernel<DH, BF>, dim3(grid), dim3(256), Cfg::kSmemBytes, stream, a);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) set_error("attention launch failed: %s", cudaGetErrorString(e));
   return (int)e;
@@ -311,8 +283,8 @@ int launch_attention_simt(const AttnArgs& a, const uint16_t* qkv, cudaStream_t s
 }
 
 int launch_attention(const AttnArgs& a, cudaStream_t stream) {
-  if (a.dh == 128) return launch_tc<128>(a, stream);
-  if (a.dh == 64) return launch_tc<64>(a, stream);
+  if (a.dh == 128) return a.fmt ? launch_tc<128, 1>(a, stream) : launch_tc<128, 0>(a, stream);
+  if (a.dh == 64) return a.fmt ? launch_tc<64, 1>(a, stream) : launch_tc<64, 0>(a, stream);
   set_error("launch_attention: tensor-core path needs dh in {64,128}, got %d", a.dh);
   return (int)cudaErrorInvalidValue;
 }

@@ -1,54 +1,31 @@
-// Attention backward on tcgen05 (SURVEY.md A.6): per (batch, head, 128-key tile) CTA, loop over 128-query tiles.
-//   S  = Q K^T                (recomputed)          P  = exp(scale * S - lse)  (key padding -> 0)
-//   dP = dO V^T                                     dZ = P o (dP - delta),  dS = scale * dZ
-//   dV += P^T dO    dK += dS^T Q    dQ_i = dS K     (dQ accumulated over key tiles in fp32 global memory)
-// Five MMAs per (query tile, key tile); every operand is a 128B-swizzled 16-bit tile in shared memory that is read
-// either K-major or MN-major, so no transposed copies are ever made:
-//   S : A = Q  [q x dh]  K-major      B = K  [kv x dh] K-major
-//   dP: A = dO [q x dh]  K-major      B = V  [kv x dh] K-major
-//   dV: A = P  [q x kv]  MN-major (M = kv)   B = dO [q x dh] MN-major (N = dh)   contraction over q
-//   dK: A = dS [q x kv]  MN-major            B = Q  [q x dh] MN-major
-//   dQ: A = dS [q x kv]  K-major             B = K  [kv x dh] MN-major (N = dh)  contraction over kv
-// TMEM (512 columns): [0,128) S then dQ_i, [128,256) dP, [256,256+dh) dV, [384,384+dh) dK.
-// Activations (Q, K, V, P) are fp16/bf16 per plan; gradients (dO, dS) are bf16.
-// warp 0 lane 0: TMA + MMA issue; warps 1..4: softmax / gradient math (thread = tile row).
+// Attention backward on wgmma (SURVEY.md A.6): per (batch, head, 128-key tile) CTA, loop over 128-query tiles, each processed
+// as two 64-query halves.  Everything is computed transposed (rows = keys), so that P^T and dS^T come out of the accumulators
+// in the layout of a wgmma A fragment and the dV / dK products take them straight from registers:
+//   S^T  = K Q^T   (recomputed)                      P^T  = exp(scale * S^T - lse)  (key padding -> 0)
+//   dP^T = V dO^T                                    dS^T = P^T o (dP^T - delta) * scale
+//   dV  += P^T dO       dK += dS^T Q                 dQ_i = dS K  (dS^T staged through smem; fp32 global accumulation over key tiles)
+// Two warpgroups, warpgroup w owns keys [64 w, 64 w + 64) of the tile (S^T / dP^T: wgmma m64n64, A = K / V rows, B = Q / dO
+// rows, all K-major; dV / dK: A from registers, B = dO / Q rows of the half, MN-major).  dQ of a half: A = dS^T (MN-major smem,
+// M = queries), B = K (MN-major, N = dh); with dh = 128 each warpgroup computes 64 of the dh columns, with dh = 64 warpgroup 0.
+// Q, K, V, dO, P and dS share one 16-bit format (a wgmma takes A and B in one format).
 #include <math.h>
 
 #include "backward.h"
 #include "kernels.h"
 #include "ptx.cuh"
+#include "wgmma.cuh"
 
 namespace uv {
 
 template <int DH>
 struct AttnBwdCfg {
   static constexpr int kTile = 128 * DH * 2;  // Q, dO, K, V tiles: DH/64 boxes of [128 rows x 64]
-  static constexpr int kPS = 32768;           // P and dS tiles [128 x 128] 16-bit: 2 boxes of [128 rows x 64]
-  static constexpr int kSmemBytes = 1024 + 4 * kTile + 2 * kPS + 128 * 4 + 256;
-  static constexpr uint32_t kTmemCols = 512;
+  static constexpr int kDS = 128 * 128;       // dS^T of one 64-query half: [128 keys x 64 queries] 16-bit, 128B-swizzled rows
+  static constexpr int kSmemBytes = 1024 + 4 * kTile + kDS + 3 * 128 * 4 + 64;
 };
 
-// 32 fp32 accumulator columns of this thread's row -> 16-bit at dqkv16[elem_off ..] (single-key-tile fast path: the values are
-// final, so they go straight to the operand buffer of the in-projection dgrad / wgrad GEMMs; the in_proj_bias gradient is a
-// separate column-sum pass over that buffer - accumulating it here with a transposing warp reduction measured slower).
-__device__ __forceinline__ void store16_colsum(const AttnBwdArgs& a, const uint32_t (&r)[32], bool valid, size_t elem_off, int col0,
-                                               int lane) {
-  (void)col0;
-  (void)lane;
-  if (valid) {
-    uint16_t* dst = a.dqkv16 + elem_off;
-#pragma unroll
-    for (int e = 0; e < 32; e += 8)
-      *reinterpret_cast<uint4*>(dst + e) =
-          make_uint4(cvt16x2(__uint_as_float(r[e]), __uint_as_float(r[e + 1]), a.fmt_grad),
-                     cvt16x2(__uint_as_float(r[e + 2]), __uint_as_float(r[e + 3]), a.fmt_grad),
-                     cvt16x2(__uint_as_float(r[e + 4]), __uint_as_float(r[e + 5]), a.fmt_grad),
-                     cvt16x2(__uint_as_float(r[e + 6]), __uint_as_float(r[e + 7]), a.fmt_grad));
-  }
-}
-
-template <int DH>
-__global__ void __launch_bounds__(160, 1) attention_bwd_tcgen05_kernel(const __grid_constant__ AttnBwdArgs a) {
+template <int DH, int BF>
+__global__ void __launch_bounds__(256, 1) attention_bwd_wgmma_kernel(const __grid_constant__ AttnBwdArgs a) {
   using Cfg = AttnBwdCfg<DH>;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw_addr = smem_u32(smem_raw);
@@ -57,237 +34,207 @@ __global__ void __launch_bounds__(160, 1) attention_bwd_tcgen05_kernel(const __g
   uint8_t* sdO = sQ + Cfg::kTile;
   uint8_t* sK = sdO + Cfg::kTile;
   uint8_t* sV = sK + Cfg::kTile;
-  uint8_t* sP = sV + Cfg::kTile;
-  uint8_t* sdS = sP + Cfg::kPS;
-  float* s_bias = reinterpret_cast<float*>(sdS + Cfg::kPS);  // [128] 0 / -inf per key of this CTA's key tile
-  uint64_t* bars = reinterpret_cast<uint64_t*>(s_bias + 128);
+  uint8_t* sdS = sV + Cfg::kTile;
+  float* s_kbias = reinterpret_cast<float*>(sdS + Cfg::kDS);  // [128] 0 / -inf per key of this CTA's key tile
+  float* s_lse2 = s_kbias + 128;                              // [128] lse * log2(e) per query of the tile (+inf: no query)
+  float* s_dlt = s_lse2 + 128;                                // [128] delta per query of the tile
+  uint64_t* bars = reinterpret_cast<uint64_t*>(s_dlt + 128);
   uint64_t* kv_full = bars + 0;
   uint64_t* qdo_full = bars + 1;
-  uint64_t* sdp_full = bars + 2;
-  uint64_t* pds_full = bars + 3;
-  uint64_t* it_done = bars + 4;
-  uint64_t* dq_read = bars + 5;
-  uint32_t* tmem_holder = reinterpret_cast<uint32_t*>(bars + 6);
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7;
+  const int tid = threadIdx.x & 127;
+  const int fr = 16 * (tid >> 5) + (lane >> 2);  // accumulator rows fr, fr + 8; columns 8 i + fc, + 1
+  const int fc = 2 * (lane & 3);
   const int j = blockIdx.x;  // key tile
   const int h = blockIdx.y;
   const int b = blockIdx.z;
   const int L = a.L;
   const int num_q = (L + 127) / 128;
+  const size_t ld3 = (size_t)3 * a.d;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&a.tm_qkv);
     tma_prefetch_desc(&a.tm_do);
     mbar_init(kv_full, 1);
     mbar_init(qdo_full, 1);
-    mbar_init(sdp_full, 1);
-    mbar_init(pds_full, 4);
-    mbar_init(it_done, 1);
-    mbar_init(dq_read, 4);
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc<Cfg::kTmemCols>(tmem_holder);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  // Only now (this CTA owns its TMEM columns) may the next grid be scheduled: a dependent CTA that grabbed TMEM first and
-  // then blocked in griddepcontrol.wait could starve a CTA of this grid sharing its SM.
   pdl_launch_dependents();
   pdl_wait();  // setup done; everything below reads the previous kernels' outputs
-  const uint32_t tmem_base = *tmem_holder;
-  const uint32_t tm_s = tmem_base, tm_dp = tmem_base + 128, tm_dv = tmem_base + 256, tm_dk = tmem_base + 384;
-
-  if (warp == 0) {
-    if (lane == 0) {
-      const int fa = a.fmt_act, fg = a.fmt_grad;
-      const uint32_t id_s = make_idesc_f16_ab(128, 128, fa, fa, 0, 0);
-      const uint32_t id_dp = make_idesc_f16_ab(128, 128, fg, fa, 0, 0);
-      const uint32_t id_dv = make_idesc_f16_ab(128, DH, fa, fg, 1, 1);
-      const uint32_t id_dk = make_idesc_f16_ab(128, DH, fg, fa, 1, 1);
-      const uint32_t id_dq = make_idesc_f16_ab(128, DH, fg, fa, 0, 1);
-      mbar_arrive_expect_tx(kv_full, 2 * Cfg::kTile);
+  if (threadIdx.x == 0) {
+    mbar_arrive_expect_tx(kv_full, 2 * Cfg::kTile);
 #pragma unroll
-      for (int kb = 0; kb < DH / 64; ++kb) {
-        tma_load_2d(sK + kb * 16384, &a.tm_qkv, kv_full, a.d + h * DH + kb * 64, b * L + j * 128);
-        tma_load_2d(sV + kb * 16384, &a.tm_qkv, kv_full, 2 * a.d + h * DH + kb * 64, b * L + j * 128);
-      }
-      for (int i = 0; i < num_q; ++i) {
-        const uint32_t ph = i & 1;
-        if (i > 0) mbar_wait(it_done, ph ^ 1);  // MMAs of the previous query tile retired: Q, dO, P, dS tiles are free
-        mbar_arrive_expect_tx(qdo_full, 2 * Cfg::kTile);
-#pragma unroll
-        for (int kb = 0; kb < DH / 64; ++kb) {
-          tma_load_2d(sQ + kb * 16384, &a.tm_qkv, qdo_full, h * DH + kb * 64, b * L + i * 128);
-          tma_load_2d(sdO + kb * 16384, &a.tm_do, qdo_full, h * DH + kb * 64, b * L + i * 128);
-        }
-        if (i == 0) mbar_wait(kv_full, 0);
-        mbar_wait(qdo_full, ph);
-        if (i > 0) mbar_wait(dq_read, ph ^ 1);  // dQ_{i-1} has been drained from the S columns
-        tc_fence_after();
-#pragma unroll
-        for (int ks = 0; ks < DH / 16; ++ks) {
-          const uint32_t off = (ks / 4) * 16384 + (ks % 4) * 32;
-          umma_f16_ss(tm_s, make_smem_desc_sw128(smem_u32(sQ) + off, 16, 1024), make_smem_desc_sw128(smem_u32(sK) + off, 16, 1024),
-                      id_s, ks > 0 ? 1u : 0u);
-        }
-#pragma unroll
-        for (int ks = 0; ks < DH / 16; ++ks) {
-          const uint32_t off = (ks / 4) * 16384 + (ks % 4) * 32;
-          umma_f16_ss(tm_dp, make_smem_desc_sw128(smem_u32(sdO) + off, 16, 1024),
-                      make_smem_desc_sw128(smem_u32(sV) + off, 16, 1024), id_dp, ks > 0 ? 1u : 0u);
-        }
-        umma_commit(sdp_full);
-        mbar_wait(pds_full, ph);
-        tc_fence_after();
-#pragma unroll
-        for (int ks = 0; ks < 8; ++ks) {  // contraction over the 128 query rows, 16 per step = two 1024 B atoms
-          const uint32_t offk = ks * 2048;
-          umma_f16_ss(tm_dv, make_smem_desc_sw128(smem_u32(sP) + offk, 16384, 1024),
-                      make_smem_desc_sw128(smem_u32(sdO) + offk, 16384, 1024), id_dv, (i > 0 || ks > 0) ? 1u : 0u);
-        }
-#pragma unroll
-        for (int ks = 0; ks < 8; ++ks) {
-          const uint32_t offk = ks * 2048;
-          umma_f16_ss(tm_dk, make_smem_desc_sw128(smem_u32(sdS) + offk, 16384, 1024),
-                      make_smem_desc_sw128(smem_u32(sQ) + offk, 16384, 1024), id_dk, (i > 0 || ks > 0) ? 1u : 0u);
-        }
-#pragma unroll
-        for (int ks = 0; ks < 8; ++ks) {  // contraction over the 128 keys
-          const uint32_t offa = (ks / 4) * 16384 + (ks % 4) * 32;
-          umma_f16_ss(tm_s, make_smem_desc_sw128(smem_u32(sdS) + offa, 16, 1024),
-                      make_smem_desc_sw128(smem_u32(sK) + ks * 2048, 16384, 1024), id_dq, ks > 0 ? 1u : 0u);
-        }
-        umma_commit(it_done);
-      }
-    }
-  } else {
-    const int wq = warp & 3;
-    const int row = wq * 32 + lane;
-    const int tid = threadIdx.x - 32;
-    const uint32_t lane_addr = (uint32_t)(wq * 32) << 16;
-    const float c_log2e = 1.4426950408889634f;
-    const float sc2 = a.scale * c_log2e;
-    {
-      const int key = j * 128 + tid;
-      s_bias[tid] = (key < L && a.key_mask[(size_t)b * L + key] != 0.f) ? 0.f : -INFINITY;
-    }
-    asm volatile("bar.sync 1, 128;" ::: "memory");
-    const size_t ld3 = (size_t)3 * a.d;
-    for (int i = 0; i < num_q; ++i) {
-      const uint32_t ph = i & 1;
-      const int qi = i * 128 + row;
-      const bool qvalid = qi < L;
-      float lse2 = 0.f, dlt = 0.f;
-      if (qvalid) {
-        lse2 = a.lse[((size_t)b * a.H + h) * L + qi] * c_log2e;
-        dlt = a.delta[((size_t)b * a.H + h) * L + qi];
-      }
-      mbar_wait(sdp_full, ph);
-      tc_fence_after();
-#pragma unroll
-      for (int c = 0; c < 4; ++c) {
-        uint32_t rs[32], rp[32];
-        tmem_ld_32x32b_x32(tm_s + lane_addr + c * 32, rs);
-        tmem_ld_32x32b_x32(tm_dp + lane_addr + c * 32, rp);
-        tmem_ld_wait();
-        uint32_t pk[16], dk[16];
-#pragma unroll
-        for (int e = 0; e < 32; e += 2) {
-          float p0 = 0.f, p1 = 0.f;
-          if (qvalid) {
-            p0 = exp2f(__uint_as_float(rs[e]) * sc2 + s_bias[c * 32 + e] - lse2);
-            p1 = exp2f(__uint_as_float(rs[e + 1]) * sc2 + s_bias[c * 32 + e + 1] - lse2);
-          }
-          const float d0 = p0 * (__uint_as_float(rp[e]) - dlt) * a.scale;
-          const float d1 = p1 * (__uint_as_float(rp[e + 1]) - dlt) * a.scale;
-          pk[e / 2] = cvt16x2(p0, p1, a.fmt_act);
-          dk[e / 2] = cvt16x2(p0 == 0.f ? 0.f : d0, p1 == 0.f ? 0.f : d1, a.fmt_grad);
-        }
-        uint8_t* prow = sP + (c / 2) * 16384 + row * 128;
-        uint8_t* drow = sdS + (c / 2) * 16384 + row * 128;
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          const int chunk = ((c & 1) * 4 + q) ^ (row & 7);
-          *reinterpret_cast<uint4*>(prow + chunk * 16) = make_uint4(pk[q * 4], pk[q * 4 + 1], pk[q * 4 + 2], pk[q * 4 + 3]);
-          *reinterpret_cast<uint4*>(drow + chunk * 16) = make_uint4(dk[q * 4], dk[q * 4 + 1], dk[q * 4 + 2], dk[q * 4 + 3]);
-        }
-      }
-      fence_proxy_async_smem();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(pds_full);
-      // dQ_i (this thread's query row) -> fp32 global
-      mbar_wait(it_done, ph);
-      tc_fence_after();
-#pragma unroll
-      for (int c = 0; c < DH / 32; ++c) {
-        uint32_t r[32];
-        tmem_ld_32x32b_x32(tm_s + lane_addr + c * 32, r);
-        tmem_ld_wait();
-        if (a.dqkv16 != nullptr) {  // single key tile: final values, straight to the 16-bit GEMM operand (+ bias-gradient sums)
-          store16_colsum(a, r, qvalid, ((size_t)b * L + qi) * ld3 + h * DH + c * 32, h * DH + c * 32, lane);
-        } else if (qvalid) {
-          float* dst = a.dqkv32 + ((size_t)b * L + qi) * ld3 + h * DH + c * 32;
-          if (a.dq_atomic) {
-#pragma unroll
-            for (int e = 0; e < 32; ++e) atomicAdd(dst + e, __uint_as_float(r[e]));
-          } else {
-#pragma unroll
-            for (int e = 0; e < 32; e += 4)
-              *reinterpret_cast<float4*>(dst + e) = make_float4(__uint_as_float(r[e]), __uint_as_float(r[e + 1]),
-                                                                __uint_as_float(r[e + 2]), __uint_as_float(r[e + 3]));
-          }
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(dq_read);
-    }
-    // dV, dK of this key tile (thread = key row).  tcgen05.ld is warp-collective: loads are unconditional, stores predicated.
-    const int kv = j * 128 + row;
-    const bool kvalid = kv < L;
-    float* dk_dst = a.dqkv32 + ((size_t)b * L + (kvalid ? kv : 0)) * ld3 + a.d + h * DH;
-    float* dv_dst = a.dqkv32 + ((size_t)b * L + (kvalid ? kv : 0)) * ld3 + 2 * a.d + h * DH;
-#pragma unroll
-    for (int c = 0; c < DH / 32; ++c) {
-      uint32_t r[32];
-      tmem_ld_32x32b_x32(tm_dv + lane_addr + c * 32, r);
-      tmem_ld_wait();
-      if (a.dqkv16 != nullptr) {
-        store16_colsum(a, r, kvalid, ((size_t)b * L + (kvalid ? kv : 0)) * ld3 + 2 * a.d + h * DH + c * 32, 2 * a.d + h * DH + c * 32, lane);
-      } else if (kvalid) {
-#pragma unroll
-        for (int e = 0; e < 32; e += 4)
-          *reinterpret_cast<float4*>(dv_dst + c * 32 + e) =
-              make_float4(__uint_as_float(r[e]), __uint_as_float(r[e + 1]), __uint_as_float(r[e + 2]), __uint_as_float(r[e + 3]));
-      }
-      tmem_ld_32x32b_x32(tm_dk + lane_addr + c * 32, r);
-      tmem_ld_wait();
-      if (a.dqkv16 != nullptr) {
-        store16_colsum(a, r, kvalid, ((size_t)b * L + (kvalid ? kv : 0)) * ld3 + a.d + h * DH + c * 32, a.d + h * DH + c * 32, lane);
-      } else if (kvalid) {
-#pragma unroll
-        for (int e = 0; e < 32; e += 4)
-          *reinterpret_cast<float4*>(dk_dst + c * 32 + e) =
-              make_float4(__uint_as_float(r[e]), __uint_as_float(r[e + 1]), __uint_as_float(r[e + 2]), __uint_as_float(r[e + 3]));
-      }
+    for (int kb = 0; kb < DH / 64; ++kb) {
+      tma_load_2d(sK + kb * 16384, &a.tm_qkv, kv_full, a.d + h * DH + kb * 64, b * L + j * 128);
+      tma_load_2d(sV + kb * 16384, &a.tm_qkv, kv_full, 2 * a.d + h * DH + kb * 64, b * L + j * 128);
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc<Cfg::kTmemCols>(tmem_base);
+  if (threadIdx.x < 128) {
+    const int key = j * 128 + threadIdx.x;
+    s_kbias[threadIdx.x] = (key < L && a.key_mask[(size_t)b * L + key] != 0.f) ? 0.f : -INFINITY;
+  }
+  const float c_log2e = 1.4426950408889634f;
+  const float sc2 = a.scale * c_log2e;
+  const uint32_t uQ = smem_u32(sQ), udO = smem_u32(sdO), uK = smem_u32(sK), uV = smem_u32(sV), udS = smem_u32(sdS);
+
+  float dv[DH / 2], dk[DH / 2];
+#pragma unroll
+  for (int i = 0; i < DH / 2; ++i) dv[i] = dk[i] = 0.f;
+
+  for (int i = 0; i < num_q; ++i) {
+    __syncthreads();  // every wgmma of the previous query tile has retired: Q / dO tiles and the per-query rows are free
+    if (threadIdx.x == 0) {
+      mbar_arrive_expect_tx(qdo_full, 2 * Cfg::kTile);
+#pragma unroll
+      for (int kb = 0; kb < DH / 64; ++kb) {
+        tma_load_2d(sQ + kb * 16384, &a.tm_qkv, qdo_full, h * DH + kb * 64, b * L + i * 128);
+        tma_load_2d(sdO + kb * 16384, &a.tm_do, qdo_full, h * DH + kb * 64, b * L + i * 128);
+      }
+    }
+    if (threadIdx.x < 128) {
+      const int qi = i * 128 + threadIdx.x;
+      const bool qvalid = qi < L;
+      s_lse2[threadIdx.x] = qvalid ? a.lse[((size_t)b * a.H + h) * L + qi] * c_log2e : INFINITY;
+      s_dlt[threadIdx.x] = qvalid ? a.delta[((size_t)b * a.H + h) * L + qi] : 0.f;
+    }
+    __syncthreads();
+    if (i == 0) mbar_wait(kv_full, 0);
+    mbar_wait(qdo_full, i & 1);
+
+#pragma unroll 1
+    for (int hq = 0; hq < 2; ++hq) {
+      float st[32], dpt[32];
+      wgmma_fence();
+#pragma unroll
+      for (int ks = 0; ks < DH / 16; ++ks) {
+        const uint32_t off = (ks / 4) * 16384 + (ks % 4) * 32;
+        WG<64, BF>::template ss<0, 0>(st, make_smem_desc_sw128(uK + wg * 8192 + off, 16, 1024),
+                                      make_smem_desc_sw128(uQ + hq * 8192 + off, 16, 1024), ks > 0 ? 1u : 0u);
+      }
+#pragma unroll
+      for (int ks = 0; ks < DH / 16; ++ks) {
+        const uint32_t off = (ks / 4) * 16384 + (ks % 4) * 32;
+        WG<64, BF>::template ss<0, 0>(dpt, make_smem_desc_sw128(uV + wg * 8192 + off, 16, 1024),
+                                      make_smem_desc_sw128(udO + hq * 8192 + off, 16, 1024), ks > 0 ? 1u : 0u);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+#pragma unroll
+      for (int e = 0; e < 32; ++e) {
+        reg_fence(st[e]);
+        reg_fence(dpt[e]);
+      }
+      // P^T and dS^T (rows = keys fr / fr + 8 of this warpgroup, columns = queries 64 hq + 8 c + fc + {0, 1})
+      const float kb2[2] = {s_kbias[wg * 64 + fr], s_kbias[wg * 64 + fr + 8]};
+      uint32_t pf[4][4], df[4][4];
+#pragma unroll
+      for (int c = 0; c < 8; ++c) {
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+          float p[2], d[2];
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int col = hq * 64 + 8 * c + fc + e;
+            p[e] = exp2f(st[4 * c + 2 * r + e] * sc2 + kb2[r] - s_lse2[col]);
+            d[e] = p[e] == 0.f ? 0.f : p[e] * (dpt[4 * c + 2 * r + e] - s_dlt[col]) * a.scale;
+          }
+          // accumulator block c, row half r -> A-fragment k-chunk c / 2, register (c & 1) * 2 + r
+          pf[c >> 1][(c & 1) * 2 + r] = cvt16x2(p[0], p[1], BF);
+          df[c >> 1][(c & 1) * 2 + r] = cvt16x2(d[0], d[1], BF);
+          // dS^T row -> smem: 128 B per key row (64 queries), 16-byte chunk c XOR-swizzled with row % 8
+          const int row = wg * 64 + fr + 8 * r;
+          *reinterpret_cast<uint32_t*>(sdS + row * 128 + ((c ^ (row & 7)) << 4) + fc * 2) = df[c >> 1][(c & 1) * 2 + r];
+        }
+      }
+      fence_proxy_async_smem();  // generic-proxy smem writes -> visible to the tensor core (async proxy)
+      wgmma_fence();
+#pragma unroll
+      for (int kc = 0; kc < 4; ++kc)  // contraction over the 64 queries of the half, 16 per step = two 1024 B atoms
+        WG<DH, BF>::template rs<1>(dv, pf[kc], make_smem_desc_sw128(udO + hq * 8192 + kc * 2048, 16384, 1024), 1u);
+#pragma unroll
+      for (int kc = 0; kc < 4; ++kc)
+        WG<DH, BF>::template rs<1>(dk, df[kc], make_smem_desc_sw128(uQ + hq * 8192 + kc * 2048, 16384, 1024), 1u);
+      wgmma_commit();
+      wgmma_wait<0>();
+#pragma unroll
+      for (int e = 0; e < DH / 2; ++e) {
+        reg_fence(dv[e]);
+        reg_fence(dk[e]);
+      }
+#pragma unroll
+      for (int kc = 0; kc < 4; ++kc)
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+          reg_fence(pf[kc][q]);
+          reg_fence(df[kc][q]);
+        }
+      __syncthreads();  // both warpgroups' dS^T rows are in smem
+      if (DH == 128 || wg == 0) {
+        const int c0 = DH == 128 ? wg * 64 : 0;  // dh columns of dQ this warpgroup computes
+        float dq[32];
+        wgmma_fence();
+#pragma unroll
+        for (int kc = 0; kc < 8; ++kc)  // contraction over the 128 keys
+          WG<64, BF>::template ss<1, 1>(dq, make_smem_desc_sw128(udS + kc * 2048, 8192, 1024),
+                                        make_smem_desc_sw128(uK + (c0 / 64) * 16384 + kc * 2048, 16384, 1024), kc > 0 ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait<0>();
+#pragma unroll
+        for (int e = 0; e < 32; ++e) reg_fence(dq[e]);
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+          const int qi = i * 128 + hq * 64 + fr + 8 * r;
+          if (qi < L) {
+            const size_t base = ((size_t)b * L + qi) * ld3 + h * DH + c0 + fc;
+#pragma unroll
+            for (int c = 0; c < 8; ++c) {
+              const float x0 = dq[4 * c + 2 * r], x1 = dq[4 * c + 2 * r + 1];
+              if (a.dqkv16 != nullptr) {  // single key tile: final values, straight to the 16-bit GEMM operand
+                *reinterpret_cast<uint32_t*>(a.dqkv16 + base + 8 * c) = cvt16x2(x0, x1, a.fmt_grad);
+              } else if (a.dq_atomic) {
+                atomicAdd(a.dqkv32 + base + 8 * c, x0);
+                atomicAdd(a.dqkv32 + base + 8 * c + 1, x1);
+              } else {
+                *reinterpret_cast<float2*>(a.dqkv32 + base + 8 * c) = make_float2(x0, x1);
+              }
+            }
+          }
+        }
+      }
+      __syncthreads();  // dS^T buffer free for the next half
+    }
+  }
+  // dK, dV of this key tile (rows = keys)
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    const int kv = j * 128 + wg * 64 + fr + 8 * r;
+    if (kv < L) {
+      const size_t row = ((size_t)b * L + kv) * ld3 + h * DH + fc;
+#pragma unroll
+      for (int c = 0; c < DH / 8; ++c) {
+        const float k0 = dk[4 * c + 2 * r], k1 = dk[4 * c + 2 * r + 1];
+        const float v0 = dv[4 * c + 2 * r], v1 = dv[4 * c + 2 * r + 1];
+        if (a.dqkv16 != nullptr) {
+          *reinterpret_cast<uint32_t*>(a.dqkv16 + row + a.d + 8 * c) = cvt16x2(k0, k1, a.fmt_grad);
+          *reinterpret_cast<uint32_t*>(a.dqkv16 + row + 2 * a.d + 8 * c) = cvt16x2(v0, v1, a.fmt_grad);
+        } else {
+          *reinterpret_cast<float2*>(a.dqkv32 + row + a.d + 8 * c) = make_float2(k0, k1);
+          *reinterpret_cast<float2*>(a.dqkv32 + row + 2 * a.d + 8 * c) = make_float2(v0, v1);
+        }
+      }
+    }
   }
 }
 
-template <int DH>
+template <int DH, int BF>
 static int launch_bwd_tc(const AttnBwdArgs& a, cudaStream_t stream) {
   using Cfg = AttnBwdCfg<DH>;
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(attention_bwd_tcgen05_kernel<DH>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    cudaError_t e = cudaFuncSetAttribute(attention_bwd_wgmma_kernel<DH, BF>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                          Cfg::kSmemBytes);
     if (e != cudaSuccess) {
       set_error("cudaFuncSetAttribute(attention_bwd): %s", cudaGetErrorString(e));
@@ -296,15 +243,20 @@ static int launch_bwd_tc(const AttnBwdArgs& a, cudaStream_t stream) {
     attr_set = true;
   }
   dim3 grid((a.L + 127) / 128, a.H, a.B);
-  launch_k(attention_bwd_tcgen05_kernel<DH>, dim3(grid), dim3(160), Cfg::kSmemBytes, stream, a);
+  launch_k(attention_bwd_wgmma_kernel<DH, BF>, dim3(grid), dim3(256), Cfg::kSmemBytes, stream, a);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) set_error("attention_bwd launch failed: %s", cudaGetErrorString(e));
   return (int)e;
 }
 
 int launch_attention_bwd(const AttnBwdArgs& a, cudaStream_t stream) {
-  if (a.dh == 128) return launch_bwd_tc<128>(a, stream);
-  if (a.dh == 64) return launch_bwd_tc<64>(a, stream);
+  if (a.fmt_act != a.fmt_grad) {
+    set_error("launch_attention_bwd: activations and gradients must share one 16-bit format (got %d and %d)", a.fmt_act, a.fmt_grad);
+    return (int)cudaErrorInvalidValue;
+  }
+  const bool bf = a.fmt_act != 0;
+  if (a.dh == 128) return bf ? launch_bwd_tc<128, 1>(a, stream) : launch_bwd_tc<128, 0>(a, stream);
+  if (a.dh == 64) return bf ? launch_bwd_tc<64, 1>(a, stream) : launch_bwd_tc<64, 0>(a, stream);
   set_error("launch_attention_bwd: tensor-core path needs dh in {64,128}, got %d", a.dh);
   return (int)cudaErrorInvalidValue;
 }

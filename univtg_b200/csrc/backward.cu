@@ -196,7 +196,7 @@ __global__ void __launch_bounds__(128) layernorm_bwd_vec_kernel(const LnBwdArgs 
 
 // Warp-per-row variant for d == NV * 128 (256 / 512 / 1024: every LayerNorm of the encoder and the inner projector layers).  A warp
 // holds its whole row in registers, so the two row statistics are warp shuffles - no block barrier per row (the block-per-row
-// kernel above spends two __syncthreads per 1024-element row and measured 45 % of the HBM roofline).  Column partials (dgamma,
+// kernel above spends two __syncthreads per 1024-element row).  Column partials (dgamma,
 // dbeta, bias column sums) stay in registers over the rows a warp visits, are combined across the block's 8 warps through
 // shared memory and leave as ONE vector reduction per block and column group.
 template <int NV>
@@ -354,7 +354,7 @@ int launch_layernorm_bwd(const LnBwdArgs& a, cudaStream_t stream) {
   }
   const bool warp_ok = use_warp && vec && (a.d == 256 || a.d == 512 || a.d == 1024) && (!a.dbr16 || a.ld16 == a.d);
   if (warp_ok) {
-    int dev = 0, sms = 148;
+    int dev = 0, sms = 132;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     int wgrid = (a.rows + 7) / 8;

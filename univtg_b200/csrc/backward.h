@@ -64,11 +64,11 @@ struct AttnBwdArgs {
   int B, L, H, dh, d;
   int fmt_act, fmt_grad;  // formats of qkv / dO
   int dq_atomic;          // 1 when dqkv32 was pre-zeroed and dQ must be accumulated (more than one key tile or SIMT path)
-  // Single-key-tile fast path (L <= 128, tcgen05 kernel): write dQ | dK | dV directly as 16-bit operands of the in-projection
+  // Single-key-tile fast path (L <= 128, tensor-core kernel): write dQ | dK | dV directly as 16-bit operands of the in-projection
   // dgrad / wgrad GEMMs; dqkv32 is then not written (the in_proj_bias gradient comes from launch_colsum16 over this buffer).
   uint16_t* dqkv16;       // [B*L, 3d] or null
 };
-int launch_attention_bwd(const AttnBwdArgs& a, cudaStream_t stream);       // tcgen05, dh in {64, 128}
+int launch_attention_bwd(const AttnBwdArgs& a, cudaStream_t stream);       // wgmma, dh in {64, 128}
 int launch_attention_bwd_simt(const AttnBwdArgs& a, cudaStream_t stream);  // any dh; needs dqkv32 pre-zeroed
 
 // ---- conv heads: last layer (1 / 2 output channels) ----

@@ -1,59 +1,57 @@
-// Persistent, warp-specialised tcgen05 GEMM for sm_100a with a fused, run-time configured epilogue.
+// Persistent, warp-specialised wgmma GEMM for sm_90a with a fused, run-time configured epilogue.
 //
-//   C[M,N] = epilogue( sum_k A[m,k] * B[n,k] ),  A/B 16-bit (fp16 or bf16), fp32 accumulation in TMEM.
+//   C[M,N] = epilogue( sum_k A[m,k] * B[n,k] ),  A/B 16-bit (fp16 or bf16, both operands in one format), fp32 accumulation.
 //
 // This one kernel serves every dense contraction of the UniVTG hot path (SURVEY.md §2.2 rows K1-K3, K5, K7,
 // K9-K11 and their backward passes): input projectors (model/univtg.py:399-406), the three attention
 // in-projections + out-projection (torch MHA called at model/transformer_encoder_droppath.py:118), the FFN
 // (:122) and the k=3 Conv1d heads (model/univtg.py:378-382) expressed as three row-shifted K segments.
 //
-// Roles (384 threads, 1 CTA / SM, persistent over a static round-robin tile schedule):
-//   warp 0 lane 0 : TMA producer   (cp.async.bulk.tensor -> 128B-swizzled smem ring, mbarrier expect_tx)
-//   warp 1 lane 0 : MMA issuer     (tcgen05.mma cta_group::1, M=128, N=BN, K=16 x4 per 64-wide k-block)
-//   warp 2        : TMEM allocator (2 accumulator stages of BN fp32 columns)
-//   warps 4..11   : epilogue       (tcgen05.ld 32x32b; thread = row owns whole 32 B sectors -> 128-bit global loads/stores;
-//                                   the TMEM load + residual loads of step c+1 are in flight while step c is processed)
+// Roles (384 threads = 3 warpgroups, 1 CTA / SM, persistent over a static round-robin tile schedule of 128 x BN tiles):
+//   warpgroup 2 (one elected lane of warp 8): TMA producer (cp.async.bulk.tensor -> 128B-swizzled smem ring, mbarrier
+//                    expect_tx); it gives most of its registers to the consumers (setmaxnreg)
+//   warpgroups 0, 1: consumers.  Each issues wgmma m64 x BN x k16 for its 64 rows of the tile (accumulators in registers),
+//                    then runs the epilogue of those rows: the accumulators go through shared memory 32 columns at a time so
+//                    that a thread owns 16 consecutive columns of one row (whole 32 B sectors, 128-bit global accesses).
+// CL = 2 (clusters of two CTAs, K-major B only): the pair computes two vertically adjacent 128-row tiles of the same BN
+// columns; each CTA loads half of the B tile and multicasts it to both, so every B byte crosses L2 once per pair.
 #include <stdarg.h>
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
 
-#include <type_traits>
-
 #include "kernels.h"
 #include "ptx.cuh"
+#include "wgmma.cuh"
 
 namespace uv {
 
-// The tile width BN is a RUN-TIME value (multiple of 16, 32..256; multiple of 64 when B is MN-major): the host picks it per
-// launch so that the tile count fills the 148 SMs with as little wave quantisation as possible.  Stage and TMEM strides are
-// sized for the maximum (256).
-// Operand ring: kRingBytes of shared memory cut into as many stages as the run-time tile width allows (a stage = the 16 KB A tile
-// + BN x 128 B of B, or half of that B in CTA-pair mode where each CTA stages only its half), at most kMaxStages.  The TMA round
-// trip under load is ~1.5 us, so the mainloop needs that many k-blocks in flight to keep the tensor pipe fed.
+// The tile width BN is a RUN-TIME value (multiple of 16, 16..256; multiple of 64 when B is MN-major, of 128 for MN-major B in
+// clusters): the host picks it per launch so that the tile count fills the SMs with as little wave quantisation as possible.
+// Operand ring: kRingBytes of shared memory cut into as many stages as the tile width allows (a stage = the 16 KB A tile + BN x
+// 128 B of B), at most kMaxStages.
 template <int CL>
 struct GemmCfg {
   static constexpr int kMaxStages = 8;
-  static constexpr int kABytes = GEMM_BM * 128;          // 128 rows x 64 x 2 B
+  static constexpr int kABytes = GEMM_BM * 128;                 // 128 rows x 64 x 2 B
   static constexpr int kRingBytes = 4 * (kABytes + 256 * 128);  // 192 KB
-  static constexpr int kEpiFloats = 8 * 128;              // per-epilogue-warp bias slice (<= 128 columns per warp)
+  static constexpr int kEpiStride = 36;                         // floats per staged accumulator row (32 columns + 4 pad)
+  static constexpr int kEpiFloats = 2 * 64 * kEpiStride;        // one 64 x 32 staging tile per consumer warpgroup
   static constexpr int kSmemBytes = 1024 /*align slack*/ + kRingBytes + kEpiFloats * 4 + 256;
-  static constexpr uint32_t kTmemCols = 512;              // two accumulator stages of up to 256 fp32 columns
-  static constexpr int kAccStride = 256;
-  __host__ __device__ static constexpr int stage_bytes(int bn) { return kABytes + (bn / CL) * 128; }  // multiple of 1024 (bn % 16 == 0, % 32 for pairs)
+  __host__ __device__ static constexpr int stage_bytes(int bn) { return kABytes + bn * 128; }  // multiple of 1024 (bn % 16 == 0)
   __host__ __device__ static constexpr int num_stages(int bn) {
     return kRingBytes / stage_bytes(bn) < kMaxStages ? kRingBytes / stage_bytes(bn) : kMaxStages;
   }
 };
 
+constexpr int kGemmThreads = 384;  // two consumer warpgroups + the producer warpgroup
+
 struct TileInfo {
   int p, m_blk, n_blk, kb0, kb1, split;
 };
 
-// CL = 1: `t` is this CTA's tile index.  CL = 2 (CTA pairs, tcgen05 cta_group::2): `t` indexes a 256-row PAIR tile made of two
-// vertically adjacent 128-row tiles (m_blk = 2*pair + rank, same n_blk); the leader CTA (rank 0) issues one M=256 MMA for both,
-// each CTA stages its own A rows and HALF of the B rows (32 KB instead of 48 KB per k-block through the SM's 64 B/clk L2 port -
-// the limiter of the single-CTA mainloop).  The odd tail tile of a problem is a phantom whose rows are all out of range.
+// CL = 1: `t` is this CTA's tile index.  CL = 2: `t` indexes a 256-row PAIR tile made of two vertically adjacent 128-row tiles
+// (m_blk = 2*pair + rank, same n_blk).  The odd tail tile of a problem is a phantom whose rows are all out of range.
 template <int CL>
 __device__ __forceinline__ bool decode_tile(const GemmGroup& g, int bn, int t, int rank, TileInfo& ti) {
   for (int p = 0; p < g.num; ++p) {
@@ -87,16 +85,252 @@ __device__ __forceinline__ void stamp(unsigned long long* dbg, int slot) {
   }
 }
 
+// ---- mainloop: one 64-wide k-block of the warpgroup's 64 x N tile ----
+// N is cut into wgmma widths 256 / 128 / 64 / 32 / 16 (largest first); slice [OFF, OFF + W) accumulates into acc[OFF/2 ...],
+// which keeps the register layout of one m64nN accumulator.
+template <int N, int OFF, int BF, int TA, int TB>
+__device__ __forceinline__ void mma_cols(float* acc, uint64_t da, uint64_t db, uint32_t scale_d) {
+  constexpr int W = N >= 256 ? 256 : N >= 128 ? 128 : N >= 64 ? 64 : N >= 32 ? 32 : 16;
+  WG<W, BF>::template ss<TA, TB>(acc + OFF / 2, da, db, scale_d);
+  if constexpr (N > W) {
+    // next slice of B: K-major rows are 128 B apart; MN-major 64-wide blocks 8 KB apart (W is then a multiple of 64)
+    constexpr uint32_t adv = TB ? (W / 64) * 8192 / 16 : W * 128 / 16;
+    mma_cols<N - W, OFF + W, BF, TA, TB>(acc, da, db + adv, scale_d);
+  }
+}
+template <int N, int BF, int TA, int TB>
+__device__ __forceinline__ void mma_kblock(float* acc, uint64_t da, uint64_t db, uint32_t a_step, uint32_t b_step, bool acc_in) {
+#pragma unroll
+  for (int k = 0; k < GEMM_BK / 16; ++k) mma_cols<N, 0, BF, TA, TB>(acc, da + k * a_step, db + k * b_step, (acc_in || k > 0) ? 1u : 0u);
+}
+template <int N>
+__device__ __forceinline__ void mma_kblock_n(float* acc, int bf, int a_mn, int b_mn, uint64_t da, uint64_t db, uint32_t a_step,
+                                             uint32_t b_step, bool acc_in) {
+  if constexpr (N % 64 == 0) {
+    if (b_mn) {
+      if (bf) {
+        if (a_mn) mma_kblock<N, 1, 1, 1>(acc, da, db, a_step, b_step, acc_in);
+        else mma_kblock<N, 1, 0, 1>(acc, da, db, a_step, b_step, acc_in);
+      } else {
+        if (a_mn) mma_kblock<N, 0, 1, 1>(acc, da, db, a_step, b_step, acc_in);
+        else mma_kblock<N, 0, 0, 1>(acc, da, db, a_step, b_step, acc_in);
+      }
+      return;
+    }
+  }
+  if (bf) {
+    if (a_mn) mma_kblock<N, 1, 1, 0>(acc, da, db, a_step, b_step, acc_in);
+    else mma_kblock<N, 1, 0, 0>(acc, da, db, a_step, b_step, acc_in);
+  } else {
+    if (a_mn) mma_kblock<N, 0, 1, 0>(acc, da, db, a_step, b_step, acc_in);
+    else mma_kblock<N, 0, 0, 0>(acc, da, db, a_step, b_step, acc_in);
+  }
+}
+__device__ __forceinline__ void mma_kblock_bn(int bn, float* acc, int bf, int a_mn, int b_mn, uint64_t da, uint64_t db,
+                                              uint32_t a_step, uint32_t b_step, bool acc_in) {
+  switch (bn >> 4) {
+#define UV_BN_CASE(k) \
+  case k: mma_kblock_n<16 * k>(acc, bf, a_mn, b_mn, da, db, a_step, b_step, acc_in); break;
+    UV_BN_CASE(1) UV_BN_CASE(2) UV_BN_CASE(3) UV_BN_CASE(4) UV_BN_CASE(5) UV_BN_CASE(6) UV_BN_CASE(7) UV_BN_CASE(8)
+    UV_BN_CASE(9) UV_BN_CASE(10) UV_BN_CASE(11) UV_BN_CASE(12) UV_BN_CASE(13) UV_BN_CASE(14) UV_BN_CASE(15) UV_BN_CASE(16)
+#undef UV_BN_CASE
+    default: break;
+  }
+}
+
+// ---- epilogue of one 16-column step of one row ----
+struct EpiRow {
+  bool valid;
+  float rsc;
+  const float* resid_row;
+  const float* aux_row;
+  const uint16_t* mask_row;
+  const float* add_row;
+  float* o32_row;
+  float* o32i_row;
+  uint16_t* o16_row;
+  uint16_t* o16p_row;
+  float* pre_row;
+  uint16_t* dact_row;
+};
+
+__device__ __forceinline__ void ld16f(const float* p, float (&v)[16]) {
+#pragma unroll
+  for (int q = 0; q < 4; ++q) {
+    const float4 t4 = reinterpret_cast<const float4*>(p)[q];
+    v[4 * q] = t4.x; v[4 * q + 1] = t4.y; v[4 * q + 2] = t4.z; v[4 * q + 3] = t4.w;
+  }
+}
+
 // FULL = false drops the training-only epilogue options at compile time (pre-activation save, aux / mask multiplies, atomic and
-// strided fp32 stores, second fp32 output, column sums, scalar fallback): the forward's step loop then fits the instruction
-// cache (the all-options loop measured ~2x slower per step for the same work).  The host picks the variant per launch.
+// strided fp32 stores, second fp32 output, column sums, scalar fallback); the host picks the variant per launch.
+// v: accumulator + bias of columns [n0, n0 + 16) of this thread's row.  n0 is warp-uniform (column sums use the whole warp).
+template <bool FULL>
+__device__ __forceinline__ void epi_step(const GemmProblem& pr, const EpiRow& r, float (&v)[16], int n0, int fmt, int lane) {
+  const int pN = pr.N;
+  const int act = pr.act;
+  const int ofmt = pr.out_fmt < 0 ? fmt : pr.out_fmt;
+  const bool vec = FULL ? pr.vec_ok != 0 : true;  // the lean variant is only launched when every access can be vectorised
+  const bool atomic = (pr.accumulate != 0) || (pr.ksplit > 1);
+  const bool mask_mul = FULL && pr.mask_mul != 0;
+  const float rsc = r.rsc;
+  if (FULL && r.pre_row != nullptr && r.valid) {  // training: keep the pre-activation (needs N % 4 == 0, checked on the host)
+    if (vec) {  // vec_ok implies N % 16 == 0: the whole step is in range
+      st_global_256f(r.pre_row + n0, v[0], v[1], v[2], v[3], v[4], v[5], v[6], v[7]);
+      st_global_256f(r.pre_row + n0 + 8, v[8], v[9], v[10], v[11], v[12], v[13], v[14], v[15]);
+    } else {
+#pragma unroll
+      for (int q = 0; q < 4; ++q)
+        if (n0 + 4 * q < pN)
+          *reinterpret_cast<float4*>(r.pre_row + n0 + 4 * q) = make_float4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]);
+    }
+  }
+  if (FULL && act == ACT_GELU && r.dact_row != nullptr) {  // training forward: activation and its derivative in one pass
+    float dg[16];
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+      float gj;
+      gelu_erf_both(v[j], gj, dg[j]);
+      v[j] = gj * rsc;
+    }
+    if (r.valid) {
+      if (vec) {
+        uint32_t w8[8];
+#pragma unroll
+        for (int q = 0; q < 8; ++q) w8[q] = cvt16x2(dg[2 * q], dg[2 * q + 1], ofmt);
+        st_global_256(r.dact_row + n0, w8);
+      } else {
+#pragma unroll
+        for (int j = 0; j < 16; ++j)
+          if (n0 + j < pN) r.dact_row[n0 + j] = cvt16(dg[j], ofmt);
+      }
+    }
+  } else if (act == ACT_GELU) {
+#pragma unroll
+    for (int j = 0; j < 16; ++j) v[j] = gelu_erf(v[j]) * rsc;
+  } else if (act == ACT_RELU) {
+#pragma unroll
+    for (int j = 0; j < 16; ++j) v[j] = fmaxf(v[j], 0.f) * rsc;
+  } else {
+#pragma unroll
+    for (int j = 0; j < 16; ++j) v[j] *= rsc;
+  }
+  if (vec) {
+    if (r.valid) {
+      if (r.resid_row != nullptr) {
+        float rv[16];
+        ld16f(r.resid_row + n0, rv);
+#pragma unroll
+        for (int j = 0; j < 16; ++j) v[j] += rv[j];
+      }
+      if (FULL && r.aux_row != nullptr) {
+        float av[16];
+        ld16f(r.aux_row + n0, av);
+        if (pr.aux_mode == 1) {
+#pragma unroll
+          for (int j = 0; j < 16; ++j) v[j] *= gelu_erf_grad(av[j]);
+        } else {
+#pragma unroll
+          for (int j = 0; j < 16; ++j) v[j] *= av[j];
+        }
+      }
+      if (FULL && r.mask_row != nullptr) {
+#pragma unroll
+        for (int q = 0; q < 2; ++q) {
+          const uint4 mk = reinterpret_cast<const uint4*>(r.mask_row + n0)[q];
+          const uint32_t w4[4] = {mk.x, mk.y, mk.z, mk.w};
+#pragma unroll
+          for (int e = 0; e < 4; ++e) {
+            if (mask_mul) {  // saved activation derivative (GELU'): multiply
+              v[8 * q + 2 * e] *= ld16((uint16_t)(w4[e] & 0xffff), fmt);
+              v[8 * q + 2 * e + 1] *= ld16((uint16_t)(w4[e] >> 16), fmt);
+            } else {  // ReLU mask: zero where the saved activation is <= 0
+              if (!pos16((uint16_t)(w4[e] & 0xffff))) v[8 * q + 2 * e] = 0.f;
+              if (!pos16((uint16_t)(w4[e] >> 16))) v[8 * q + 2 * e + 1] = 0.f;
+            }
+          }
+        }
+      }
+      if (r.o32_row != nullptr) {
+        if (FULL && atomic) {  // split-K / accumulate: 128-bit reductions (4x fewer L2 atomic operations than scalar REDs)
+#pragma unroll
+          for (int q = 0; q < 4; ++q)
+            red_add_f32x4(r.o32_row + n0 + 4 * q, make_float4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]));
+        } else {
+          st_global_256f(r.o32_row + n0, v[0], v[1], v[2], v[3], v[4], v[5], v[6], v[7]);
+          st_global_256f(r.o32_row + n0 + 8, v[8], v[9], v[10], v[11], v[12], v[13], v[14], v[15]);
+        }
+      }
+      if (FULL && r.o32i_row != nullptr) {
+        st_global_256f(r.o32i_row + n0, v[0], v[1], v[2], v[3], v[4], v[5], v[6], v[7]);
+        st_global_256f(r.o32i_row + n0 + 8, v[8], v[9], v[10], v[11], v[12], v[13], v[14], v[15]);
+      }
+      if (r.o16_row != nullptr) {
+        uint32_t w8[8];
+#pragma unroll
+        for (int q = 0; q < 8; ++q) w8[q] = cvt16x2(v[2 * q], v[2 * q + 1], ofmt);
+        st_global_256(r.o16_row + n0, w8);
+      }
+      if (r.o16p_row != nullptr) {
+        float p[16];
+#pragma unroll
+        for (int j = 0; j < 16; ++j) p[j] = v[j];
+        if (r.add_row != nullptr) {
+          float av[16];
+          ld16f(r.add_row + n0, av);
+#pragma unroll
+          for (int j = 0; j < 16; ++j) p[j] += av[j];
+        }
+        uint32_t w8[8];
+#pragma unroll
+        for (int q = 0; q < 8; ++q) w8[q] = cvt16x2(p[2 * q], p[2 * q + 1], ofmt);
+        st_global_256(r.o16p_row + n0, w8);
+      }
+    } else {
+#pragma unroll
+      for (int j = 0; j < 16; ++j) v[j] = 0.f;  // invalid rows contribute nothing to the column sums
+    }
+  } else if constexpr (FULL) {
+    // unaligned leading dimensions / ragged N (e.g. the [d, 2818] projector weight gradient, strided conv wgrad): scalar accesses
+    const int cs32 = pr.cs32 > 1 ? pr.cs32 : 1;
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+      const int n = n0 + j;
+      float x = v[j];
+      if (r.valid && n < pN) {
+        if (r.resid_row != nullptr) x += r.resid_row[n];
+        if (r.aux_row != nullptr) x *= (pr.aux_mode == 1) ? gelu_erf_grad(r.aux_row[n]) : r.aux_row[n];
+        if (r.mask_row != nullptr) {
+          if (mask_mul) x *= ld16(r.mask_row[n], fmt);
+          else if (!pos16(r.mask_row[n])) x = 0.f;
+        }
+        if (r.o32_row != nullptr) {
+          float* dst = r.o32_row + (size_t)n * cs32;
+          if (atomic) atomicAdd(dst, x);
+          else *dst = x;
+        }
+        if (r.o32i_row != nullptr) r.o32i_row[n] = x;
+        if (r.o16_row != nullptr) r.o16_row[n] = cvt16(x, ofmt);
+        if (r.o16p_row != nullptr) r.o16p_row[n] = cvt16(x + (r.add_row ? r.add_row[n] : 0.f), ofmt);
+      } else {
+        x = 0.f;
+      }
+      v[j] = x;
+    }
+  }
+  if (FULL && pr.colsum != nullptr) {  // warp-uniform: column sums over this warp's 32 rows, one atomic per column
+    const float sj = warp_colsum16(v, lane);  // 16 shuffles; lane l holds column l & 15
+    if (lane < 16 && n0 + lane < pN) atomicAdd(pr.colsum + n0 + lane, sj * pr.colsum_scale);
+  }
+}
+
 template <int CL, bool FULL>
-__global__ void __launch_bounds__(384, 1) gemm_tcgen05_kernel(const __grid_constant__ GemmGroup g) {
+__global__ void __launch_bounds__(kGemmThreads, 1) gemm_wgmma_kernel(const __grid_constant__ GemmGroup g) {
   using Cfg = GemmCfg<CL>;
   const int BN = g.bn;
   const int kStageBytes = Cfg::stage_bytes(BN);
   const int kStages = Cfg::num_stages(BN);
-  const int crank = (CL > 1) ? (int)cluster_ctarank() : 0;          // rank inside the CTA pair
+  const int crank = (CL > 1) ? (int)cluster_ctarank() : 0;  // rank inside the cluster
   const int tile0 = (CL > 1) ? (int)(blockIdx.x / CL) : (int)blockIdx.x;
   const int tstep = (int)(gridDim.x / CL);
   extern __shared__ __align__(1024) uint8_t smem_raw[];
@@ -107,58 +341,39 @@ __global__ void __launch_bounds__(384, 1) gemm_tcgen05_kernel(const __grid_const
   uint8_t* stage_base = smem;
   float* epi_buf = reinterpret_cast<float*>(smem + Cfg::kRingBytes);
   uint64_t* bars = reinterpret_cast<uint64_t*>(epi_buf + Cfg::kEpiFloats);
-  uint64_t* full_bar = bars;                           // [kMaxStages]
-  uint64_t* empty_bar = bars + Cfg::kMaxStages;        // [kMaxStages]
-  uint64_t* tmem_full = bars + 2 * Cfg::kMaxStages;    // [2]
-  uint64_t* tmem_empty = tmem_full + 2;             // [2]
-  uint32_t* tmem_holder = reinterpret_cast<uint32_t*>(tmem_empty + 2);
+  uint64_t* full_bar = bars;                     // [kMaxStages]
+  uint64_t* empty_bar = bars + Cfg::kMaxStages;  // [kMaxStages]
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7;
   if (threadIdx.x == 0) stamp(g.dbg, 0);  // kernel entry (profiling buffer only; never an output of a preceding kernel)
 
-  if (warp == 0 && lane == 0) {
+  if (warp == 8 && lane == 0) {
     for (int p = 0; p < g.num; ++p) {
       tma_prefetch_desc(&g.p[p].tm_a);
       tma_prefetch_desc(&g.p[p].tm_b);
     }
   }
-  if (warp == 1 && lane == 0) {
+  if (warp == 0 && lane == 0) {
     for (int s = 0; s < kStages; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);  // CL = 2: the leader's multicast commit arrives here in both CTAs
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&tmem_full[s], 1);
-      mbar_init(&tmem_empty[s], 8 * CL);  // CL = 2: the leader's barrier collects the epilogue warps of both CTAs
+      mbar_init(&empty_bar[s], 2 * CL);  // both consumer warpgroups of every CTA the stage's B tile is multicast to
     }
     fence_barrier_init();
   }
-  if (warp == 2) {
-    if (CL == 1) tmem_alloc<Cfg::kTmemCols>(tmem_holder);
-    else tmem_alloc_2sm<Cfg::kTmemCols>(tmem_holder);
-  }
-  tc_fence_before();
   __syncthreads();
   if (CL > 1) cluster_sync_all();  // the peer's barriers are initialised before any multicast can reach them
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_holder;
-  // Only now (this CTA owns its TMEM columns) may the next grid be scheduled: a dependent CTA that grabbed TMEM first and
-  // then blocked in griddepcontrol.wait could starve a CTA of this grid sharing its SM.
   pdl_launch_dependents();
-  pdl_wait();  // barriers, TMEM and tensor-map prefetch happened under the previous kernel's tail; its results are visible from here
-  if (threadIdx.x == 0) stamp(g.dbg, 1);  // setup done (barriers, TMEM)
+  pdl_wait();  // barriers and tensor-map prefetch happened under the previous kernel's tail; its results are visible from here
+  if (threadIdx.x == 0) stamp(g.dbg, 1);  // setup done
 
-  if (warp == 0) {
-    // ======================================= TMA producer =======================================
-    // The whole warp walks the schedule convergently and ONE elected lane issues (elect.sync): inside a plain `if (lane == 0)`
-    // region ptxas cannot prove the TMA / MMA operands warp-uniform and wraps every UTMALDG / UTCHMMA / UTCBAR in an
-    // ELECT + BRA.U.ANY "waterfall" loop (round 2: -10 % GEMM time).  What paces the mainloop now is tcgen05.commit: two commits are
-    // at least ~615 SM cycles apart (tools/probes/mma_probe.cu), so a 64-wide k-block (4 MMAs, one commit to free its stage)
-    // costs ~0.33 us whatever the tile width.  Releasing stages in pairs with one commit was tried and measured SLOWER here
-    // (profiles/README.md, r2c/r2d): with a 192 KB ring of 42-48 KB stages only two groups fit, and the commit -> refill -> landed
-    // round trip (~1 us) then stalls the MMA warp; the same holds for requesting weight tiles before griddepcontrol.wait.
-    {
+  if (wg == 2) {
+    setmaxnreg_dec<40>();
+    if (warp == 8) {
+      // ======================================= TMA producer =======================================
+      // The whole warp walks the schedule convergently and ONE elected lane issues (elect.sync), so that the TMA operands are
+      // provably warp-uniform.
       int stage = 0;
       uint32_t phase = 0;
       TileInfo ti;
@@ -176,8 +391,7 @@ __global__ void __launch_bounds__(384, 1) gemm_tcgen05_kernel(const __grid_const
           const int a1 = pr.ca.base1 + m0 * pr.ca.mn1s + tap * pr.ca.tap1 + kk * pr.ca.k1s;
           const int b0 = pr.cb.base0 + n0 * pr.cb.mn0s + tap * pr.cb.tap0 + kk * pr.cb.k0s;
           const int b1 = pr.cb.base1 + n0 * pr.cb.mn1s + tap * pr.cb.tap1 + kk * pr.cb.k1s;
-          if (!elect_one()) {
-          } else if (CL == 1) {
+          if (elect_one()) {
             mbar_arrive_expect_tx(&full_bar[stage], Cfg::kABytes + BN * 128);
             if (!pr.a_mn) {
               tma_load_2d(sa, &pr.tm_a, &full_bar[stage], a0, a1);
@@ -185,29 +399,17 @@ __global__ void __launch_bounds__(384, 1) gemm_tcgen05_kernel(const __grid_const
 #pragma unroll
               for (int j = 0; j < GEMM_BM / 64; ++j) tma_load_2d(sa + j * 8192, &pr.tm_a, &full_bar[stage], a0 + 64 * j, a1);
             }
-            if (!pr.b_mn) {
-              tma_load_2d(sb, &pr.tm_b, &full_bar[stage], b0, b1);
-            } else if (pr.b_3d) {
-              tma_load_3d(sb, &pr.tm_b, &full_bar[stage], 0, b1, b0 >> 6);  // all BN/64 blocks of the k-block in one TMA operation
+            if (CL == 1) {
+              if (!pr.b_mn) {
+                tma_load_2d(sb, &pr.tm_b, &full_bar[stage], b0, b1);
+              } else if (pr.b_3d) {
+                tma_load_3d(sb, &pr.tm_b, &full_bar[stage], 0, b1, b0 >> 6);  // all BN/64 blocks of the k-block in one TMA operation
+              } else {
+                for (int j = 0; j < BN / 64; ++j) tma_load_2d(sb + j * 8192, &pr.tm_b, &full_bar[stage], b0 + 64 * j, b1);
+              }
             } else {
-              for (int j = 0; j < BN / 64; ++j) tma_load_2d(sb + j * 8192, &pr.tm_b, &full_bar[stage], b0 + 64 * j, b1);
-            }
-          } else {
-            // both CTAs credit the LEADER's barrier: it expects the A tile + half B tile of each CTA
-            const uint32_t lead_bar = mapa_shared(smem_u32(&full_bar[stage]), 0);
-            if (crank == 0) mbar_arrive_expect_tx(&full_bar[stage], 2 * Cfg::kABytes + BN * 128);
-            if (!pr.a_mn) {
-              tma_load_2d_2sm(sa, &pr.tm_a, lead_bar, a0, a1);
-            } else {
-#pragma unroll
-              for (int j = 0; j < GEMM_BM / 64; ++j) tma_load_2d_2sm(sa + j * 8192, &pr.tm_a, lead_bar, a0 + 64 * j, a1);
-            }
-            if (!pr.b_mn) {
-              const int hr = BN / 2;  // tensor-map box = BN/2 rows: this CTA's half of the B tile, at the same smem offset in both CTAs
-              tma_load_2d_2sm(sb, &pr.tm_b, lead_bar, b0, b1 + crank * hr);
-            } else {
-              const int nb = BN / 128;  // 64-wide N blocks per CTA
-              for (int j = 0; j < nb; ++j) tma_load_2d_2sm(sb + j * 8192, &pr.tm_b, lead_bar, b0 + 64 * (crank * nb + j), b1);
+              const int hr = BN / 2;  // tensor-map box = BN/2 rows: this CTA's half of the B tile, multicast to both CTAs
+              tma_load_2d_mc(sb + crank * hr * 128, &pr.tm_b, &full_bar[stage], b0, b1 + crank * hr, (uint16_t)0x3);
             }
           }
           __syncwarp();
@@ -219,543 +421,120 @@ __global__ void __launch_bounds__(384, 1) gemm_tcgen05_kernel(const __grid_const
       }
       if (lane == 0) stamp(g.dbg, 2);  // all TMA loads issued
     }
-  } else if (warp == 1) {
-    // ======================================== MMA issuer ========================================
-    if (CL == 1 || crank == 0) {  // CTA pair: the leader issues for both; convergent warp, one elected lane issues
-      int stage = 0;
-      uint32_t phase = 0;
-      int as = 0;
-      uint32_t aphase = 0;
-      TileInfo ti;
-      for (int t = tile0; decode_tile<CL>(g, BN, t, crank, ti); t += tstep) {
-        const GemmProblem& pr = g.p[ti.p];
-        const uint32_t idesc = make_idesc_f16_ab(GEMM_BM * CL, BN, pr.a_fmt < 0 ? g.fmt : pr.a_fmt, pr.b_fmt < 0 ? g.fmt : pr.b_fmt, pr.a_mn, pr.b_mn);
-        mbar_wait(&tmem_empty[as], aphase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + as * Cfg::kAccStride;
-        // descriptor = constant high part (layout, LBO/SBO) + start address; one k-step of 16 elements advances the address by
-        // 32 B inside the 128 B swizzle span (K-major) or by two 1024 B swizzle atoms (MN-major), in 16-byte units
-        const uint64_t da_hi = pr.a_mn ? make_smem_desc_sw128(0, 8192, 1024) : make_smem_desc_sw128(0, 16, 1024);
-        const uint64_t db_hi = pr.b_mn ? make_smem_desc_sw128(0, 8192, 1024) : make_smem_desc_sw128(0, 16, 1024);
-        const uint32_t a_step = pr.a_mn ? 128u : 2u, b_step = pr.b_mn ? 128u : 2u;
-        for (int kb = ti.kb0; kb < ti.kb1; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          if (lane == 0 && kb == ti.kb0 && t == tile0) stamp(g.dbg, 3);  // first operand stage landed
-          tc_fence_after();
-          const uint32_t sa = smem_u32(stage_base + stage * kStageBytes);
-          const uint64_t da = da_hi + (uint64_t)(sa >> 4);
-          const uint64_t db = db_hi + (uint64_t)((sa + Cfg::kABytes) >> 4);
-          if (elect_one()) {
-#pragma unroll
-            for (int k = 0; k < GEMM_BK / 16; ++k) {
-              if (CL == 1) umma_f16_ss(d_tmem, da + k * a_step, db + k * b_step, idesc, (kb > ti.kb0 || k > 0) ? 1u : 0u);
-              else umma_f16_ss_2sm(d_tmem, da + k * a_step, db + k * b_step, idesc, (kb > ti.kb0 || k > 0) ? 1u : 0u);
-            }
-            if (CL == 1) umma_commit(&empty_bar[stage]);  // frees the smem slot when these MMAs retire
-            else umma_commit_2sm(&empty_bar[stage], (uint16_t)0x3);  // ... in both CTAs of the pair
-          }
-          __syncwarp();
-          if (++stage == kStages) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-        if (elect_one()) {
-          if (CL == 1) umma_commit(&tmem_full[as]);  // accumulator complete -> epilogue
-          else umma_commit_2sm(&tmem_full[as], (uint16_t)0x3);
-        }
-        __syncwarp();
-        if (lane == 0) stamp(g.dbg, 4);  // last MMA of the tile issued
-        if (++as == 2) {
-          as = 0;
-          aphase ^= 1;
-        }
-      }
-    }
-  } else if (warp >= 4) {
-    // ========================================= epilogue =========================================
-    // 8 warps: warp w may only touch TMEM lanes [32*(w%4), +32); the two warps of a lane quarter split the columns.
-    // thread = output row: every thread owns 16 consecutive columns per step = 32 B (16-bit) / 64 B (fp32) of one row,
-    // i.e. whole 32-byte sectors, so loads and stores go straight from/to registers with 128-bit accesses.
-    const int wq = warp & 3;
-    const int half = (warp - 4) >> 2;
-    const int ew = warp - 4;
-    float* bias_s = epi_buf + ew * 128;
+  } else {
+    setmaxnreg_inc<232>();
+    // ======================================= consumers =======================================
+    const int cw = wg;                       // rows [64 cw, 64 cw + 64) of the tile
+    const int tid = threadIdx.x & 127;
+    const int fr = 16 * (tid >> 5) + (lane >> 2);  // accumulator fragment: rows fr, fr + 8; columns 8 i + fc, + 1
+    const int fc = 2 * (lane & 3);
+    const int erow = tid & 63, ehalf = tid >> 6;  // epilogue: thread = row erow, columns [16 ehalf, +16) of each 32-column chunk
+    float* ebuf = epi_buf + cw * 64 * Cfg::kEpiStride;
     const int fmt = g.fmt;
-    int as = 0;
-    uint32_t aphase = 0;
+    float acc[128];
+#pragma unroll
+    for (int i = 0; i < 128; ++i) acc[i] = 0.f;
+    int stage = 0;
+    uint32_t phase = 0;
     TileInfo ti;
+    auto release = [&](int s) {  // this warpgroup is done with stage s (in every CTA the stage was multicast from)
+      if (tid == 0) {
+        mbar_arrive(&empty_bar[s]);
+        if (CL > 1) mbar_arrive_cluster(mapa_shared(smem_u32(&empty_bar[s]), (uint32_t)(crank ^ 1)));
+      }
+    };
+    bool first_tile = true;
     for (int t = tile0; decode_tile<CL>(g, BN, t, crank, ti); t += tstep) {
       const GemmProblem& pr = g.p[ti.p];
-      // hoist the problem description into registers (the struct lives in the constant bank)
-      const int pM = pr.M, pN = pr.N, rps_in = pr.rps_in;
-      const int act = pr.act;
-      const float* __restrict__ bias = (ti.split == 0) ? pr.bias : nullptr;
-      const float* __restrict__ resid = pr.resid;
-      const float* __restrict__ addtab = pr.addtab;
-      float* __restrict__ out32 = pr.out32;
-      float* __restrict__ out32_id = pr.out32_id;
-      uint16_t* __restrict__ out16 = pr.out16;
-      uint16_t* __restrict__ out16p = pr.out16p;
-      const bool atomic = (pr.accumulate != 0) || (pr.ksplit > 1);
-      const bool vec = pr.vec_ok != 0;
-      const bool v256 = FULL ? (pr.vec_ok == 2) : true;  // the lean variant is only launched when every access can be 256-bit
-      const int ofmt = pr.out_fmt < 0 ? fmt : pr.out_fmt;
-      const float* __restrict__ aux32 = pr.aux32;
-      const int aux_mode = pr.aux_mode;
-      const uint16_t* __restrict__ mask16 = pr.mask16;
-      float* __restrict__ colsum = pr.colsum;
-      const int cs32 = pr.cs32 > 1 ? pr.cs32 : 1;
-      float* __restrict__ pre32 = pr.pre32;
-      uint16_t* __restrict__ dact16 = FULL ? pr.dact16 : nullptr;
-      const bool mask_mul = FULL && pr.mask_mul != 0;
+      const int bf = pr.a_fmt < 0 ? fmt : pr.a_fmt;  // both operands share it (checked on the host)
+      // descriptor = constant high part (layout, LBO/SBO) + start address; one k-step of 16 elements advances the address by
+      // 32 B inside the 128 B swizzle span (K-major) or by two 1024 B swizzle atoms (MN-major), in 16-byte units
+      const uint64_t da_hi = pr.a_mn ? make_smem_desc_sw128(0, 8192, 1024) : make_smem_desc_sw128(0, 16, 1024);
+      const uint64_t db_hi = pr.b_mn ? make_smem_desc_sw128(0, 8192, 1024) : make_smem_desc_sw128(0, 16, 1024);
+      const uint32_t a_step = pr.a_mn ? 128u : 2u, b_step = pr.b_mn ? 128u : 2u;
+      int prev = -1;
+      for (int kb = ti.kb0; kb < ti.kb1; ++kb) {
+        mbar_wait(&full_bar[stage], phase);
+        if (tid == 0 && cw == 0 && kb == ti.kb0 && first_tile) stamp(g.dbg, 3);  // first operand stage landed
+        const uint32_t sa = smem_u32(stage_base + stage * kStageBytes);
+        // this warpgroup's 64 rows of A: K-major rows 64 cw.. (64 x 128 B); MN-major the cw-th 64-wide M block (8 KB each)
+        const uint64_t da = da_hi + (uint64_t)((sa + cw * 8192) >> 4);
+        const uint64_t db = db_hi + (uint64_t)((sa + Cfg::kABytes) >> 4);
+        wgmma_fence();
+        mma_kblock_bn(BN, acc, bf, pr.a_mn, pr.b_mn, da, db, a_step, b_step, kb > ti.kb0);
+        wgmma_commit();
+        wgmma_wait<1>();  // the previous k-block's MMAs have retired: its stage can be refilled
+        if (prev >= 0) release(prev);
+        prev = stage;
+        if (++stage == kStages) {
+          stage = 0;
+          phase ^= 1;
+        }
+      }
+      wgmma_wait<0>();
+#pragma unroll
+      for (int i = 0; i < 128; ++i) reg_fence(acc[i]);
+      if (prev >= 0) release(prev);
+      if (tid == 0 && cw == 0) stamp(g.dbg, 4);  // last MMA of the tile retired
+      first_tile = false;
 
-      const int m0 = ti.m_blk * GEMM_BM + wq * 32;
-      // the BN/16 column steps of the tile are split between the two warps of this lane quarter (first warp gets the extra one)
-      const int tot_steps = BN / 16;
-      const int my_first = half ? (tot_steps + 1) / 2 : 0;
-      const int my_steps = half ? tot_steps / 2 : (tot_steps + 1) / 2;
-      const int n_base = ti.n_blk * BN + my_first * 16;
-      // ---- this thread's row ----
-      const int m = m0 + lane;
+      // ========================================= epilogue =========================================
+      const int pM = pr.M, pN = pr.N, rps_in = pr.rps_in;
+      const int m = ti.m_blk * GEMM_BM + cw * 64 + erow;
       int b = 0, l = m;
       if (rps_in > 0) {
         b = m / rps_in;
         l = m - b * rps_in;
       }
       const bool is_sep = (rps_in > 0) && (l == rps_in - 1);
-      const bool valid = (m < pM) && !(pr.skip_sep && is_sep);
-      float rsc = pr.alpha;
-      if (pr.row_scale != nullptr && m < pM) rsc *= pr.row_scale[b];
-      if (pr.zero_sep && is_sep) rsc = 0.f;
+      EpiRow r;
+      r.valid = (m < pM) && !(pr.skip_sep && is_sep);
+      r.rsc = pr.alpha;
+      if (pr.row_scale != nullptr && m < pM) r.rsc *= pr.row_scale[b];
+      if (pr.zero_sep && is_sep) r.rsc = 0.f;
       const size_t orow = (size_t)((rps_in > 0 ? b * pr.rps_out + l : m) + pr.row_off);
-      const float* resid_row = resid ? resid + orow * pr.ld_resid : nullptr;
-      const float* aux_row = aux32 ? aux32 + orow * pr.ld_aux : nullptr;
-      const uint16_t* mask_row = mask16 ? mask16 + orow * pr.ld_mask : nullptr;
-      const float* add_row = addtab ? addtab + (size_t)m * pr.ld_addtab : nullptr;
-      float* o32_row = out32 ? out32 + orow * pr.ld32 : nullptr;
-      float* o32i_row = out32_id ? out32_id + (size_t)m * pr.ld32_id : nullptr;
-      uint16_t* o16_row = out16 ? out16 + orow * pr.ld16 : nullptr;
-      uint16_t* o16p_row = out16p ? out16p + orow * pr.ld16 : nullptr;
-      float* pre_row = pre32 ? pre32 + orow * pr.ld_pre : nullptr;
-      uint16_t* dact_row = dact16 ? dact16 + orow * pr.ld_dact : nullptr;
-
-      // bias slice of this warp's columns -> smem (broadcast reads in the column loop)
-      __syncwarp();
-      for (int j = lane; j < my_steps * 16; j += 32) {
-        const int n = n_base + j;
-        bias_s[j] = (bias != nullptr && n < pN) ? __ldg(bias + n) : 0.f;
-      }
-      __syncwarp();
-
-      mbar_wait(&tmem_full[as], aphase);
-      if (ew == 0 && lane == 0) stamp(g.dbg, 5);  // accumulator ready
-      tc_fence_after();
-      const uint32_t t_addr = tmem_base + ((uint32_t)(wq * 32) << 16) + as * Cfg::kAccStride + my_first * 16;
-
-      // number of 16-column steps this warp owns in this tile (warp-uniform)
-      int nsteps = (pN - n_base + 15) / 16;
-      nsteps = nsteps < 0 ? 0 : (nsteps > my_steps ? my_steps : nsteps);
-      // the fp32 side input of a step (residual, or the aux multiplier when there is no residual) is fetched one step ahead
-      const float* side_row = resid_row != nullptr ? resid_row : ((FULL && aux_row != nullptr) ? aux_row : add_row);
-      const bool aux_prefetched = FULL && resid_row == nullptr && aux_row != nullptr;
-      const bool add_prefetched = resid_row == nullptr && !(FULL && aux_row != nullptr) && add_row != nullptr;
-      const bool load_resid = vec && valid && (side_row != nullptr);
-      uint32_t r[16];
-      float rv_next[16];
-      uint4 mk_next[2] = {make_uint4(0, 0, 0, 0), make_uint4(0, 0, 0, 0)};
-      const bool load_mask = FULL && vec && valid && (mask_row != nullptr);
-      // software pipeline: the TMEM load and the residual loads of step c+1 are in flight while step c is processed
-      if (nsteps > 0) {
-        tmem_ld_32x32b_x16(t_addr, r);
-        if (load_mask) {
-          mk_next[0] = *reinterpret_cast<const uint4*>(mask_row + n_base);
-          mk_next[1] = *reinterpret_cast<const uint4*>(mask_row + n_base + 8);
-        }
-        if (load_resid) {
-          if (v256) {
-            ld_global_256f(side_row + n_base, rv_next);
-            ld_global_256f(side_row + n_base + 8, rv_next + 8);
-          } else {
+      r.resid_row = pr.resid ? pr.resid + orow * pr.ld_resid : nullptr;
+      r.aux_row = (FULL && pr.aux32) ? pr.aux32 + orow * pr.ld_aux : nullptr;
+      r.mask_row = (FULL && pr.mask16) ? pr.mask16 + orow * pr.ld_mask : nullptr;
+      r.add_row = pr.addtab ? pr.addtab + (size_t)m * pr.ld_addtab : nullptr;
+      r.o32_row = pr.out32 ? pr.out32 + orow * pr.ld32 : nullptr;
+      r.o32i_row = (FULL && pr.out32_id) ? pr.out32_id + (size_t)m * pr.ld32_id : nullptr;
+      r.o16_row = pr.out16 ? pr.out16 + orow * pr.ld16 : nullptr;
+      r.o16p_row = pr.out16p ? pr.out16p + orow * pr.ld16 : nullptr;
+      r.pre_row = (FULL && pr.pre32) ? pr.pre32 + orow * pr.ld_pre : nullptr;
+      r.dact_row = (FULL && pr.dact16) ? pr.dact16 + orow * pr.ld_dact : nullptr;
+      const float* __restrict__ bias = (ti.split == 0) ? pr.bias : nullptr;
+      const int nt0 = ti.n_blk * BN;
 #pragma unroll
-            for (int q = 0; q < 4; ++q) {
-              const float4 t4 = *reinterpret_cast<const float4*>(side_row + n_base + 4 * q);
-              rv_next[4 * q] = t4.x; rv_next[4 * q + 1] = t4.y; rv_next[4 * q + 2] = t4.z; rv_next[4 * q + 3] = t4.w;
-            }
+      for (int cc = 0; cc < 8; ++cc) {
+        if (cc * 32 < BN && nt0 + cc * 32 < pN) {  // warpgroup-uniform
+#pragma unroll
+          for (int ii = 0; ii < 4; ++ii) {
+            const int i = 4 * cc + ii;
+            *reinterpret_cast<float2*>(ebuf + fr * Cfg::kEpiStride + 8 * ii + fc) = make_float2(acc[4 * i], acc[4 * i + 1]);
+            *reinterpret_cast<float2*>(ebuf + (fr + 8) * Cfg::kEpiStride + 8 * ii + fc) = make_float2(acc[4 * i + 2], acc[4 * i + 3]);
           }
+          named_bar_sync(1 + cw, 128);
+          const int n0 = nt0 + cc * 32 + ehalf * 16;
+          if (cc * 32 + ehalf * 16 < BN && n0 < pN) {  // warp-uniform (a warp's rows share ehalf)
+            float v[16];
+            ld16f(ebuf + erow * Cfg::kEpiStride + ehalf * 16, v);
+            if (bias != nullptr) {
+#pragma unroll
+              for (int j = 0; j < 16; ++j) v[j] += (n0 + j < pN) ? __ldg(bias + n0 + j) : 0.f;
+            }
+            epi_step<FULL>(pr, r, v, n0, fmt, lane);
+          }
+          named_bar_sync(1 + cw, 128);
         }
       }
-      // The step loop is instantiated twice (vector / scalar accesses) so that each instance's body stays small: the epilogue is
-      // instruction-fetch sensitive (8 warps walking a multi-KB unrolled body).
-      auto step_loop = [&](auto vec_tag) {
-      constexpr bool VEC = decltype(vec_tag)::value;
-      for (int c = 0; c < nsteps; ++c) {
-        const int n0 = n_base + c * 16;
-        tmem_ld_wait();
-        float v[16], rv[16];
-#pragma unroll
-        for (int j = 0; j < 16; ++j) {
-          v[j] = __uint_as_float(r[j]) + bias_s[c * 16 + j];
-          rv[j] = rv_next[j];
-        }
-        const uint4 mk_cur[2] = {mk_next[0], mk_next[1]};
-        if (c + 1 < nsteps) {
-          tmem_ld_32x32b_x16(t_addr + (c + 1) * 16, r);
-          if (load_mask) {
-            mk_next[0] = *reinterpret_cast<const uint4*>(mask_row + n0 + 16);
-            mk_next[1] = *reinterpret_cast<const uint4*>(mask_row + n0 + 24);
-          }
-          if (load_resid) {
-            if (v256) {
-              ld_global_256f(side_row + n0 + 16, rv_next);
-              ld_global_256f(side_row + n0 + 24, rv_next + 8);
-            } else {
-#pragma unroll
-              for (int q = 0; q < 4; ++q) {
-                const float4 t4 = *reinterpret_cast<const float4*>(side_row + n0 + 16 + 4 * q);
-                rv_next[4 * q] = t4.x; rv_next[4 * q + 1] = t4.y; rv_next[4 * q + 2] = t4.z; rv_next[4 * q + 3] = t4.w;
-              }
-            }
-          }
-        }
-        if (FULL && pre_row != nullptr && valid) {  // training: keep the pre-activation (needs N % 4 == 0, checked on the host)
-          if (v256) {  // vec_ok implies N % 16 == 0: the whole step is in range
-            st_global_256f(pre_row + n0, v[0], v[1], v[2], v[3], v[4], v[5], v[6], v[7]);
-            st_global_256f(pre_row + n0 + 8, v[8], v[9], v[10], v[11], v[12], v[13], v[14], v[15]);
-          } else {
-#pragma unroll
-            for (int q = 0; q < 4; ++q)
-              if (n0 + 4 * q < pN)
-                *reinterpret_cast<float4*>(pre_row + n0 + 4 * q) = make_float4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]);
-          }
-        }
-        if (FULL && act == ACT_GELU && dact_row != nullptr) {  // training forward: activation and its derivative in one pass
-          float dg[16];
-#pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            float gj;
-            gelu_erf_both(v[j], gj, dg[j]);
-            v[j] = gj * rsc;
-          }
-          if (valid) {
-            if (v256) {
-              uint32_t w8[8];
-#pragma unroll
-              for (int q = 0; q < 8; ++q) w8[q] = cvt16x2(dg[2 * q], dg[2 * q + 1], ofmt);
-              st_global_256(dact_row + n0, w8);
-            } else {
-#pragma unroll
-              for (int j = 0; j < 16; ++j)
-                if (n0 + j < pN) dact_row[n0 + j] = cvt16(dg[j], ofmt);
-            }
-          }
-        } else if (act == ACT_GELU) {
-#pragma unroll
-          for (int j = 0; j < 16; ++j) v[j] = gelu_erf(v[j]) * rsc;
-        } else if (act == ACT_RELU) {
-#pragma unroll
-          for (int j = 0; j < 16; ++j) v[j] = fmaxf(v[j], 0.f) * rsc;
-        } else {
-#pragma unroll
-          for (int j = 0; j < 16; ++j) v[j] *= rsc;
-        }
-        if constexpr (VEC) {
-          if (valid) {
-            if (resid_row != nullptr) {
-#pragma unroll
-              for (int j = 0; j < 16; ++j) v[j] += rv[j];
-            }
-            if (FULL && aux_row != nullptr) {
-              float av[16];
-              if (aux_prefetched) {
-#pragma unroll
-                for (int j = 0; j < 16; ++j) av[j] = rv[j];
-              } else {
-#pragma unroll
-                for (int q = 0; q < 4; ++q) {
-                  const float4 a4 = *reinterpret_cast<const float4*>(aux_row + n0 + 4 * q);
-                  av[4 * q] = a4.x; av[4 * q + 1] = a4.y; av[4 * q + 2] = a4.z; av[4 * q + 3] = a4.w;
-                }
-              }
-              if (aux_mode == 1) {
-#pragma unroll
-                for (int j = 0; j < 16; ++j) v[j] *= gelu_erf_grad(av[j]);
-              } else {
-#pragma unroll
-                for (int j = 0; j < 16; ++j) v[j] *= av[j];
-              }
-            }
-            if (FULL && mask_row != nullptr) {
-#pragma unroll
-              for (int q = 0; q < 2; ++q) {
-                const uint4 mk = mk_cur[q];
-                const uint32_t w4[4] = {mk.x, mk.y, mk.z, mk.w};
-#pragma unroll
-                for (int e = 0; e < 4; ++e) {
-                  if (mask_mul) {  // saved activation derivative (GELU'): multiply
-                    v[8 * q + 2 * e] *= ld16((uint16_t)(w4[e] & 0xffff), fmt);
-                    v[8 * q + 2 * e + 1] *= ld16((uint16_t)(w4[e] >> 16), fmt);
-                  } else {         // ReLU mask: zero where the saved activation is <= 0
-                    if (!pos16((uint16_t)(w4[e] & 0xffff))) v[8 * q + 2 * e] = 0.f;
-                    if (!pos16((uint16_t)(w4[e] >> 16))) v[8 * q + 2 * e + 1] = 0.f;
-                  }
-                }
-              }
-            }
-            if (o32_row != nullptr) {
-              if (FULL && atomic) {  // split-K / accumulate: 128-bit reductions (4x fewer L2 atomic operations than scalar REDs)
-#pragma unroll
-                for (int q = 0; q < 4; ++q)
-                  red_add_f32x4(o32_row + n0 + 4 * q, make_float4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]));
-              } else if (v256) {
-                st_global_256f(o32_row + n0, v[0], v[1], v[2], v[3], v[4], v[5], v[6], v[7]);
-                st_global_256f(o32_row + n0 + 8, v[8], v[9], v[10], v[11], v[12], v[13], v[14], v[15]);
-              } else {
-#pragma unroll
-                for (int q = 0; q < 4; ++q)
-                  *reinterpret_cast<float4*>(o32_row + n0 + 4 * q) = make_float4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]);
-              }
-            }
-            if (FULL && o32i_row != nullptr) {
-              if (v256) {
-                st_global_256f(o32i_row + n0, v[0], v[1], v[2], v[3], v[4], v[5], v[6], v[7]);
-                st_global_256f(o32i_row + n0 + 8, v[8], v[9], v[10], v[11], v[12], v[13], v[14], v[15]);
-              } else {
-#pragma unroll
-                for (int q = 0; q < 4; ++q)
-                  *reinterpret_cast<float4*>(o32i_row + n0 + 4 * q) = make_float4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]);
-              }
-            }
-            if (o16_row != nullptr) {
-              if (v256) {
-                uint32_t w8[8];
-#pragma unroll
-                for (int q = 0; q < 8; ++q) w8[q] = cvt16x2(v[2 * q], v[2 * q + 1], ofmt);
-                st_global_256(o16_row + n0, w8);
-              } else {
-#pragma unroll
-                for (int q = 0; q < 2; ++q)
-                  *reinterpret_cast<uint4*>(o16_row + n0 + 8 * q) =
-                      make_uint4(cvt16x2(v[8 * q], v[8 * q + 1], ofmt), cvt16x2(v[8 * q + 2], v[8 * q + 3], ofmt),
-                                 cvt16x2(v[8 * q + 4], v[8 * q + 5], ofmt), cvt16x2(v[8 * q + 6], v[8 * q + 7], ofmt));
-              }
-            }
-            if (o16p_row != nullptr) {
-              float p[16];
-#pragma unroll
-              for (int j = 0; j < 16; ++j) p[j] = v[j];
-              if (add_prefetched) {
-#pragma unroll
-                for (int j = 0; j < 16; ++j) p[j] += rv[j];
-              } else if (add_row != nullptr) {
-#pragma unroll
-                for (int q = 0; q < 4; ++q) {
-                  const float4 a4 = *reinterpret_cast<const float4*>(add_row + n0 + 4 * q);
-                  p[4 * q] += a4.x; p[4 * q + 1] += a4.y; p[4 * q + 2] += a4.z; p[4 * q + 3] += a4.w;
-                }
-              }
-              if (v256) {
-                uint32_t w8[8];
-#pragma unroll
-                for (int q = 0; q < 8; ++q) w8[q] = cvt16x2(p[2 * q], p[2 * q + 1], ofmt);
-                st_global_256(o16p_row + n0, w8);
-              } else {
-#pragma unroll
-                for (int q = 0; q < 2; ++q)
-                  *reinterpret_cast<uint4*>(o16p_row + n0 + 8 * q) =
-                      make_uint4(cvt16x2(p[8 * q], p[8 * q + 1], ofmt), cvt16x2(p[8 * q + 2], p[8 * q + 3], ofmt),
-                                 cvt16x2(p[8 * q + 4], p[8 * q + 5], ofmt), cvt16x2(p[8 * q + 6], p[8 * q + 7], ofmt));
-              }
-            }
-          } else {
-#pragma unroll
-            for (int j = 0; j < 16; ++j) v[j] = 0.f;  // invalid rows contribute nothing to the column sums
-          }
-        } else {
-          // unaligned leading dimensions / ragged N (e.g. the [d, 2818] projector weight gradient, strided conv wgrad): scalar accesses
-#pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            const int n = n0 + j;
-            float x = v[j];
-            if (valid && n < pN) {
-              if (resid_row != nullptr) x += resid_row[n];
-              if (aux_row != nullptr) x *= (aux_mode == 1) ? gelu_erf_grad(aux_row[n]) : aux_row[n];
-              if (mask_row != nullptr) {
-                if (mask_mul) x *= ld16(mask_row[n], fmt);
-                else if (!pos16(mask_row[n])) x = 0.f;
-              }
-              if (o32_row != nullptr) {
-                float* dst = o32_row + (size_t)n * cs32;
-                if (atomic) atomicAdd(dst, x);
-                else *dst = x;
-              }
-              if (o32i_row != nullptr) o32i_row[n] = x;
-              if (o16_row != nullptr) o16_row[n] = cvt16(x, ofmt);
-              if (o16p_row != nullptr) o16p_row[n] = cvt16(x + (add_row ? add_row[n] : 0.f), ofmt);
-            } else {
-              x = 0.f;
-            }
-            v[j] = x;
-          }
-        }
-        if (FULL && colsum != nullptr) {  // warp-uniform: column sums over this warp's 32 rows, one atomic per column
-          const float sj = warp_colsum16(v, lane);  // 16 shuffles; lane l holds column l & 15
-          if (lane < 16 && n0 + lane < pN) atomicAdd(colsum + n0 + lane, sj * pr.colsum_scale);
-        }
-      }
-      };
-      if (!FULL || vec) step_loop(std::true_type{});
-      else if constexpr (FULL) step_loop(std::false_type{});
-      // release the accumulator stage
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        if (CL == 1 || crank == 0) mbar_arrive(&tmem_empty[as]);
-        else mbar_arrive_cluster(mapa_shared(smem_u32(&tmem_empty[as]), 0));
-      }
-      if (ew == 7 && lane == 0) stamp(g.dbg, 6);  // epilogue of the tile done (last warp)
-      if (++as == 2) {
-        as = 0;
-        aphase ^= 1;
-      }
+      if (tid == 0 && cw == 1) stamp(g.dbg, 6);  // epilogue of the tile done (second warpgroup)
     }
   }
 
-  tc_fence_before();
   __syncthreads();
   if (CL > 1) cluster_sync_all();  // no CTA leaves while its peer may still multicast into it or signal its barriers
-  if (warp == 2) {
-    tc_fence_after();
-    if (CL == 1) tmem_dealloc<Cfg::kTmemCols>(tmem_base);
-    else tmem_dealloc_2sm<Cfg::kTmemCols>(tmem_base);
-  }
   if (threadIdx.x == 0) stamp(g.dbg, 7);  // exit
-}
-
-// ------------------------------------------------------------------------------------------------
-// Microbenchmark: issue rate of tcgen05.mma (M=128, N=n, K=16, SW128 K-major operands resident in shared memory, no TMA in the
-// loop).  One CTA per SM; thread 0 issues `iters` groups of `per_commit` MMAs, each group followed by a commit, and waits for
-// the last commit.  out[blockIdx.x] = nanoseconds per MMA.  Used to separate the tensor-pipe rate from the operand feed.
-// ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(128, 1) mma_rate_kernel(int n, int iters, int per_commit, int kstep_bytes, float* out, int a_mn, int b_mn) {
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  const uint32_t raw_addr = smem_u32(smem_raw);
-  uint8_t* smem = smem_raw + ((1024u - (raw_addr & 1023u)) & 1023u);
-  __shared__ uint64_t bar;
-  __shared__ uint32_t holder;
-  for (int i = threadIdx.x; i < 48 * 1024 / 4; i += blockDim.x) reinterpret_cast<uint32_t*>(smem)[i] = 0x3c003c00u;  // fp16 1.0
-  if (threadIdx.x == 0) {
-    mbar_init(&bar, 8);
-    fence_barrier_init();
-  }
-  fence_proxy_async_smem();
-  if (threadIdx.x < 32) tmem_alloc<512>(&holder);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = holder;
-  if (threadIdx.x == 0) {
-    const uint32_t sa = smem_u32(smem), sb = sa + 16384;
-    const uint32_t idesc = make_idesc_f16_ab(128, n, 0, 0, a_mn, b_mn);
-    unsigned long long t0, t1;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t0));
-    uint32_t phase = 0;
-    for (int it = 0; it < iters; ++it) {
-      for (int k = 0; k < per_commit; ++k) {
-        const uint32_t off = (uint32_t)((k & 3) * kstep_bytes);
-        const uint32_t offm = (uint32_t)((k & 3) * 2048);  // MN-major: 16 k-rows = two 1024 B swizzle atoms
-        const uint64_t da = a_mn ? make_smem_desc_sw128(sa + offm, 8192, 1024) : make_smem_desc_sw128(sa + off, 16, 1024);
-        const uint64_t db = b_mn ? make_smem_desc_sw128(sb + offm, 8192, 1024) : make_smem_desc_sw128(sb + off, 16, 1024);
-        umma_f16_ss(tmem, da, db, idesc, 1u);
-      }
-      umma_commit(&bar);
-      if ((it & 7) == 7) {  // eight commits complete one barrier phase (iters is a multiple of 8)
-        mbar_wait(&bar, phase);
-        phase ^= 1;
-      }
-    }
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t1));
-    out[blockIdx.x] = (float)(t1 - t0) / (float)((long long)iters * per_commit);
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (threadIdx.x < 32) {
-    tc_fence_after();
-    tmem_dealloc<512>(tmem);
-  }
-}
-
-// Microbenchmark: tcgen05.ld 32x32b.x16 rate with the epilogue's access pattern (8 warps, warp w reads lane quarter w % 4,
-// the two warps of a quarter read different column halves).  mode 0: load + wait per step; mode 1: next load in flight while the
-// current step's 16 values are consumed (the epilogue's software pipeline); mode 2: x32 loads.  out[block] = ns per 16-column step.
-__global__ void __launch_bounds__(256, 1) tmem_ld_rate_kernel(int iters, int mode, float* out, float* sink) {
-  __shared__ uint32_t holder;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (warp == 0) tmem_alloc<512>(&holder);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t base = holder + ((uint32_t)((warp & 3) * 32) << 16) + (warp >> 2) * 128;
-  float acc = 0.f;
-  unsigned long long t0, t1;
-  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t0));
-  for (int it = 0; it < iters; ++it) {
-    if (mode == 0) {
-      for (int c = 0; c < 8; ++c) {
-        uint32_t r[16];
-        tmem_ld_32x32b_x16(base + c * 16, r);
-        tmem_ld_wait();
-#pragma unroll
-        for (int j = 0; j < 16; ++j) acc += __uint_as_float(r[j]);
-      }
-    } else if (mode == 1) {
-      uint32_t r[16];
-      tmem_ld_32x32b_x16(base, r);
-      for (int c = 0; c < 8; ++c) {
-        tmem_ld_wait();
-        float v[16];
-#pragma unroll
-        for (int j = 0; j < 16; ++j) v[j] = __uint_as_float(r[j]);
-        if (c + 1 < 8) tmem_ld_32x32b_x16(base + (c + 1) * 16, r);
-#pragma unroll
-        for (int j = 0; j < 16; ++j) acc += v[j];
-      }
-    } else {
-      for (int c = 0; c < 4; ++c) {
-        uint32_t r[32];
-        tmem_ld_32x32b_x32(base + c * 32, r);
-        tmem_ld_wait();
-#pragma unroll
-        for (int j = 0; j < 32; ++j) acc += __uint_as_float(r[j]);
-      }
-    }
-  }
-  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t1));
-  if (threadIdx.x == 0) out[blockIdx.x] = (float)(t1 - t0) / (float)((long long)iters * 8);
-  if (acc == 123.456f) sink[threadIdx.x] = acc;
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    tc_fence_after();
-    tmem_dealloc<512>(holder);
-  }
-  (void)lane;
-}
-
-int debug_tmem_ld_rate(int iters, int mode, int blocks, float* out, float* sink, cudaStream_t stream) {
-  tmem_ld_rate_kernel<<<blocks, 256, 0, stream>>>(iters, mode, out, sink);
-  return (int)cudaGetLastError();
-}
-
-int debug_mma_rate(int n, int iters, int per_commit, int kstep_bytes, int blocks, float* out, cudaStream_t stream, int a_mn, int b_mn) {
-  iters = (iters + 7) / 8 * 8;
-  static bool attr = false;
-  if (!attr) {
-    cudaFuncSetAttribute(mma_rate_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 50 * 1024);
-    attr = true;
-  }
-  mma_rate_kernel<<<blocks, 128, 50 * 1024, stream>>>(n, iters, per_commit, kstep_bytes, out, a_mn, b_mn);
-  return (int)cudaGetLastError();
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -922,13 +701,13 @@ int launch_gemm_group(GemmGroup& g, int bn, int num_sms, cudaStream_t stream) {
   const int cl = g.cluster == 2 ? 2 : 1;
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(gemm_tcgen05_kernel<1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes);
+    cudaError_t e = cudaFuncSetAttribute(gemm_wgmma_kernel<1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes);
     if (e == cudaSuccess)
-      e = cudaFuncSetAttribute(gemm_tcgen05_kernel<1, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes);
+      e = cudaFuncSetAttribute(gemm_wgmma_kernel<1, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes);
     if (e == cudaSuccess)
-      e = cudaFuncSetAttribute(gemm_tcgen05_kernel<2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes);
+      e = cudaFuncSetAttribute(gemm_wgmma_kernel<2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes);
     if (e == cudaSuccess)
-      e = cudaFuncSetAttribute(gemm_tcgen05_kernel<2, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes);
+      e = cudaFuncSetAttribute(gemm_wgmma_kernel<2, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes);
     if (e != cudaSuccess) {
       set_error("cudaFuncSetAttribute(gemm, smem=%d): %s", Cfg::kSmemBytes, cudaGetErrorString(e));
       return (int)e;
@@ -950,12 +729,21 @@ int launch_gemm_group(GemmGroup& g, int bn, int num_sms, cudaStream_t stream) {
       set_error("gemm problem %d: B tensor-map box has %d rows but the launch uses bn %d (cluster %d)", p, pr.b_box_rows, bn, cl);
       return (int)cudaErrorInvalidValue;
     }
-    if (pr.b_mn && pr.b_3d != 0 && (cl != 1 || pr.b_3d != bn / 64)) {
-      set_error("gemm problem %d: 3-D B tensor map was built for bn %d, single-CTA launches (got bn %d, cluster %d)", p, 64 * pr.b_3d, bn, cl);
+    if (cl == 2 && pr.b_mn) {
+      set_error("gemm problem %d: cluster launches need a K-major B operand", p);
+      return (int)cudaErrorInvalidValue;
+    }
+    if (pr.b_mn && pr.b_3d != 0 && pr.b_3d != bn / 64) {
+      set_error("gemm problem %d: 3-D B tensor map was built for bn %d (got bn %d)", p, 64 * pr.b_3d, bn);
       return (int)cudaErrorInvalidValue;
     }
     if (pr.b_mn && bn % (64 * cl) != 0) {
       set_error("gemm problem %d: MN-major B needs BN %% %d == 0 (got %d)", p, 64 * cl, bn);
+      return (int)cudaErrorInvalidValue;
+    }
+    const int fa = pr.a_fmt < 0 ? g.fmt : pr.a_fmt, fb = pr.b_fmt < 0 ? g.fmt : pr.b_fmt;
+    if (fa != fb) {
+      set_error("gemm problem %d: A and B must share one 16-bit format (wgmma), got %d and %d", p, fa, fb);
       return (int)cudaErrorInvalidValue;
     }
     const int total_kb = pr.taps * pr.kblk_per_tap;
@@ -991,8 +779,8 @@ int launch_gemm_group(GemmGroup& g, int bn, int num_sms, cudaStream_t stream) {
   cudaError_t e;
   if (cl == 1) {
     const int grid = total < num_sms ? total : num_sms;
-    if (full) launch_k(gemm_tcgen05_kernel<1, true>, dim3(grid), dim3(384), Cfg::kSmemBytes, stream, g);
-    else launch_k(gemm_tcgen05_kernel<1, false>, dim3(grid), dim3(384), Cfg::kSmemBytes, stream, g);
+    if (full) launch_k(gemm_wgmma_kernel<1, true>, dim3(grid), dim3(kGemmThreads), Cfg::kSmemBytes, stream, g);
+    else launch_k(gemm_wgmma_kernel<1, false>, dim3(grid), dim3(kGemmThreads), Cfg::kSmemBytes, stream, g);
     e = cudaGetLastError();
   } else {
     const int max_clusters = num_sms / 2;
@@ -1000,7 +788,7 @@ int launch_gemm_group(GemmGroup& g, int bn, int num_sms, cudaStream_t stream) {
     cudaLaunchConfig_t cfg;
     memset(&cfg, 0, sizeof(cfg));
     cfg.gridDim = dim3(2 * clusters);
-    cfg.blockDim = dim3(384);
+    cfg.blockDim = dim3(kGemmThreads);
     cfg.dynamicSmemBytes = Cfg::kSmemBytes;
     cfg.stream = stream;
     cudaLaunchAttribute attr[2];
@@ -1013,7 +801,7 @@ int launch_gemm_group(GemmGroup& g, int bn, int num_sms, cudaStream_t stream) {
     cfg.attrs = attr;
     cfg.numAttrs = pdl_enabled() ? 2 : 1;
     ++*launch_counter();
-    e = full ? cudaLaunchKernelEx(&cfg, gemm_tcgen05_kernel<2, true>, g) : cudaLaunchKernelEx(&cfg, gemm_tcgen05_kernel<2, false>, g);
+    e = full ? cudaLaunchKernelEx(&cfg, gemm_wgmma_kernel<2, true>, g) : cudaLaunchKernelEx(&cfg, gemm_wgmma_kernel<2, false>, g);
   }
   if (e != cudaSuccess) {
     set_error("gemm launch failed: %s", cudaGetErrorString(e));
@@ -1022,10 +810,11 @@ int launch_gemm_group(GemmGroup& g, int bn, int num_sms, cudaStream_t stream) {
   return 0;
 }
 
-// Tile width (and split-K factor) that minimise the modelled time of one grouped launch.  Constants are measurements on B200
-// (profiles/README.md, round 2): a 64-wide k-block (4 MMAs + one tcgen05.commit) costs ~0.33 us per CTA WHATEVER the tile width
-// (two commits are never closer than ~615 cycles, which hides the N/2-cycle cost of the MMAs in between), ~2 us from kernel entry to the first MMA, an epilogue of ~0.5 us + 2.5 us x bn/256 (4 us x
-// bn/256 with split-K reductions), of which only a fraction is exposed when a CTA has further tiles to run.
+// Tile width (and split-K factor) that minimise the modelled time of one grouped launch on H100.  The constants are a model,
+// not a measurement: a 64-wide k-block of a 128 x bn tile is 128 * bn * 64 multiply-adds at the data-sheet dense fp16 rate of one
+// SM (989 TFLOP/s over 132 SMs, ~0.0018 us per tile column) plus ~0.15 us of TMA / barrier overhead, ~1 us from kernel entry
+// to the first MMA, and an epilogue of ~0.5 us + 2 us x bn/256 (3 us x bn/256 with split-K reductions), of which only a
+// fraction is exposed when a CTA has further tiles to run.
 //   kblocks[p] = 64-wide k-blocks of problem p (taps included); max_split = 1 disables split-K.
 TileChoice choose_tile(const int* Ms, const int* Ns, const int* kblocks, int num, int num_sms, int step, int max_split) {
   TileChoice best{256, 1};
@@ -1049,8 +838,8 @@ TileChoice choose_tile(const int* Ms, const int* Ns, const int* kblocks, int num
       long kb_cta = 0;
       for (int i = 0; i < ncta; ++i) kb_cta = load[i] > kb_cta ? load[i] : kb_cta;
       const long rounds = (tiles + ncta - 1) / ncta;
-      const double epi = 0.5 + bn * (ks > 1 ? 4.0 : 2.5) / 256.0;
-      const double t = 2.0 + 0.33 * (double)kb_cta + epi * (1.0 + 0.3 * (double)(rounds - 1));
+      const double epi = 0.5 + bn * (ks > 1 ? 3.0 : 2.0) / 256.0;
+      const double t = 1.0 + (0.15 + 0.0018 * bn) * (double)kb_cta + epi * (1.0 + 0.3 * (double)(rounds - 1));
       if (best_t < 0 || t < best_t - 1e-9) {
         best_t = t;
         best = TileChoice{bn, ks};

@@ -7,7 +7,7 @@
 
 namespace uv {
 
-constexpr int GEMM_BM = 128;  // UMMA M (cta_group::1)
+constexpr int GEMM_BM = 128;  // tile rows: two consumer warpgroups of wgmma M = 64
 constexpr int GEMM_BK = 64;   // one 128-byte swizzle span of 16-bit elements
 constexpr int GEMM_MAX_GROUP = 4;
 
@@ -88,7 +88,8 @@ struct GemmGroup {
   GemmProblem p[GEMM_MAX_GROUP];
 };
 
-// bn: tile width, multiple of 16 in [32, 256] (multiple of 64 when a problem has an MN-major B).  Returns cudaError_t as int.
+// bn: tile width, multiple of 16 in [32, 256] (multiple of 64 when a problem has an MN-major B).  A and B of a problem must share
+// one 16-bit format.  Returns cudaError_t as int.
 int launch_gemm_group(GemmGroup& g, int bn, int num_sms, cudaStream_t stream);
 // Tile width minimising waves x tile-time for problems that share a launch (step 16: K-major B, 64: MN-major B).
 struct TileChoice {
@@ -96,7 +97,7 @@ struct TileChoice {
 };
 TileChoice choose_tile(const int* Ms, const int* Ns, const int* kblocks, int num, int num_sms, int step, int max_split);
 // MN-major B operand [rows = K, cols = N] (N contiguous): a 3-D view {64, K, N/64} lets one TMA instruction fetch the whole
-// 64 x bn tile of a k-block (five TMA operations per k-block instead of two measured 48 % slower); needs cols % 64 == 0.
+// 64 x bn tile of a k-block (fewer TMA operations per k-block than one 2-D box per 64-wide block); needs cols % 64 == 0.
 int make_tmap_b_mn(GemmProblem& p, const void* base, uint64_t rows, uint64_t cols, uint64_t ld_elems, int bn, bool allow_3d = true);
 int choose_bn(const int* Ms, const int* Ns, const int* kblocks, int num, int num_sms, int step);
 
@@ -112,7 +113,7 @@ void set_error(const char* fmt, ...);
 // Every kernel of this library starts with pdl_prologue() (griddepcontrol.launch_dependents + griddepcontrol.wait, ptx.cuh):
 // the next kernel in the stream may be scheduled while this one is still running and blocks at its own
 // griddepcontrol.wait until this grid has completed and flushed - the launch latency and the next kernel's prologue
-// (barrier init, TMEM allocation, tensor-map prefetch) disappear under the current kernel's tail.  UNIVTG_PDL=0 disables it.
+// (barrier init, tensor-map prefetch) disappear under the current kernel's tail.  UNIVTG_PDL=0 disables it.
 bool pdl_enabled();
 long long* launch_counter();  // kernels launched by this library since it was loaded (bench accounting: gpu_launches)
 template <typename... KArgs, typename... Args>
@@ -150,7 +151,5 @@ int adamw_step_impl(float* params, float* grads, float* exp_avg, float* exp_avg_
                     float eps, float weight_decay, int32_t step, float max_grad_norm, int32_t write_clipped_grads, float* scratch3,
                     const PackSegTable* segs, void* stream);
 
-int debug_tmem_ld_rate(int iters, int mode, int blocks, float* out, float* sink, cudaStream_t stream);
-int debug_mma_rate(int n, int iters, int per_commit, int kstep_bytes, int blocks, float* out, cudaStream_t stream, int a_mn = 0, int b_mn = 0);
 
 }  // namespace uv

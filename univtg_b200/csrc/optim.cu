@@ -157,7 +157,7 @@ int adamw_step_impl(float* params, float* grads, float* exp_avg, float* exp_avg_
     set_error("univtg_adamw_step: buffers must be 16-byte aligned with n %% 4 == 0, step >= 1, scratch non-null");
     return (int)cudaErrorInvalidValue;
   }
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   const size_t n4 = n / 4;

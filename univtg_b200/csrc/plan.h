@@ -298,7 +298,7 @@ struct univtg_plan {
   int profiling;
   int n_marks;
   cudaEvent_t marks[kMaxMarks];
-  int mark_kind[kMaxMarks];  // kind of the interval that ENDS at mark i (i >= 1): 0 row kernel, 1 tcgen05 GEMM, 2 attention, 3 other work
+  int mark_kind[kMaxMarks];  // kind of the interval that ENDS at mark i (i >= 1): 0 row kernel, 1 tensor-core GEMM, 2 attention, 3 other work
 };
 
 namespace {

@@ -1,6 +1,6 @@
-// Thin inline-PTX wrappers for the sm_100a features the UniVTG hot path uses:
-// mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit / ld) and the
-// UMMA shared-memory + instruction descriptors.  sm_100a only - no other arch is supported.
+// Thin inline-PTX wrappers for the sm_90a features the UniVTG hot path uses:
+// mbarrier, TMA (cp.async.bulk.tensor, cluster multicast), wgmma fences and the GMMA shared-memory descriptor.
+// sm_90a only - no other arch is supported.
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -95,7 +95,6 @@ UV_DEVINL void cluster_sync_all() {
   asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
   asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
-// ---- CTA pair (cta_group::2) helpers ----
 // shared::cluster address of `smem_addr` (a shared::cta address of this CTA) in CTA `rank` of the cluster
 UV_DEVINL uint32_t mapa_shared(uint32_t smem_addr, uint32_t rank) {
   uint32_t r;
@@ -106,13 +105,13 @@ UV_DEVINL uint32_t mapa_shared(uint32_t smem_addr, uint32_t rank) {
 UV_DEVINL void mbar_arrive_cluster(uint32_t cluster_addr) {
   asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
 }
-// 2-D tiled load issued by either CTA of a pair: the tile lands in THIS CTA's smem, the transaction bytes are credited to the
-// mbarrier at `bar_cluster_addr` (the leader CTA's barrier).
-UV_DEVINL void tma_load_2d_2sm(void* smem_dst, const CUtensorMap* m, uint32_t bar_cluster_addr, int c0, int c1) {
+// 2-D tiled load multicast to every CTA of `cta_mask`: the tile lands at the same smem offset in each of them and the bytes are
+// credited to the mbarrier at the same offset in each of them.
+UV_DEVINL void tma_load_2d_mc(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1, uint16_t cta_mask) {
   asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4}], [%2], %5;"
       :
-      : "r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar_cluster_addr), "r"(c0), "r"(c1)
+      : "r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(cta_mask)
       : "memory");
 }
 UV_DEVINL void tma_load_3d(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2) {
@@ -124,126 +123,41 @@ UV_DEVINL void tma_load_3d(void* smem_dst, const CUtensorMap* m, uint64_t* bar, 
 }
 
 // ----------------------------------------------------------------------------------------------
-// tcgen05: TMEM allocation, fences, MMA, commit, loads
+// wgmma (warpgroup MMA, sm_90a): fences and the shared-memory matrix descriptor.  The MMAs themselves are in wgmma.cuh.
 // ----------------------------------------------------------------------------------------------
-template <uint32_t kCols>
-UV_DEVINL void tmem_alloc(uint32_t* smem_holder) {  // whole warp
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_holder)), "n"(kCols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+UV_DEVINL void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+UV_DEVINL void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+UV_DEVINL void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-template <uint32_t kCols>
-UV_DEVINL void tmem_dealloc(uint32_t taddr) {  // whole warp (the allocating one)
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(kCols) : "memory");
+// keeps the compiler from moving accumulator reads / writes across a wgmma that is still in flight
+UV_DEVINL void reg_fence(float& r) { asm volatile("" : "+f"(r)::"memory"); }
+UV_DEVINL void reg_fence(uint32_t& r) { asm volatile("" : "+r"(r)::"memory"); }
+template <uint32_t kRegs>
+UV_DEVINL void setmaxnreg_inc() {
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kRegs));
 }
-template <uint32_t kCols>
-UV_DEVINL void tmem_alloc_2sm(uint32_t* smem_holder) {  // one warp (same warp index) in EACH CTA of the pair
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_holder)), "n"(kCols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
+template <uint32_t kRegs>
+UV_DEVINL void setmaxnreg_dec() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kRegs));
 }
-template <uint32_t kCols>
-UV_DEVINL void tmem_dealloc_2sm(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(kCols) : "memory");
-}
-UV_DEVINL void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-UV_DEVINL void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
+// named barrier over `count` threads (ids 1..15; 0 is __syncthreads)
+UV_DEVINL void named_bar_sync(int id, int count) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory"); }
 
-// D[tmem] (+)= A[smem desc] * B[smem desc]; issued by ONE thread.
-UV_DEVINL void umma_f16_ss(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}\n"
-      :
-      : "r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// CTA-pair MMA (M = 256: 128 rows per CTA; each CTA's smem holds its A rows and HALF of the B rows); issued by the leader CTA.
-UV_DEVINL void umma_f16_ss_2sm(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}\n"
-      :
-      : "r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// ... and its commit: arrives on the mbarrier at this offset in every CTA of `cta_mask`.
-UV_DEVINL void umma_commit_2sm(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-                   smem_u32(bar)),
-               "h"(cta_mask)
-               : "memory");
-}
-// Arrive on an mbarrier once all previously issued tcgen05.mma of this thread retire.
-UV_DEVINL void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-
-// 32 lanes x 32 consecutive fp32 columns: thread i of the warp reads TMEM lane (32*(warp%4) + i).
-UV_DEVINL void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-UV_DEVINL void tmem_ld_32x32b_x16(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-UV_DEVINL void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// ----------------------------------------------------------------------------------------------
-// UMMA descriptors (sm_100 encoding; cf. cute/arch/mma_sm100_desc.hpp field tables)
-// ----------------------------------------------------------------------------------------------
-// Shared-memory matrix descriptor for a SWIZZLE_128B tile of 16-bit elements.
+// Shared-memory matrix descriptor for a SWIZZLE_128B tile of 16-bit elements (sm_90 GMMA encoding).
 //   K-major : rows of 128 B (64 elements of K), 8-row swizzle atoms of 1024 B stacked along M/N.
-//             SBO = 1024 B (next 8-row group); LBO unused (1).
+//             SBO = 1024 B (next 8-row group); LBO unused (1).  One k-step of 16 elements = +32 B.
 //   MN-major: "rows" of 128 B are 64 consecutive M/N elements for one k; 8 k's form a 1024 B atom.
-//             SBO = 1024 B (next 8 k's); LBO = byte distance between 64-element M/N blocks.
-// bits [0,14) addr>>4, [16,30) LBO>>4, [32,46) SBO>>4, [46,48) version=1, [61,64) layout=2 (SW128).
+//             SBO = 1024 B (next 8 k's); LBO = byte distance between 64-element M/N blocks.  One k-step = +2048 B.
+// bits [0,14) addr>>4, [16,30) LBO>>4, [32,46) SBO>>4, [62,64) layout = 1 (128B swizzle).
 UV_DEVINL uint64_t make_smem_desc_sw128(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
+  d |= (uint64_t)1 << 62;
   return d;
-}
-
-// Instruction descriptor for kind::f16 with fp32 accumulation.
-//   ab_fmt: 0 = fp16, 1 = bf16.  a_mn / b_mn: 1 if the operand is MN-major in shared memory.
-__host__ __device__ constexpr uint32_t make_idesc_f16(int M, int N, int ab_fmt, int a_mn, int b_mn) {
-  return (1u << 4)                         // c_format = F32
-         | ((uint32_t)ab_fmt << 7)         // a_format
-         | ((uint32_t)ab_fmt << 10)        // b_format
-         | ((uint32_t)a_mn << 15)          // a_major
-         | ((uint32_t)b_mn << 16)          // b_major
-         | ((uint32_t)(N >> 3) << 17)      // n_dim
-         | ((uint32_t)(M >> 4) << 24);     // m_dim
-}
-
-// Same with independent A / B operand formats (gradients are bf16, activations and weights fp16).
-__host__ __device__ constexpr uint32_t make_idesc_f16_ab(int M, int N, int a_fmt, int b_fmt, int a_mn, int b_mn) {
-  return (1u << 4) | ((uint32_t)a_fmt << 7) | ((uint32_t)b_fmt << 10) | ((uint32_t)a_mn << 15) | ((uint32_t)b_mn << 16) |
-         ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
 }
 
 // ----------------------------------------------------------------------------------------------
@@ -254,23 +168,22 @@ UV_DEVINL float warp_sum(float v) {
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
   return v;
 }
-// 256-bit global accesses (sm_100: STG/LDG.E.ENL2.256): a thread moves one whole 32-byte sector per instruction.
-// Addresses must be 32-byte aligned.
+// 32-byte global accesses (one whole sector per thread) as two 128-bit accesses.  Addresses must be 32-byte aligned.
 UV_DEVINL void st_global_256(void* p, const uint32_t (&w)[8]) {
-  asm volatile("st.global.v8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"l"(p), "r"(w[0]), "r"(w[1]), "r"(w[2]), "r"(w[3]), "r"(w[4]),
-               "r"(w[5]), "r"(w[6]), "r"(w[7])
-               : "memory");
+  uint4* q = reinterpret_cast<uint4*>(p);
+  q[0] = make_uint4(w[0], w[1], w[2], w[3]);
+  q[1] = make_uint4(w[4], w[5], w[6], w[7]);
 }
 UV_DEVINL void st_global_256f(float* p, float a0, float a1, float a2, float a3, float a4, float a5, float a6, float a7) {
-  asm volatile("st.global.v8.f32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"l"(p), "f"(a0), "f"(a1), "f"(a2), "f"(a3), "f"(a4), "f"(a5),
-               "f"(a6), "f"(a7)
-               : "memory");
+  float4* q = reinterpret_cast<float4*>(p);
+  q[0] = make_float4(a0, a1, a2, a3);
+  q[1] = make_float4(a4, a5, a6, a7);
 }
 UV_DEVINL void ld_global_256f(const float* p, float* v) {
-  asm volatile("ld.global.v8.f32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-               : "=f"(v[0]), "=f"(v[1]), "=f"(v[2]), "=f"(v[3]), "=f"(v[4]), "=f"(v[5]), "=f"(v[6]), "=f"(v[7])
-               : "l"(p)
-               : "memory");
+  const float4 a = reinterpret_cast<const float4*>(p)[0];
+  const float4 b = reinterpret_cast<const float4*>(p)[1];
+  v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w;
+  v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
 }
 // one 128-bit reduction (four fp32 adds, relaxed, gpu scope) - addr must be 16-byte aligned
 UV_DEVINL void red_add_f32x4(float* addr, float4 v) {

@@ -407,7 +407,7 @@ __global__ void __launch_bounds__(256) droppath_scales_kernel(unsigned long long
 int launch_dropout_mask(const DropSpec& spec, size_t n, size_t cols, float* out, cudaStream_t stream) {
   if (n == 0) return 0;
   size_t blocks = (n + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   launch_k(dropout_mask_kernel, dim3((unsigned)blocks), dim3(256), 0, stream, spec, n, cols, out);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) set_error("dropout_mask launch failed: %s", cudaGetErrorString(e));

@@ -153,7 +153,7 @@ TrainWs make_train_ws(const univtg_config& c, const univtg_shape& s, const Packe
   return w;
 }
 
-// Gradient operands use the plan's 16-bit format (one tcgen05.mma takes A and B in ONE format).  With fp16 they would
+// Gradient operands use the plan's 16-bit format (one wgmma takes A and B in ONE format).  With fp16 they would
 // underflow, so the whole backward runs on gradients multiplied by a power-of-two loss scale S: the upstream output
 // gradients are scaled on entry, every intermediate stays scaled, and each PARAMETER gradient is multiplied by 1/S where it
 // is written (GEMM alpha, column-sum / LayerNorm / head kernels).  bf16 plans simply use S = 1.
@@ -545,7 +545,7 @@ int univtg_backward(univtg_plan* P, void* ws, const float* src_txt, const float*
   const int d = P->d, ff = P->ff, fmt = c.operand_format, M = P->M, Mv = P->Mv, Mt = P->Mt, Mh = P->Mh, L = P->L, Lv = P->Lv,
             Lt = P->Lt, B = P->B;
   // persistent GEMM grids assume every CTA is resident at once; when a gradient all-reduce runs beside the backward its CTAs
-  // hold some SMs, and a 148-CTA grid would wait for them (a second wave): launch on the SMs that are left
+  // hold some SMs, and a full-width grid would wait for them (a second wave): launch on the SMs that are left
   const int sms = (P->num_sms_bwd > 0 && P->num_sms_bwd < P->num_sms) ? P->num_sms_bwd : P->num_sms;
   const int FMT_G = fmt;                 // gradient operand format == activation operand format
   const float GS = grad_scale;           // loss scale carried by every intermediate gradient
@@ -661,7 +661,7 @@ int univtg_backward(univtg_plan* P, void* ws, const float* src_txt, const float*
       p.out16 = T.dh1 + s * d;
       p.ld16 = 2 * d;
       p.out_fmt = FMT_G;
-      p.colsum = s == 0 ? G_cls(1) : G_span(1);  // bias gradient of conv layer 0 (a separate column-sum pass measured 30 us/step slower)
+      p.colsum = s == 0 ? G_cls(1) : G_span(1);  // bias gradient of conv layer 0 (saves a separate column-sum pass)
       p.colsum_scale = INV;
     }
     rc = gemm_launch(P, g, bn_c2d, sms, st);
@@ -770,9 +770,8 @@ int univtg_backward(univtg_plan* P, void* ws, const float* src_txt, const float*
     }
     // ---- FFN2: dgrad -> d(hpre) = (dF W2) * gelu'(hpre) (saved 16-bit derivative);  wgrad dW2 = dF^T h ----
     // ---- FFN1: dgrad d(x1) = dhpre W1 + dy (residual);          wgrad dW1 = dhpre^T x1 ----
-    // (sharing one launch between a data-gradient GEMM and the weight-gradient GEMM that reads the same dY was measured: fewer
-    //  launches and 10 % less event-timed GEMM time, but the pipelined step got 50 us SLOWER - profiles/README.md round 2 - so the
-    //  launches stay separate and are chained by programmatic dependent launch)
+    // (the data-gradient and weight-gradient GEMMs that read the same dY are separate launches chained by programmatic
+    //  dependent launch; sharing one launch was slower per step on the earlier GPU generation and has not been re-measured)
     auto ffn2_dgrad = [&](GemmProblem& p, int bnn) -> int {
       int r = setup_gemm(p, Mat16{T.dbr16, M, d, d}, 0, Mat16{W16(lp.w2), d, ff, ff}, 1, M, ff, d, bnn);
       p.a_fmt = FMT_G;
@@ -929,7 +928,7 @@ int univtg_backward(univtg_plan* P, void* ws, const float* src_txt, const float*
       const int num_kv = (L + 127) / 128;
       a.dq_atomic = (!tc || num_kv > 1) ? 1 : 0;
       fused16 = !a.dq_atomic;  // one key tile: the kernel emits the 16-bit operands and the in_proj_bias gradient itself
-      if (fused16) a.dqkv16 = T.dqkv16;  // (the kernel could also accumulate the column sums; a separate pass measured faster)
+      if (fused16) a.dqkv16 = T.dqkv16;  // (the in_proj_bias column sums are a separate pass)
       if (a.dq_atomic) cudaMemsetAsync(T.dqkv32, 0, (size_t)M * 3 * d * 4, st);
       if (tc) {
         if (make_tmap_2d(&a.tm_qkv, T.qkv16[l], (uint64_t)M, (uint64_t)3 * d, (uint64_t)3 * d, 128, 64)) return 1;

@@ -82,8 +82,7 @@ class OverlappedGradExchange:
         self.events = None
         self.comm_stream = None
         # SMs left to the collective's CTAs while it overlaps the backward: an NCCL CTA cannot share an SM with a GEMM CTA (registers),
-        # so the reserve follows NCCL_MAX_CTAS, the cap on what NCCL takes.  Measured at N=8 (profiles/README.md section 7): 8 / 16 /
-        # 24 / 32 CTAs -> 3.98 / 3.08 / 2.95 / 2.90 ms per step - the NVLS all-reduce is channel-bound below 32.
+        # so the reserve follows NCCL_MAX_CTAS, the cap on what NCCL takes (default 32; tools/scaling_sweep.sh sweeps it).
         default_reserve = os.environ.get("NCCL_MAX_CTAS", "32")
         self.sm_reserve = int(os.environ.get("UNIVTG_DDP_SM_RESERVE", default_reserve)) if self.backend == "nccl" else 0
 

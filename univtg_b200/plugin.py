@@ -122,7 +122,7 @@ class _WorkspaceLease:
 
 
 class Model(nn.Module):
-    """B200-native UniVTG model: the reference `Model` (model/univtg.py:51-155) behind the same interface."""
+    """H100-native UniVTG model: the reference `Model` (model/univtg.py:51-155) behind the same interface."""
 
     def __init__(self, args):
         super().__init__()
@@ -165,7 +165,7 @@ class Model(nn.Module):
         self.weightedpool = _Params(weight=(d, 1))
         self.reset_parameters()
 
-        # One 16-bit operand format per model (a tcgen05.mma takes A and B in ONE format): fp16 by default - its 11-bit
+        # One 16-bit operand format per model (a wgmma takes A and B in ONE format): fp16 by default - its 11-bit
         # significand keeps the north-star tolerance - with gradients carried under a power-of-two loss scale in backward
         # (fp16 would underflow otherwise); "bf16" needs no scaling but is 8x coarser.
         self._packed = {}
@@ -531,7 +531,7 @@ class Model(nn.Module):
 
     def profile_forward(self, inputs):
         """Run one inference forward with the per-launch CUDA-event timeline on; returns [(kind, ms), ...]
-        (kind 0 = row kernel, 1 = tcgen05 GEMM, 2 = attention)."""
+        (kind 0 = row kernel, 1 = tensor-core GEMM, 2 = attention)."""
         lib = _lib.load_library()
         B, Lv, _ = inputs["src_vid"].shape
         Lt = inputs["src_txt"].shape[1]
@@ -553,7 +553,7 @@ class Model(nn.Module):
 
     def profile_train_step(self, B, Lv, Lt, run):
         """CUDA-event timeline of ONE training step of shape (B, Lv, Lt): `run()` must execute forward + criterion + backward.
-        Returns [(kind, ms), ...]: kind 1 = one tcgen05 GEMM launch, 2 = one attention launch (forward or backward), 3 = whatever
+        Returns [(kind, ms), ...]: kind 1 = one tensor-core GEMM launch, 2 = one attention launch (forward or backward), 3 = whatever
         ran between two of those (row kernels, criterion, launch gaps)."""
         lib = _lib.load_library()
         with torch.cuda.device(self._device()):
