@@ -56,7 +56,7 @@ typedef struct univtg_rng {
   float droppath;       /* args.droppath (drop probability); 0 = off */
 } univtg_rng;
 
-typedef struct univtg_plan univtg_plan; /* opaque; host memory only (tensor maps + pointer table) */
+typedef struct univtg_plan univtg_plan; /* opaque; host memory only (shape, tile widths, buffer pointers) */
 
 const char* univtg_last_error(void);
 int univtg_abi_version(void);
@@ -83,7 +83,7 @@ size_t univtg_workspace_bytes(const univtg_config* cfg, const univtg_shape* shap
  * between shapes: size them for the largest shape).  training_ws: 0 = workspace of univtg_plan_create (univtg_workspace_bytes),
  * 1 = training workspace (univtg_train_workspace_bytes). */
 int univtg_prepare_workspace(const univtg_config* cfg, const univtg_shape* shape, void* workspace, int32_t training_ws, void* stream);
-/* Build a plan: tensor maps over `packed` and `workspace` (both must stay alive and must not move).
+/* Build a plan for one shape over `packed` and `workspace` (both must stay alive and must not move).
  * `dim_t`: device fp32 [hidden_dim], the sine-embedding denominators temperature**(2*(j//2)/d)
  * (reference model/position_encoding.py:75) evaluated by the caller.  Calls univtg_prepare_workspace on `stream`. */
 int univtg_plan_create(const univtg_config* cfg, const univtg_shape* shape, const void* packed, void* workspace,

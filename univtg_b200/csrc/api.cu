@@ -1,5 +1,5 @@
-// C-ABI layer (include/univtg_b200.h): weight packing, plan construction (tensor maps + launch descriptors)
-// and the forward orchestration of reference Model.forward (model/univtg.py:105-155).
+// C-ABI layer (include/univtg_b200.h): weight packing, plan construction (shapes and tile widths) and the forward
+// orchestration of reference Model.forward (model/univtg.py:105-155), shared by inference and training.
 #include <math.h>
 #include <stdio.h>
 #include <string.h>
@@ -203,7 +203,7 @@ extern "C" {
 
 size_t univtg_workspace_bytes(const univtg_config* cfg, const univtg_shape* shape) {
   if (!check_cfg(cfg) || !check_shape(shape)) return 0;
-  return make_ws(*cfg, *shape, make_layout(*cfg)).total;
+  return make_infer_ws(*cfg, *shape, make_layout(*cfg), nullptr).total;
 }
 
 int univtg_plan_create(const univtg_config* cfg, const univtg_shape* shape, const void* packed, void* workspace,
@@ -242,209 +242,20 @@ int univtg_plan_create(const univtg_config* cfg, const univtg_shape* shape, cons
   P->Mv = P->B * P->Lv;
   P->Mt = P->B * P->Lt;
   P->Mh = P->B * (P->Lv + 1);
-  const WsLayout w = make_ws(*cfg, *shape, P->lay);
   if (univtg_prepare_workspace(cfg, shape, workspace, 0, stream) != 0) {  // zero rows of the conv-head buffers
     delete P;
     return 1;
   }
-  uint8_t* ws = P->ws;
-  for (int i = 0; i < cfg->n_input_proj; ++i) {
-    P->a_vid[i] = reinterpret_cast<uint16_t*>(ws + w.a_vid[i]);
-    P->a_txt[i] = reinterpret_cast<uint16_t*>(ws + w.a_txt[i]);
-  }
-  P->p_vid32 = reinterpret_cast<float*>(ws + w.p_vid32);
-  P->p_txt32 = reinterpret_cast<float*>(ws + w.p_txt32);
-  P->txtproj32 = reinterpret_cast<float*>(ws + w.txtproj32);
-  P->pos = reinterpret_cast<float*>(ws + w.pos);
-  P->key_mask = reinterpret_cast<float*>(ws + w.key_mask);
-  P->pool_logits = reinterpret_cast<float*>(ws + w.pool_logits);
-  P->x32 = reinterpret_cast<float*>(ws + w.x32);
-  P->br16 = reinterpret_cast<uint16_t*>(ws + w.br16);
-  P->x16 = reinterpret_cast<uint16_t*>(ws + w.x16);
-  P->xpos16 = reinterpret_cast<uint16_t*>(ws + w.xpos16);
-  P->qkv16 = reinterpret_cast<uint16_t*>(ws + w.qkv16);
-  P->attn16 = reinterpret_cast<uint16_t*>(ws + w.attn16);
-  P->h16 = reinterpret_cast<uint16_t*>(ws + w.h16);
-  P->hA = reinterpret_cast<uint16_t*>(ws + w.hA);
-  P->h1 = reinterpret_cast<uint16_t*>(ws + w.h1);
-  P->hc2 = reinterpret_cast<uint16_t*>(ws + w.hc2);
-  P->hs2 = reinterpret_cast<uint16_t*>(ws + w.hs2);
-
-  const PackedLayout& Lw = P->lay;
-  const uint8_t* pk = P->packed;
-  auto W16 = [&](size_t off) { return reinterpret_cast<const uint16_t*>(pk + off); };
-  auto F32 = [&](size_t off) { return reinterpret_cast<const float*>(pk + off); };
-  const int fmt = cfg->operand_format;
-  int rc = 0;
-  // tile width: 256 when the N extent has at least one full 256 tile, else 128
-  P->bn_main = (d % 256 == 0) ? 256 : 128;
-  {
-    // per-launch tile widths: fill the SMs with as little wave quantisation as possible
-    const int sms = P->num_sms;
-    auto bn2 = [&](int M0, int N0, int K0, int M1, int N1, int K1) {  // K in elements
-      const int Ms[2] = {M0, M1}, Ns[2] = {N0, N1}, kb[2] = {(K0 + 63) / 64, (K1 + 63) / 64};
-      return choose_bn(Ms, Ns, kb, M1 > 0 ? 2 : 1, sms, 16);
-    };
-    for (int i = 0; i < cfg->n_input_proj; ++i) P->bn_proj[i] = bn2(P->Mv, d, Lw.vid[i].kpad, P->Mt, d, Lw.txt[i].kpad);
-    P->bn_qkv = bn2(P->M, 2 * d, d, P->M, d, d);
-    P->bn_out = bn2(P->M, d, d, 0, 0, 0);
-    P->bn_ffn1 = bn2(P->M, ff, d, 0, 0, 0);
-    P->bn_ffn2 = bn2(P->M, d, ff, 0, 0, 0);
-    P->bn_conv1 = bn2(P->Mh, 2 * d, 3 * d, 0, 0, 0);
-    P->bn_conv2 = bn2(P->Mh, d, 3 * d, P->Mh, d, 3 * d);
-  }
-
-  // ---- input projectors: one grouped launch per projector depth (video + text problems) ----
-  for (int i = 0; i < cfg->n_input_proj && !rc; ++i) {
-    GemmGroup& g = P->g_proj[i];
-    memset(&g, 0, sizeof(g));
-    g.num = 2;
-    g.fmt = fmt;
-    const bool last = (i == cfg->n_input_proj - 1);
-    const int bn = P->bn_proj[i];
-    GemmProblem& pv = g.p[0];
-    GemmProblem& pt = g.p[1];
-    rc |= setup_linear(pv, P->a_vid[i], P->Mv, Lw.vid[i].kpad, Lw.vid[i].kpad, W16(Lw.vid[i].w16), d, Lw.vid[i].kpad, bn);
-    rc |= setup_linear(pt, P->a_txt[i], P->Mt, Lw.txt[i].kpad, Lw.txt[i].kpad, W16(Lw.txt[i].w16), d, Lw.txt[i].kpad, bn);
-    pv.bias = F32(Lw.vid[i].bias);
-    pt.bias = F32(Lw.txt[i].bias);
-    if (!last) {
-      pv.act = pt.act = ACT_RELU;
-      pv.out32 = P->p_vid32;
-      pt.out32 = P->p_txt32;
-      pv.ld32 = pt.ld32 = d;
-    } else {
-      // video tokens -> stream rows b*L + l; text tokens -> rows b*L + Lv + l   (cat on the sequence axis, univtg.py:119)
-      pv.rps_in = P->Lv;
-      pv.rps_out = P->L;
-      pv.row_off = 0;
-      pt.rps_in = P->Lt;
-      pt.rps_out = P->L;
-      pt.row_off = P->Lv;
-      pv.out32 = pt.out32 = P->x32;
-      pv.ld32 = pt.ld32 = d;
-      pv.out16 = pt.out16 = P->x16;
-      pv.out16p = pt.out16p = P->xpos16;
-      pv.ld16 = pt.ld16 = d;
-      pv.addtab = P->pos;
-      pv.ld_addtab = d;
-      pv.out32_id = nullptr;  // vid_mem_proj: set per call
-      pv.ld32_id = d;
-      pt.out32_id = P->txtproj32;
-      pt.ld32_id = d;
-    }
-  }
-  // ---- encoder layers ----
-  const float qscale = 1.0f / sqrtf((float)P->dh);
-  for (int l = 0; l < cfg->enc_layers && !rc; ++l) {
-    const LayerPacked& lp = Lw.layer[l];
-    {
-      GemmGroup& g = P->g_qkv[l];
-      memset(&g, 0, sizeof(g));
-      g.num = 2;
-      g.fmt = fmt;
-      // q = k = x + pos -> columns [0, 2d) of qkv16; v = x -> columns [2d, 3d)   (in_proj rows: Wq, Wk, Wv)
-      rc |= setup_linear(g.p[0], P->xpos16, P->M, d, d, W16(lp.w_in), 2 * d, d, P->bn_qkv);
-      rc |= setup_linear(g.p[1], P->x16, P->M, d, d, W16(lp.w_in) + (size_t)2 * d * d, d, d, P->bn_qkv);
-      g.p[0].bias = F32(lp.b_in);
-      g.p[0].out16 = P->qkv16;
-      g.p[0].ld16 = 3 * d;
-      g.p[1].bias = F32(lp.b_in) + 2 * d;
-      g.p[1].out16 = P->qkv16 + 2 * d;
-      g.p[1].ld16 = 3 * d;
-    }
-    {
-      AttnArgs& a = P->attn[l];
-      memset(&a, 0, sizeof(a));
-      a.key_mask = P->key_mask;
-      a.out = P->attn16;
-      a.lse = nullptr;
-      a.scale = qscale;  // torch MHA: q * dh**-0.5 before q k^T
-      a.B = P->B;
-      a.L = P->L;
-      a.H = P->H;
-      a.dh = P->dh;
-      a.d = d;
-      a.fmt = fmt;
-      if (P->dh == 64 || P->dh == 128)
-        rc |= make_tmap_2d(&a.tm_qkv, P->qkv16, (uint64_t)P->M, (uint64_t)3 * d, (uint64_t)3 * d, 128, 64);
-    }
-    {
-      GemmGroup& g = P->g_out[l];
-      memset(&g, 0, sizeof(g));
-      g.num = 1;
-      g.fmt = fmt;
-      rc |= setup_linear(g.p[0], P->attn16, P->M, d, d, W16(lp.w_out), d, d, P->bn_out);
-      g.p[0].bias = F32(lp.b_out);
-      g.p[0].rps_in = P->L;
-      g.p[0].rps_out = P->L;
-      g.p[0].out16 = P->br16;  // DropPath-scaled branch; the LayerNorm kernel adds it to the fp32 residual stream
-      g.p[0].ld16 = d;
-    }
-    {
-      GemmGroup& g = P->g_ffn1[l];
-      memset(&g, 0, sizeof(g));
-      g.num = 1;
-      g.fmt = fmt;
-      rc |= setup_linear(g.p[0], P->x16, P->M, d, d, W16(lp.w1), ff, d, P->bn_ffn1);
-      g.p[0].bias = F32(lp.b1);
-      g.p[0].act = ACT_GELU;
-      g.p[0].out16 = P->h16;
-      g.p[0].ld16 = ff;
-    }
-    {
-      GemmGroup& g = P->g_ffn2[l];
-      memset(&g, 0, sizeof(g));
-      g.num = 1;
-      g.fmt = fmt;
-      rc |= setup_linear(g.p[0], P->h16, P->M, ff, ff, W16(lp.w2), d, ff, P->bn_ffn2);
-      g.p[0].bias = F32(lp.b2);
-      g.p[0].rps_in = P->L;
-      g.p[0].rps_out = P->L;
-      g.p[0].out16 = P->br16;
-      g.p[0].ld16 = d;
-    }
-  }
-  // ---- conv heads (k=3, pad=1) as 3-tap GEMMs over the separated layout ----
-  if (!rc) {
-    auto conv_problem = [&](GemmProblem& p, const uint16_t* A, int lda, const uint16_t* W, int N, const float* bias,
-                            uint16_t* out, int ldo, int bn) -> int {
-      init_problem(p);
-      p.M = P->Mh;
-      p.N = N;
-      p.taps = 3;
-      p.kblk_per_tap = d / 64;
-      // A tile row for tap t: buffer row m0 + t  (buffer row = logical row + 1)
-      p.ca = OperandCoord{0, 0, 0, 1, 0, 1, 1, 0};
-      // W2 [N, 3d]: column tap*d + k
-      p.cb = OperandCoord{0, 0, d, 1, 0, 1, 0, 0};
-      int r = make_tmap_2d(&p.tm_a, A, (uint64_t)P->Mh + 2, (uint64_t)d, (uint64_t)lda, GEMM_BM, 64);
-      r |= make_tmap_2d(&p.tm_b, W, (uint64_t)N, (uint64_t)3 * d, (uint64_t)3 * d, (uint32_t)bn, 64);
-      p.b_box_rows = bn;
-      p.bias = bias;
-      p.act = ACT_RELU;
-      p.rps_in = P->Lv + 1;
-      p.rps_out = P->Lv + 1;
-      p.row_off = 1;
-      p.zero_sep = 1;
-      p.out16 = out;
-      p.ld16 = ldo;
-      return r;
-    };
-    memset(&P->g_conv1, 0, sizeof(GemmGroup));
-    P->g_conv1.num = 1;
-    P->g_conv1.fmt = fmt;
-    rc |= conv_problem(P->g_conv1.p[0], P->hA, d, W16(Lw.conv1_w), 2 * d, F32(Lw.conv1_b), P->h1, 2 * d, P->bn_conv1);
-    memset(&P->g_conv2, 0, sizeof(GemmGroup));
-    P->g_conv2.num = 2;
-    P->g_conv2.fmt = fmt;
-    rc |= conv_problem(P->g_conv2.p[0], P->h1, 2 * d, W16(Lw.conv2c_w), d, F32(Lw.conv2c_b), P->hc2, d, P->bn_conv2);
-    rc |= conv_problem(P->g_conv2.p[1], P->h1 + d, 2 * d, W16(Lw.conv2s_w), d, F32(Lw.conv2s_b), P->hs2, d, P->bn_conv2);
-  }
-  if (rc) {
-    delete P;
-    return 1;
-  }
+  // per-launch tile widths: fill the SMs with as little wave quantisation as possible
+  const int sms = P->num_sms, M = P->M, Mh = P->Mh;
+  for (int i = 0; i < cfg->n_input_proj; ++i)
+    P->bn_proj[i] = tile_for(sms, 16, 1, MNK{P->Mv, d, P->lay.vid[i].kpad}, MNK{P->Mt, d, P->lay.txt[i].kpad}).bn;
+  P->bn_qkv = tile_for(sms, 16, 1, MNK{M, 2 * d, d}, MNK{M, d, d}).bn;
+  P->bn_out = tile_for(sms, 16, 1, MNK{M, d, d}).bn;
+  P->bn_ffn1 = tile_for(sms, 16, 1, MNK{M, ff, d}).bn;
+  P->bn_ffn2 = tile_for(sms, 16, 1, MNK{M, d, ff}).bn;
+  P->bn_conv1 = tile_for(sms, 16, 1, MNK{Mh, 2 * d, 3 * d}).bn;
+  P->bn_conv2 = tile_for(sms, 16, 1, MNK{Mh, d, 3 * d}, MNK{Mh, d, 3 * d}).bn;
   P->launches = 1 + 3 * cfg->n_input_proj + 7 * cfg->enc_layers + 6;
   *out = P;
   return 0;
@@ -492,34 +303,48 @@ int univtg_plan_read_profile(univtg_plan* plan, float* ms, int32_t* kinds, int32
 int univtg_forward_num_launches(const univtg_plan* plan) { return plan ? plan->launches : -1; }
 int64_t univtg_launch_count(void) { return (int64_t)*uv::launch_counter(); }
 
-int univtg_forward(univtg_plan* P, const float* src_txt, const float* src_txt_mask, const float* src_vid,
-                   const float* src_vid_mask, const float* droppath_scale, float* pred_logits, float* pred_spans,
-                   float* vid_mem_proj, float* txt_mem_proj, float* saliency_scores, void* stream) {
-  if (!P || !src_txt || !src_txt_mask || !src_vid || !src_vid_mask || !pred_logits || !pred_spans || !vid_mem_proj ||
-      !txt_mem_proj || !saliency_scores) {
-    set_error("univtg_forward: null argument");
-    return 1;
-  }
-  cudaStream_t st = (cudaStream_t)stream;
+}  // extern "C"
+
+int run_forward(univtg_plan* P, const FwdBufs& W, const float* src_txt, const float* src_txt_mask, const float* src_vid,
+                const float* src_vid_mask, const float* droppath_scale, const float* const* drop_masks, const univtg_rng* rng,
+                float* pred_logits, float* pred_spans, float* vid_mem_proj, float* txt_mem_proj, float* saliency_scores,
+                cudaStream_t st) {
   const univtg_config& c = P->cfg;
   const PackedLayout& Lw = P->lay;
   const uint8_t* pk = P->packed;
+  auto W16 = [&](size_t off) { return reinterpret_cast<const uint16_t*>(pk + off); };
   auto F32 = [&](size_t off) { return reinterpret_cast<const float*>(pk + off); };
-  const int d = P->d, fmt = c.operand_format;
+  const int d = P->d, ff = P->ff, fmt = c.operand_format, M = P->M, L = P->L, Lv = P->Lv, Lt = P->Lt, sms = P->num_sms;
   int rc = 0;
+  GemmGroup g;
+  auto group = [&](int num) {
+    memset(&g, 0, sizeof(g));
+    g.num = num;
+    g.fmt = fmt;
+  };
+  // every launch is followed by a profiling mark of its kind: 0 row kernel, 1 tensor-core GEMM, 2 attention
+  auto marked = [&](int r, int kind) {
+    if (r == 0) prof_mark(P, st, kind);
+    return r;
+  };
+
+  // train-mode randomness: explicit tensors (the caller drew them, e.g. with the reference's torch calls) win over `rng`
+  const bool dp_rng = droppath_scale == nullptr && rng != nullptr && rng->droppath > 0.f;
+  const bool drop_rng = drop_masks == nullptr && rng != nullptr && rng->input_dropout > 0.f;
   prof_begin(P, st);
-
-  rc = launch_sine_pos(src_vid_mask, src_txt_mask, P->dim_t, P->pos, P->key_mask, P->B, P->Lv, P->Lt, d, st);
+  rc = launch_sine_pos(src_vid_mask, src_txt_mask, P->dim_t, W.pos, W.key_mask, P->B, Lv, Lt, d, st, dp_rng ? W.dp_scale : nullptr,
+                       W.dp_scale ? 2 * c.enc_layers : 0, rng ? rng->seed : 0ull, rng ? 1.0f - rng->droppath : 1.f);
+  rc = marked(rc, 0);
   if (rc) return rc;
-  prof_mark(P, st, 0);
+  if (dp_rng) droppath_scale = W.dp_scale;
 
-  // ---- input projectors (LinearLayer: LN -> Dropout(eval: identity) -> Linear -> ReLU) ----
+  // ---- input projectors (LinearLayer: LN -> Dropout -> Linear -> ReLU): one grouped GEMM per depth (video + text) ----
   for (int i = 0; i < c.n_input_proj; ++i) {
     for (int s = 0; s < 2; ++s) {
       const ProjPacked& pp = s == 0 ? Lw.vid[i] : Lw.txt[i];
       LnArgs a;
       memset(&a, 0, sizeof(a));
-      a.in = i == 0 ? (s == 0 ? src_vid : src_txt) : (s == 0 ? P->p_vid32 : P->p_txt32);
+      a.in = i == 0 ? (s == 0 ? src_vid : src_txt) : (s == 0 ? W.p_vid32[i - 1] : W.p_txt32[i - 1]);
       if (i == 0 && P->in_fmt != 0) {
         a.in16 = reinterpret_cast<const uint16_t*>(a.in);
         a.in_fmt = P->in_fmt - 1;
@@ -531,104 +356,216 @@ int univtg_forward(univtg_plan* P, const float* src_txt, const float* src_txt_ma
       a.beta = F32(pp.ln_b);
       a.eps = 1e-5f;
       a.fmt = fmt;
-      a.out16 = s == 0 ? P->a_vid[i] : P->a_txt[i];
+      a.out16 = s == 0 ? W.a_vid[i] : W.a_txt[i];
       a.ld16 = pp.kpad;
-      rc = launch_layernorm(a, st);
+      a.mul32 = drop_masks ? drop_masks[s * c.n_input_proj + i] : nullptr;
+      if (drop_rng) a.drop = make_drop_spec(rng->seed, (unsigned int)(s * c.n_input_proj + i), rng->input_dropout);
+      a.mean_out = s == 0 ? W.pmean_v[i] : W.pmean_t[i];
+      a.rstd_out = s == 0 ? W.prstd_v[i] : W.prstd_t[i];
+      rc = marked(launch_layernorm(a, st), 0);
       if (rc) return rc;
-      prof_mark(P, st, 0);
     }
-    GemmGroup g = P->g_proj[i];
-    if (i == c.n_input_proj - 1) g.p[0].out32_id = vid_mem_proj;
-    rc = launch_gemm_group(g, P->bn_proj[i], P->num_sms, st);
+    group(2);
+    const bool last = (i == c.n_input_proj - 1);
+    const int bn = P->bn_proj[i];
+    GemmProblem& pv = g.p[0];
+    GemmProblem& pt = g.p[1];
+    rc |= setup_linear(pv, W.a_vid[i], P->Mv, Lw.vid[i].kpad, Lw.vid[i].kpad, W16(Lw.vid[i].w16), d, Lw.vid[i].kpad, bn);
+    rc |= setup_linear(pt, W.a_txt[i], P->Mt, Lw.txt[i].kpad, Lw.txt[i].kpad, W16(Lw.txt[i].w16), d, Lw.txt[i].kpad, bn);
     if (rc) return rc;
-    prof_mark(P, st, 1);
+    pv.bias = F32(Lw.vid[i].bias);
+    pt.bias = F32(Lw.txt[i].bias);
+    if (!last) {
+      pv.act = pt.act = ACT_RELU;
+      pv.out32 = W.p_vid32[i];
+      pt.out32 = W.p_txt32[i];
+      pv.ld32 = pt.ld32 = d;
+    } else {
+      // video tokens -> stream rows b*L + l; text tokens -> rows b*L + Lv + l   (cat on the sequence axis, univtg.py:119)
+      pv.rps_in = Lv;
+      pv.rps_out = L;
+      pt.rps_in = Lt;
+      pt.rps_out = L;
+      pt.row_off = Lv;
+      pv.out32 = pt.out32 = W.x32;
+      pv.ld32 = pt.ld32 = d;
+      pv.out16 = pt.out16 = W.xin16[0];
+      pv.out16p = pt.out16p = W.xpos16[0];
+      pv.ld16 = pt.ld16 = d;
+      pv.addtab = W.pos;
+      pv.ld_addtab = d;
+      pv.out32_id = vid_mem_proj;
+      pt.out32_id = W.txtproj32;
+      pv.ld32_id = pt.ld32_id = d;
+    }
+    rc = marked(launch_gemm_group(g, bn, sms, st), 1);
+    if (rc) return rc;
   }
 
   // ---- encoder layers (post-norm; TransformerEncoderLayer.forward_post) ----
   for (int l = 0; l < c.enc_layers; ++l) {
     const LayerPacked& lp = Lw.layer[l];
-    rc = launch_gemm_group(P->g_qkv[l], P->bn_qkv, P->num_sms, st);
+    // q = k = x + pos -> columns [0, 2d) of qkv16; v = x -> columns [2d, 3d)   (in_proj rows: Wq, Wk, Wv)
+    group(2);
+    rc |= setup_linear(g.p[0], W.xpos16[l], M, d, d, W16(lp.w_in), 2 * d, d, P->bn_qkv);
+    rc |= setup_linear(g.p[1], W.xin16[l], M, d, d, W16(lp.w_in) + (size_t)2 * d * d, d, d, P->bn_qkv);
     if (rc) return rc;
-    prof_mark(P, st, 1);
-    if (P->dh == 64 || P->dh == 128) rc = launch_attention(P->attn[l], st);
-    else rc = launch_attention_simt(P->attn[l], P->qkv16, st);
+    g.p[0].bias = F32(lp.b_in);
+    g.p[0].out16 = W.qkv16[l];
+    g.p[0].ld16 = 3 * d;
+    g.p[1].bias = F32(lp.b_in) + 2 * d;
+    g.p[1].out16 = W.qkv16[l] + 2 * d;
+    g.p[1].ld16 = 3 * d;
+    rc = marked(launch_gemm_group(g, P->bn_qkv, sms, st), 1);
     if (rc) return rc;
-    prof_mark(P, st, 2);
     {
-      GemmGroup g = P->g_out[l];
-      g.p[0].row_scale = droppath_scale ? droppath_scale + (size_t)(2 * l) * P->B : nullptr;
-      rc = launch_gemm_group(g, P->bn_out, P->num_sms, st);
+      AttnArgs a;
+      memset(&a, 0, sizeof(a));
+      a.key_mask = W.key_mask;
+      a.out = W.attn16[l];
+      a.lse = W.lse[l];
+      a.scale = 1.0f / sqrtf((float)P->dh);  // torch MHA: q * dh**-0.5 before q k^T
+      a.B = P->B;
+      a.L = L;
+      a.H = P->H;
+      a.dh = P->dh;
+      a.d = d;
+      a.fmt = fmt;
+      if (P->dh == 64 || P->dh == 128) {
+        if (make_tmap_2d(&a.tm_qkv, W.qkv16[l], (uint64_t)M, (uint64_t)3 * d, (uint64_t)3 * d, 128, 64)) return 1;
+        rc = launch_attention(a, st);
+      } else {
+        rc = launch_attention_simt(a, W.qkv16[l], st);
+      }
+      rc = marked(rc, 2);
       if (rc) return rc;
-      prof_mark(P, st, 1);
     }
+    group(1);
+    rc = setup_linear(g.p[0], W.attn16[l], M, d, d, W16(lp.w_out), d, d, P->bn_out);
+    if (rc) return rc;
+    g.p[0].bias = F32(lp.b_out);
+    g.p[0].rps_in = L;
+    g.p[0].rps_out = L;
+    g.p[0].row_scale = droppath_scale ? droppath_scale + (size_t)(2 * l) * P->B : nullptr;
+    g.p[0].out16 = W.br16;  // DropPath-scaled branch; the LayerNorm kernel adds it to the fp32 residual stream
+    g.p[0].ld16 = d;
+    rc = marked(launch_gemm_group(g, P->bn_out, sms, st), 1);
+    if (rc) return rc;
     {
       LnArgs a;
       memset(&a, 0, sizeof(a));
-      a.in = P->x32;
+      a.in = W.x32;
       a.ld_in = d;
-      a.add16 = P->br16;
+      a.add16 = W.br16;
       a.ld_add16 = d;
-      a.rows = P->M;
+      a.sum_out = W.y1[l];
+      a.rows = M;
       a.d = d;
       a.gamma = F32(lp.n1w);
       a.beta = F32(lp.n1b);
       a.eps = 1e-5f;
       a.fmt = fmt;
-      a.out32 = P->x32;
-      a.out16 = P->x16;
+      a.out32 = W.x1_32;
+      a.out16 = W.x1_16[l];
       a.ld16 = d;
-      rc = launch_layernorm(a, st);
+      a.mean_out = W.mean1[l];
+      a.rstd_out = W.rstd1[l];
+      rc = marked(launch_layernorm(a, st), 0);
       if (rc) return rc;
-      prof_mark(P, st, 0);
     }
-    rc = launch_gemm_group(P->g_ffn1[l], P->bn_ffn1, P->num_sms, st);
+    group(1);
+    rc = setup_linear(g.p[0], W.x1_16[l], M, d, d, W16(lp.w1), ff, d, P->bn_ffn1);
     if (rc) return rc;
-    prof_mark(P, st, 1);
-    {
-      GemmGroup g = P->g_ffn2[l];
-      g.p[0].row_scale = droppath_scale ? droppath_scale + (size_t)(2 * l + 1) * P->B : nullptr;
-      rc = launch_gemm_group(g, P->bn_ffn2, P->num_sms, st);
-      if (rc) return rc;
-      prof_mark(P, st, 1);
+    g.p[0].bias = F32(lp.b1);
+    g.p[0].act = ACT_GELU;
+    g.p[0].out16 = W.h16[l];
+    g.p[0].ld16 = ff;
+    if (W.dgelu16[l]) {
+      g.p[0].dact16 = W.dgelu16[l];
+      g.p[0].ld_dact = ff;
     }
+    rc = marked(launch_gemm_group(g, P->bn_ffn1, sms, st), 1);
+    if (rc) return rc;
+    group(1);
+    rc = setup_linear(g.p[0], W.h16[l], M, ff, ff, W16(lp.w2), d, ff, P->bn_ffn2);
+    if (rc) return rc;
+    g.p[0].bias = F32(lp.b2);
+    g.p[0].rps_in = L;
+    g.p[0].rps_out = L;
+    g.p[0].row_scale = droppath_scale ? droppath_scale + (size_t)(2 * l + 1) * P->B : nullptr;
+    g.p[0].out16 = W.br16;
+    g.p[0].ld16 = d;
+    rc = marked(launch_gemm_group(g, P->bn_ffn2, sms, st), 1);
+    if (rc) return rc;
     {
       LnArgs a;
       memset(&a, 0, sizeof(a));
-      a.in = P->x32;
+      a.in = W.x1_32;
       a.ld_in = d;
-      a.add16 = P->br16;
+      a.add16 = W.br16;
       a.ld_add16 = d;
-      a.rows = P->M;
+      a.sum_out = W.y2[l];
+      a.rows = M;
       a.d = d;
       a.gamma = F32(lp.n2w);
       a.beta = F32(lp.n2b);
       a.eps = 1e-5f;
       a.fmt = fmt;
-      a.L = P->L;
-      a.Lv = P->Lv;
-      a.out32 = P->x32;
-      a.out16 = P->x16;
-      a.out16p = P->xpos16;
+      a.L = L;
+      a.Lv = Lv;
+      a.out32 = W.x32;
+      a.out16 = W.xin16[l + 1];
+      a.out16p = W.xpos16[l + 1];
       a.ld16 = d;
-      a.pos = P->pos;
-      if (l == c.enc_layers - 1) a.outc = P->hA;  // vid_mem = memory[:, :Lv] feeds the conv heads
-      rc = launch_layernorm(a, st);
+      a.pos = W.pos;
+      a.mean_out = W.mean2[l];
+      a.rstd_out = W.rstd2[l];
+      if (l == c.enc_layers - 1) a.outc = W.hA;  // vid_mem = memory[:, :Lv] feeds the conv heads
+      rc = marked(launch_layernorm(a, st), 0);
       if (rc) return rc;
-      prof_mark(P, st, 0);
     }
   }
 
-  // ---- heads ----
-  rc = launch_gemm_group(P->g_conv1, P->bn_conv1, P->num_sms, st);
+  // ---- heads: conv layers (k=3, pad=1) as 3-tap GEMMs over the separated layout, then the final conv and the pooling ----
+  auto conv_problem = [&](GemmProblem& p, const uint16_t* A, int lda, const uint16_t* Wc, int N, const float* bias, uint16_t* out,
+                          int ldo, int bn) -> int {
+    init_problem(p);
+    p.M = P->Mh;
+    p.N = N;
+    p.taps = 3;
+    p.kblk_per_tap = d / 64;
+    // A tile row for tap t: buffer row m0 + t  (buffer row = logical row + 1)
+    p.ca = OperandCoord{0, 0, 0, 1, 0, 1, 1, 0};
+    // W2 [N, 3d]: column tap*d + k
+    p.cb = OperandCoord{0, 0, d, 1, 0, 1, 0, 0};
+    int r = make_tmap_2d(&p.tm_a, A, (uint64_t)P->Mh + 2, (uint64_t)d, (uint64_t)lda, GEMM_BM, 64);
+    r |= make_tmap_2d(&p.tm_b, Wc, (uint64_t)N, (uint64_t)3 * d, (uint64_t)3 * d, (uint32_t)bn, 64);
+    p.b_box_rows = bn;
+    p.bias = bias;
+    p.act = ACT_RELU;
+    p.rps_in = Lv + 1;
+    p.rps_out = Lv + 1;
+    p.row_off = 1;
+    p.zero_sep = 1;
+    p.out16 = out;
+    p.ld16 = ldo;
+    return r;
+  };
+  group(1);
+  rc = conv_problem(g.p[0], W.hA, d, W16(Lw.conv1_w), 2 * d, F32(Lw.conv1_b), W.h1, 2 * d, P->bn_conv1);
   if (rc) return rc;
-  prof_mark(P, st, 1);
-  rc = launch_gemm_group(P->g_conv2, P->bn_conv2, P->num_sms, st);
+  rc = marked(launch_gemm_group(g, P->bn_conv1, sms, st), 1);
   if (rc) return rc;
-  prof_mark(P, st, 1);
+  group(2);
+  rc |= conv_problem(g.p[0], W.h1, 2 * d, W16(Lw.conv2c_w), d, F32(Lw.conv2c_b), W.hc2, d, P->bn_conv2);
+  rc |= conv_problem(g.p[1], W.h1 + d, 2 * d, W16(Lw.conv2s_w), d, F32(Lw.conv2s_b), W.hs2, d, P->bn_conv2);
+  if (rc) return rc;
+  rc = marked(launch_gemm_group(g, P->bn_conv2, sms, st), 1);
+  if (rc) return rc;
   {
     HeadFinalArgs a;
-    a.h_cls = P->hc2;
-    a.h_span = P->hs2;
+    a.h_cls = W.hc2;
+    a.h_span = W.hs2;
     a.w_cls = F32(Lw.conv3c_w);
     a.w_span = F32(Lw.conv3s_w);
     a.b_cls = F32(Lw.conv3c_b);
@@ -636,33 +573,49 @@ int univtg_forward(univtg_plan* P, const float* src_txt, const float* src_txt_ma
     a.pred_logits = pred_logits;
     a.pred_spans = pred_spans;
     a.B = P->B;
-    a.Lv = P->Lv;
+    a.Lv = Lv;
     a.d = d;
     a.fmt = fmt;
-    rc = launch_conv_head_final(a, st);
+    rc = marked(launch_conv_head_final(a, st), 0);
     if (rc) return rc;
-    prof_mark(P, st, 0);
   }
   {
     PoolSalArgs a;
-    a.x_txt = P->txtproj32;
+    a.x_txt = W.txtproj32;
     a.x_vid = vid_mem_proj;
     a.txt_mask = src_txt_mask;
     a.vid_mask = src_vid_mask;
     a.w = F32(Lw.pool_w);
     a.pooled = txt_mem_proj;
     a.saliency = saliency_scores;
-    a.alpha_out = nullptr;
-    a.logits_ws = P->pool_logits;
+    a.alpha_out = W.pool_alpha;
+    a.logits_ws = W.pool_logits;
     a.B = P->B;
-    a.Lt = P->Lt;
-    a.Lv = P->Lv;
+    a.Lt = Lt;
+    a.Lv = Lv;
     a.d = d;
-    rc = launch_pool_saliency(a, st);
+    rc = marked(launch_pool_saliency(a, st), 0);
     if (rc) return rc;
-    prof_mark(P, st, 0);
+  }
+  if (W.pred_logits) {  // keep the small outputs the backward needs (the caller owns the returned tensors and may free them)
+    cudaMemcpyAsync(W.pred_logits, pred_logits, (size_t)P->Mv * 4, cudaMemcpyDeviceToDevice, st);
+    cudaMemcpyAsync(W.pred_spans, pred_spans, (size_t)P->Mv * 8, cudaMemcpyDeviceToDevice, st);
   }
   return 0;
+}
+
+extern "C" {
+
+int univtg_forward(univtg_plan* P, const float* src_txt, const float* src_txt_mask, const float* src_vid,
+                   const float* src_vid_mask, const float* droppath_scale, float* pred_logits, float* pred_spans,
+                   float* vid_mem_proj, float* txt_mem_proj, float* saliency_scores, void* stream) {
+  if (!P || !src_txt || !src_txt_mask || !src_vid || !src_vid_mask || !pred_logits || !pred_spans || !vid_mem_proj ||
+      !txt_mem_proj || !saliency_scores) {
+    set_error("univtg_forward: null argument");
+    return 1;
+  }
+  return run_forward(P, make_infer_ws(P->cfg, P->shp, P->lay, P->ws), src_txt, src_txt_mask, src_vid, src_vid_mask, droppath_scale,
+                     nullptr, nullptr, pred_logits, pred_spans, vid_mem_proj, txt_mem_proj, saliency_scores, (cudaStream_t)stream);
 }
 
 // ------------------------------------------------------------------------------------------------

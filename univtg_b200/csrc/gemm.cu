@@ -849,10 +849,4 @@ TileChoice choose_tile(const int* Ms, const int* Ns, const int* kblocks, int num
   return best;
 }
 
-// Tile width only (no split-K), K = 1024 assumed when the caller has no k extents at hand.
-int choose_bn(const int* Ms, const int* Ns, const int* kblocks, int num, int num_sms, int step) {
-  int kb16[GEMM_MAX_GROUP] = {16, 16, 16, 16};
-  return choose_tile(Ms, Ns, kblocks ? kblocks : kb16, num, num_sms, step, 1).bn;
-}
-
 }  // namespace uv

@@ -1,5 +1,5 @@
-// Shared between api.cu (inference orchestration) and train.cu (training forward/backward): packed-weight layout,
-// workspace layout and the plan object behind the opaque univtg_plan handle.
+// Shared between api.cu (forward orchestration) and train.cu (training workspace and backward): packed-weight layout,
+// the buffers the forward writes, and the plan object behind the opaque univtg_plan handle.
 #pragma once
 #include <math.h>
 #include <stdio.h>
@@ -259,6 +259,30 @@ struct Packer {
 }  // namespace
 
 // ------------------------------------------------------------------------------------------------
+// buffers the forward writes
+// ------------------------------------------------------------------------------------------------
+// Training keeps one buffer per layer and the statistics the backward needs (TrainWs, train.cu).  Inference
+// (make_infer_ws) lets every per-layer entry alias one buffer and leaves the training-only entries null.
+struct FwdBufs {
+  uint16_t *a_vid[3], *a_txt[3];   // LN'd 16-bit projector inputs
+  float *pmean_v[3], *prstd_v[3], *pmean_t[3], *prstd_t[3];  // projector LayerNorm statistics (training)
+  float *p_vid32[3], *p_txt32[3];  // output of projector layer i (input of LayerNorm i+1)
+  float* txtproj32;                // [Mt, d] projected text tokens (+type embedding)
+  float* pool_alpha;               // [B, Lt] pooling softmax weights (training)
+  float *pos, *key_mask, *pool_logits;
+  float* dp_scale;                 // [2 * enc_layers, B] DropPath scales drawn in-kernel (training; reused by the backward)
+  uint16_t *xin16[17], *xpos16[17];  // operands of layer l's in-projections (index enc_layers: output of the last layer)
+  uint16_t *qkv16[16], *attn16[16], *x1_16[16], *h16[16];
+  float *lse[16], *y1[16], *mean1[16], *rstd1[16], *y2[16], *mean2[16], *rstd2[16];  // training
+  uint16_t* dgelu16[16];           // GELU'(pre-activation) of the FFN, written by FFN1's epilogue beside h16 (training)
+  float *x32, *x1_32;              // fp32 residual stream before / after LayerNorm 1 (the same buffer in inference)
+  uint16_t *hA, *h1, *hc2, *hs2;   // conv-head buffers (separated layout)
+  uint16_t* br16;                  // DropPath-scaled residual branch (out-proj / FFN2 output)
+  float *pred_logits, *pred_spans;  // copies of the outputs the backward needs (training)
+  size_t total;
+};
+
+// ------------------------------------------------------------------------------------------------
 // plan
 // ------------------------------------------------------------------------------------------------
 constexpr int kMaxMarks = 640;
@@ -273,22 +297,7 @@ struct univtg_plan {
   int in_fmt;       // src_vid / src_txt element type: 0 f32 (reference collate), 1 fp16, 2 bf16 (packed feature shards)
   int num_sms_bwd;  // SM budget of the backward's GEMM launches (0: num_sms); see univtg_plan_set_backward_sm_budget
   int B, Lv, Lt, L, d, ff, H, dh, M, Mv, Mt, Mh;
-  // workspace pointers
-  uint16_t *a_vid[3], *a_txt[3];  // LN'd 16-bit projector inputs
-  float *p_vid32, *p_txt32;       // fp32 projector hidden (between projector layers)
-  float* txtproj32;               // [Mt, d] projected text tokens (+type embedding)
-  float* pos;                     // [Mv, d]
-  float* key_mask;                // [B, L]
-  float* pool_logits;             // [B, Lt]
-  float* x32;                     // fp32 residual stream (LayerNorm works in place on it)
-  uint16_t *x16, *xpos16, *qkv16, *attn16, *h16, *br16;  // br16: DropPath-scaled residual branch (out-proj / FFN2 output)
-  uint16_t *hA, *h1, *hc2, *hs2;  // conv-head buffers (separated layout)
-  // launch descriptors
-  GemmGroup g_proj[3];
-  GemmGroup g_qkv[16], g_out[16], g_ffn1[16], g_ffn2[16];
-  GemmGroup g_conv1, g_conv2;
-  AttnArgs attn[16];
-  int bn_proj[3], bn_main;  // tile widths chosen per launch (choose_bn)
+  int bn_proj[3];  // tile widths of the forward's GEMM launches (tile_for)
   int bn_qkv, bn_out, bn_ffn1, bn_ffn2, bn_conv1, bn_conv2;
   int launches;
   // optional "gradients of stage k are final" events recorded by univtg_backward (gradient-exchange overlap)
@@ -318,8 +327,9 @@ inline void prof_mark(univtg_plan* P, cudaStream_t st, int kind) {
   P->mark_kind[i] = kind;
   P->n_marks = i + 1;
 }
-// training path: a GEMM / attention launch bracketed by two marks, so that the interval ending at the second mark is that kernel
-// alone (the interval ending at the first one - kind 3 - collects whatever ran since the previous mark)
+// The forward records a mark after every launch.  The backward brackets each GEMM / attention launch by two marks, so that the
+// interval ending at the second mark is that kernel alone (the interval ending at the first one - kind 3 - collects whatever ran
+// since the previous mark).
 inline int gemm_launch(univtg_plan* P, GemmGroup& g, int bn, int sms, cudaStream_t st) {
   prof_mark(P, st, 3);
   const int rc = launch_gemm_group(g, bn, sms, st);
@@ -342,61 +352,98 @@ void init_problem(GemmProblem& p) {
   p.cb = OperandCoord{0, 0, 0, 1, 0, 1, 0, 0};
 }
 
-// K-major linear problem: A [M, K] (pitch lda), W [N, K] (pitch ldw), K multiple of 64.
-int setup_linear(GemmProblem& p, const uint16_t* A, int M, int K, int lda, const uint16_t* W, int N, int ldw, int bn) {
+struct Mat16 {  // row-major 16-bit matrix view
+  const uint16_t* p;
+  int rows, cols, ld;
+};
+
+// C[M,N] = sum_k A(m,k) B(n,k).  a_mn: A is stored [K rows, M cols] (else [M rows, K cols]); same for B.
+int setup_gemm(GemmProblem& p, Mat16 A, int a_mn, Mat16 B, int b_mn, int M, int N, int K, int bn) {
   init_problem(p);
   p.M = M;
   p.N = N;
-  p.kblk_per_tap = K / 64;
-  if (K % 64 != 0) {
-    set_error("setup_linear: K %d not a multiple of 64", K);
-    return 1;
+  p.a_mn = a_mn;
+  p.b_mn = b_mn;
+  p.kblk_per_tap = (K + 63) / 64;
+  int rc = 0;
+  if (!a_mn) {
+    rc |= make_tmap_2d(&p.tm_a, A.p, (uint64_t)A.rows, (uint64_t)A.cols, (uint64_t)A.ld, GEMM_BM, 64);
+  } else {
+    rc |= make_tmap_2d(&p.tm_a, A.p, (uint64_t)A.rows, (uint64_t)A.cols, (uint64_t)A.ld, 64, 64);
+    p.ca = OperandCoord{0, 1, 0, 0, 0, 0, 0, 1};
   }
-  if (make_tmap_2d(&p.tm_a, A, (uint64_t)M, (uint64_t)K, (uint64_t)lda, GEMM_BM, 64)) return 1;
-  if (make_tmap_2d(&p.tm_b, W, (uint64_t)N, (uint64_t)K, (uint64_t)ldw, (uint32_t)bn, 64)) return 1;
-  p.b_box_rows = bn;
-  return 0;
+  if (!b_mn) {
+    rc |= make_tmap_2d(&p.tm_b, B.p, (uint64_t)B.rows, (uint64_t)B.cols, (uint64_t)B.ld, (uint32_t)bn, 64);
+    p.b_box_rows = bn;
+  } else {
+    rc |= make_tmap_b_mn(p, B.p, (uint64_t)B.rows, (uint64_t)B.cols, (uint64_t)B.ld, bn);
+    p.cb = OperandCoord{0, 1, 0, 0, 0, 0, 0, 1};
+  }
+  return rc;
 }
 
-}  // namespace
+// K-major linear problem: A [M, K] (pitch lda), W [N, K] (pitch ldw).
+inline int setup_linear(GemmProblem& p, const uint16_t* A, int M, int K, int lda, const uint16_t* W, int N, int ldw, int bn) {
+  return setup_gemm(p, Mat16{A, M, K, lda}, 0, Mat16{W, N, K, ldw}, 0, M, N, K, bn);
+}
 
-
-namespace {
-
-struct WsLayout {
-  size_t a_vid[3], a_txt[3], p_vid32, p_txt32, txtproj32, pos, key_mask, pool_logits, x32, br16, x16, xpos16, qkv16, attn16, h16, hA,
-      h1, hc2, hs2, total;
+// Tile width + split-K factor for one grouped launch (cost model: choose_tile, gemm.cu).  K in elements; step 16 when every B
+// operand is K-major, 64 when one is MN-major; max_split = 1 for launches whose epilogue cannot accumulate.
+struct MNK {
+  int M, N, K;
 };
+inline TileChoice tile_for(int sms, int step, int max_split, MNK a, MNK b = MNK{0, 0, 0}, MNK c3 = MNK{0, 0, 0}) {
+  const int Ms[3] = {a.M, b.M, c3.M}, Ns[3] = {a.N, b.N, c3.N}, kb[3] = {(a.K + 63) / 64, (b.K + 63) / 64, (c3.K + 63) / 64};
+  const int num = c3.M > 0 ? 3 : (b.M > 0 ? 2 : 1);
+  return choose_tile(Ms, Ns, kb, num, sms, step, max_split);
+}
 
-WsLayout make_ws(const univtg_config& c, const univtg_shape& s, const PackedLayout& L) {
-  WsLayout w;
+// Inference workspace: one buffer per role, shared by all layers; LayerNorm 1 works in place on the residual stream.
+FwdBufs make_infer_ws(const univtg_config& c, const univtg_shape& s, const PackedLayout& L, uint8_t* base) {
+  FwdBufs w;
   memset(&w, 0, sizeof(w));
   Cursor cur;
   const size_t d = c.hidden_dim, ff = c.dim_feedforward;
   const size_t B = s.batch, Lv = s.l_vid, Lt = s.l_txt, Lc = Lv + Lt;
   const size_t M = B * Lc, Mv = B * Lv, Mt = B * Lt, Mh = B * (Lv + 1);
+  auto take16 = [&](size_t elems) { return reinterpret_cast<uint16_t*>(base + cur.take(elems * 2)); };
+  auto take32 = [&](size_t elems) { return reinterpret_cast<float*>(base + cur.take(elems * 4)); };
   for (int i = 0; i < c.n_input_proj; ++i) {
-    w.a_vid[i] = cur.take(Mv * L.vid[i].kpad * 2);
-    w.a_txt[i] = cur.take(Mt * L.txt[i].kpad * 2);
+    w.a_vid[i] = take16(Mv * L.vid[i].kpad);
+    w.a_txt[i] = take16(Mt * L.txt[i].kpad);
   }
-  w.p_vid32 = cur.take(Mv * d * 4);
-  w.p_txt32 = cur.take(Mt * d * 4);
-  w.txtproj32 = cur.take(Mt * d * 4);
-  w.pos = cur.take(Mv * d * 4);
-  w.key_mask = cur.take(B * Lc * 4);
-  w.pool_logits = cur.take(B * Lt * 4);
-  w.x32 = cur.take(M * d * 4);
-  w.br16 = cur.take(M * d * 2);
-  w.x16 = cur.take(M * d * 2);
-  w.xpos16 = cur.take(M * d * 2);
-  w.qkv16 = cur.take(M * 3 * d * 2);
-  w.attn16 = cur.take(M * d * 2);
-  w.h16 = cur.take(M * ff * 2);
-  w.hA = cur.take((Mh + 2) * d * 2);
-  w.h1 = cur.take((Mh + 2) * 2 * d * 2);
-  w.hc2 = cur.take((Mh + 2) * d * 2);
-  w.hs2 = cur.take((Mh + 2) * d * 2);
+  float* p_vid32 = take32(Mv * d);
+  float* p_txt32 = take32(Mt * d);
+  w.txtproj32 = take32(Mt * d);
+  w.pos = take32(Mv * d);
+  w.key_mask = take32(B * Lc);
+  w.pool_logits = take32(B * Lt);
+  w.x32 = w.x1_32 = take32(M * d);
+  w.br16 = take16(M * d);
+  uint16_t* x16 = take16(M * d);
+  uint16_t* xpos16 = take16(M * d);
+  uint16_t* qkv16 = take16(M * 3 * d);
+  uint16_t* attn16 = take16(M * d);
+  uint16_t* h16 = take16(M * ff);
+  w.hA = take16((Mh + 2) * d);
+  w.h1 = take16((Mh + 2) * 2 * d);
+  w.hc2 = take16((Mh + 2) * d);
+  w.hs2 = take16((Mh + 2) * d);
   w.total = cur.off;
+  for (int i = 0; i < c.n_input_proj; ++i) {
+    w.p_vid32[i] = p_vid32;
+    w.p_txt32[i] = p_txt32;
+  }
+  for (int l = 0; l <= c.enc_layers; ++l) {
+    w.xin16[l] = x16;
+    w.xpos16[l] = xpos16;
+  }
+  for (int l = 0; l < c.enc_layers; ++l) {
+    w.qkv16[l] = qkv16;
+    w.attn16[l] = attn16;
+    w.x1_16[l] = x16;
+    w.h16[l] = h16;
+  }
   return w;
 }
 
@@ -409,4 +456,12 @@ bool check_shape(const univtg_shape* s) {
 }
 
 }  // namespace
+
+// Reference Model.forward (model/univtg.py:105-155) over the buffers `W`, for univtg_forward and univtg_forward_train (api.cu).
+// drop_masks / rng: train-mode randomness as univtg_forward_train takes it (NULL at inference).  The training-only entries of `W`
+// that are non-null are written as well.
+int run_forward(univtg_plan* P, const FwdBufs& W, const float* src_txt, const float* src_txt_mask, const float* src_vid,
+                const float* src_vid_mask, const float* droppath_scale, const float* const* drop_masks, const univtg_rng* rng,
+                float* pred_logits, float* pred_spans, float* vid_mem_proj, float* txt_mem_proj, float* saliency_scores,
+                cudaStream_t st);
 

@@ -1,72 +1,18 @@
-// Training path of the C-ABI: forward that keeps what backward needs, the backward pass (SURVEY.md A.6, reference
-// main/train_vlp_ddp.py:56-64: outputs = model(...); losses.backward()) and the criterion entry points.
-// GEMM descriptors (tensor maps) are built per call here; shapes vary per training batch anyway (collate pads to the batch max).
+// Training path of the C-ABI: the training workspace, the forward that keeps what backward needs (run_forward, api.cu), the
+// backward pass (SURVEY.md A.6, reference main/train_vlp_ddp.py:56-64: outputs = model(...); losses.backward()) and the
+// criterion entry points.  GEMM descriptors (tensor maps) are built per call; shapes vary per training batch anyway (collate
+// pads to the batch max).
 #include <stdlib.h>
 
 #include "plan.h"
 
 namespace {
 
-struct Mat16 {  // row-major 16-bit matrix view
-  const uint16_t* p;
-  int rows, cols, ld;
-};
-
-// C[M,N] = sum_k A(m,k) B(n,k).  a_mn: A is stored [K rows, M cols] (else [M rows, K cols]); same for B.
-int setup_gemm(GemmProblem& p, Mat16 A, int a_mn, Mat16 B, int b_mn, int M, int N, int K, int bn) {
-  init_problem(p);
-  p.M = M;
-  p.N = N;
-  p.a_mn = a_mn;
-  p.b_mn = b_mn;
-  p.kblk_per_tap = (K + 63) / 64;
-  int rc = 0;
-  if (!a_mn) {
-    rc |= make_tmap_2d(&p.tm_a, A.p, (uint64_t)A.rows, (uint64_t)A.cols, (uint64_t)A.ld, GEMM_BM, 64);
-  } else {
-    rc |= make_tmap_2d(&p.tm_a, A.p, (uint64_t)A.rows, (uint64_t)A.cols, (uint64_t)A.ld, 64, 64);
-    p.ca = OperandCoord{0, 1, 0, 0, 0, 0, 0, 1};
-  }
-  if (!b_mn) {
-    rc |= make_tmap_2d(&p.tm_b, B.p, (uint64_t)B.rows, (uint64_t)B.cols, (uint64_t)B.ld, (uint32_t)bn, 64);
-    p.b_box_rows = bn;
-  } else {
-    rc |= make_tmap_b_mn(p, B.p, (uint64_t)B.rows, (uint64_t)B.cols, (uint64_t)B.ld, bn);
-    p.cb = OperandCoord{0, 1, 0, 0, 0, 0, 0, 1};
-  }
-  return rc;
-}
-
-// Tile width + split-K factor for one grouped launch (cost model: choose_tile, gemm.cu).  K in elements; step 64 when a B operand
-// is MN-major; max_split = 1 for launches whose epilogue cannot accumulate.
-struct MNK {
-  int M, N, K;
-};
-inline TileChoice tile_for(int sms, int step, int max_split, MNK a, MNK b = MNK{0, 0, 0}, MNK c3 = MNK{0, 0, 0}) {
-  const int Ms[3] = {a.M, b.M, c3.M}, Ns[3] = {a.N, b.N, c3.N}, kb[3] = {(a.K + 63) / 64, (b.K + 63) / 64, (c3.K + 63) / 64};
-  const int num = c3.M > 0 ? 3 : (b.M > 0 ? 2 : 1);
-  return choose_tile(Ms, Ns, kb, num, sms, step, max_split);
-}
-inline int bn_for(int sms, int step, MNK a, MNK b = MNK{0, 0, 0}) { return tile_for(sms, step, 1, a, b).bn; }
-
-struct TrainWs {
-  // ---- saved by the forward ----
-  uint16_t *a_vid[3], *a_txt[3];
-  float *pmean_v[3], *prstd_v[3], *pmean_t[3], *prstd_t[3];
-  float *p_vid32[3], *p_txt32[3];  // output of projector layer i (input of LayerNorm i+1)
-  float *txtproj32, *pool_alpha, *pos, *key_mask, *pool_logits;
-  float* dp_scale;  // [2 * enc_layers, B] DropPath scales drawn in-kernel by the forward (univtg_rng), reused by the backward
-  uint16_t *xin16[17], *xpos16[17];  // operands of layer l's in-projections (index enc_layers: unused tail)
-  uint16_t *qkv16[16], *attn16[16], *x1_16[16], *h16[16];
-  float *lse[16], *y1[16], *mean1[16], *rstd1[16], *y2[16], *mean2[16], *rstd2[16];
-  uint16_t* dgelu16[16];  // GELU'(pre-activation) of the FFN, written by FFN1's forward epilogue beside h16
-  float *x32, *x1_32;
-  uint16_t *hA, *h1, *hc2, *hs2, *br16;
-  float *pred_logits, *pred_spans, *vid_mem_proj, *txt_mem_proj;  // copies of the outputs the backward needs
-  // ---- backward scratch ----
+// The training workspace: what the forward writes (one buffer per layer, FwdBufs) and the backward's scratch.
+struct TrainWs : FwdBufs {
+  float *vid_mem_proj, *txt_mem_proj;  // reserved beside the forward's pred_logits / pred_spans copies; not read
   float *dx, *dy, *dqkv32, *delta, *dz, *dxt_pool, *dA_v, *dA_t, *wtap;
   uint16_t *dbr16, *dhpre16, *dO16, *dqkv16, *dhc2, *dhs2, *dh1, *dxv16, *dxt16;
-  size_t total;
 };
 
 TrainWs make_train_ws(const univtg_config& c, const univtg_shape& s, const PackedLayout& L, uint8_t* base) {
@@ -178,21 +124,20 @@ int univtg_prepare_workspace(const univtg_config* cfg, const univtg_shape* shape
   auto zero = [&](void* p, size_t bytes) {
     if (e == cudaSuccess) e = cudaMemsetAsync(p, 0, bytes, st);
   };
+  auto zero_heads = [&](const FwdBufs& w) {
+    zero(w.hA, (Mh + 2) * d * 2);
+    zero(w.h1, (Mh + 2) * 2 * d * 2);
+    zero(w.hc2, (Mh + 2) * d * 2);
+    zero(w.hs2, (Mh + 2) * d * 2);
+  };
   if (training_ws) {
     const TrainWs T = make_train_ws(*cfg, *shape, L, base);
-    zero(T.hA, (Mh + 2) * d * 2);
-    zero(T.h1, (Mh + 2) * 2 * d * 2);
-    zero(T.hc2, (Mh + 2) * d * 2);
-    zero(T.hs2, (Mh + 2) * d * 2);
+    zero_heads(T);
     zero(T.dhc2, (Mh + 2) * d * 2);
     zero(T.dhs2, (Mh + 2) * d * 2);
     zero(T.dh1, (Mh + 2) * 2 * d * 2);
   } else {
-    const WsLayout w = make_ws(*cfg, *shape, L);
-    zero(base + w.hA, (Mh + 2) * d * 2);
-    zero(base + w.h1, (Mh + 2) * 2 * d * 2);
-    zero(base + w.hc2, (Mh + 2) * d * 2);
-    zero(base + w.hs2, (Mh + 2) * d * 2);
+    zero_heads(make_infer_ws(*cfg, *shape, L, base));
   }
   if (e != cudaSuccess) {
     set_error("univtg_prepare_workspace: %s", cudaGetErrorString(e));
@@ -218,297 +163,10 @@ int univtg_forward_train(univtg_plan* P, void* ws, const float* src_txt, const f
     set_error("univtg_forward_train: null argument");
     return 1;
   }
-  cudaStream_t st = (cudaStream_t)stream;
-  const univtg_config& c = P->cfg;
-  const PackedLayout& Lw = P->lay;
-  const uint8_t* pk = P->packed;
-  auto F32 = [&](size_t off) { return reinterpret_cast<const float*>(pk + off); };
-  auto W16 = [&](size_t off) { return reinterpret_cast<const uint16_t*>(pk + off); };
-  const TrainWs T = make_train_ws(c, P->shp, Lw, reinterpret_cast<uint8_t*>(ws));
-  const int d = P->d, ff = P->ff, fmt = c.operand_format, M = P->M, Mv = P->Mv, Mt = P->Mt, Mh = P->Mh, L = P->L, Lv = P->Lv;
-  const int sms = P->num_sms;
-  int rc = 0;
-  GemmGroup g;
-
-  // train-mode randomness: explicit tensors (the caller drew them, e.g. with the reference's torch calls) win over `rng`
-  prof_begin(P, st);
-  const bool dp_rng = droppath_scale == nullptr && rng != nullptr && rng->droppath > 0.f;
-  const bool drop_rng = drop_masks == nullptr && rng != nullptr && rng->input_dropout > 0.f;
-  rc = launch_sine_pos(src_vid_mask, src_txt_mask, P->dim_t, T.pos, T.key_mask, P->B, Lv, P->Lt, d, st, dp_rng ? T.dp_scale : nullptr,
-                       2 * c.enc_layers, rng ? rng->seed : 0ull, rng ? 1.0f - rng->droppath : 1.f);
+  const TrainWs T = make_train_ws(P->cfg, P->shp, P->lay, reinterpret_cast<uint8_t*>(ws));
+  const int rc = run_forward(P, T, src_txt, src_txt_mask, src_vid, src_vid_mask, droppath_scale, drop_masks, rng, pred_logits,
+                             pred_spans, vid_mem_proj, txt_mem_proj, saliency_scores, (cudaStream_t)stream);
   if (rc) return rc;
-  if (dp_rng) droppath_scale = T.dp_scale;
-
-  // ---- input projectors ----
-  for (int i = 0; i < c.n_input_proj; ++i) {
-    for (int s = 0; s < 2; ++s) {
-      const ProjPacked& pp = s == 0 ? Lw.vid[i] : Lw.txt[i];
-      LnArgs a;
-      memset(&a, 0, sizeof(a));
-      a.in = i == 0 ? (s == 0 ? src_vid : src_txt) : (s == 0 ? T.p_vid32[i - 1] : T.p_txt32[i - 1]);
-      if (i == 0 && P->in_fmt != 0) {
-        a.in16 = reinterpret_cast<const uint16_t*>(a.in);
-        a.in_fmt = P->in_fmt - 1;
-      }
-      a.ld_in = pp.din;
-      a.rows = s == 0 ? Mv : Mt;
-      a.d = pp.din;
-      a.gamma = F32(pp.ln_w);
-      a.beta = F32(pp.ln_b);
-      a.eps = 1e-5f;
-      a.fmt = fmt;
-      a.out16 = s == 0 ? T.a_vid[i] : T.a_txt[i];
-      a.ld16 = pp.kpad;
-      a.mul32 = drop_masks ? drop_masks[s * c.n_input_proj + i] : nullptr;
-      if (drop_rng) a.drop = make_drop_spec(rng->seed, (unsigned int)(s * c.n_input_proj + i), rng->input_dropout);
-      a.mean_out = s == 0 ? T.pmean_v[i] : T.pmean_t[i];
-      a.rstd_out = s == 0 ? T.prstd_v[i] : T.prstd_t[i];
-      rc = launch_layernorm(a, st);
-      if (rc) return rc;
-    }
-    memset(&g, 0, sizeof(g));
-    g.num = 2;
-    g.fmt = fmt;
-    const bool last = (i == c.n_input_proj - 1);
-    rc |= setup_linear(g.p[0], T.a_vid[i], Mv, Lw.vid[i].kpad, Lw.vid[i].kpad, W16(Lw.vid[i].w16), d, Lw.vid[i].kpad, P->bn_proj[i]);
-    rc |= setup_linear(g.p[1], T.a_txt[i], Mt, Lw.txt[i].kpad, Lw.txt[i].kpad, W16(Lw.txt[i].w16), d, Lw.txt[i].kpad, P->bn_proj[i]);
-    if (rc) return rc;
-    g.p[0].bias = F32(Lw.vid[i].bias);
-    g.p[1].bias = F32(Lw.txt[i].bias);
-    if (!last) {
-      g.p[0].act = g.p[1].act = ACT_RELU;
-      g.p[0].out32 = T.p_vid32[i];
-      g.p[1].out32 = T.p_txt32[i];
-      g.p[0].ld32 = g.p[1].ld32 = d;
-    } else {
-      g.p[0].rps_in = Lv;
-      g.p[0].rps_out = L;
-      g.p[1].rps_in = P->Lt;
-      g.p[1].rps_out = L;
-      g.p[1].row_off = Lv;
-      for (int s = 0; s < 2; ++s) {
-        g.p[s].out32 = T.x32;
-        g.p[s].ld32 = d;
-        g.p[s].out16 = T.xin16[0];
-        g.p[s].out16p = T.xpos16[0];
-        g.p[s].ld16 = d;
-        g.p[s].ld32_id = d;
-      }
-      g.p[0].addtab = T.pos;
-      g.p[0].ld_addtab = d;
-      g.p[0].out32_id = vid_mem_proj;
-      g.p[1].out32_id = T.txtproj32;
-    }
-    rc = gemm_launch(P, g, P->bn_proj[i], sms, st);
-    if (rc) return rc;
-  }
-
-  // ---- encoder layers ----
-  for (int l = 0; l < c.enc_layers; ++l) {
-    const LayerPacked& lp = Lw.layer[l];
-    memset(&g, 0, sizeof(g));
-    g.num = 2;
-    g.fmt = fmt;
-    rc |= setup_linear(g.p[0], T.xpos16[l], M, d, d, W16(lp.w_in), 2 * d, d, P->bn_qkv);
-    rc |= setup_linear(g.p[1], T.xin16[l], M, d, d, W16(lp.w_in) + (size_t)2 * d * d, d, d, P->bn_qkv);
-    if (rc) return rc;
-    g.p[0].bias = F32(lp.b_in);
-    g.p[0].out16 = T.qkv16[l];
-    g.p[0].ld16 = 3 * d;
-    g.p[1].bias = F32(lp.b_in) + 2 * d;
-    g.p[1].out16 = T.qkv16[l] + 2 * d;
-    g.p[1].ld16 = 3 * d;
-    rc = gemm_launch(P, g, P->bn_qkv, sms, st);
-    if (rc) return rc;
-    {
-      AttnArgs a;
-      memset(&a, 0, sizeof(a));
-      a.key_mask = T.key_mask;
-      a.out = T.attn16[l];
-      a.lse = T.lse[l];
-      a.scale = 1.0f / sqrtf((float)P->dh);
-      a.B = P->B;
-      a.L = L;
-      a.H = P->H;
-      a.dh = P->dh;
-      a.d = d;
-      a.fmt = fmt;
-      if (P->dh == 64 || P->dh == 128) {
-        if (make_tmap_2d(&a.tm_qkv, T.qkv16[l], (uint64_t)M, (uint64_t)3 * d, (uint64_t)3 * d, 128, 64)) return 1;
-        prof_mark(P, st, 3);
-        rc = launch_attention(a, st);
-        prof_mark(P, st, 2);
-      } else {
-        rc = launch_attention_simt(a, T.qkv16[l], st);
-      }
-      if (rc) return rc;
-    }
-    memset(&g, 0, sizeof(g));
-    g.num = 1;
-    g.fmt = fmt;
-    rc = setup_linear(g.p[0], T.attn16[l], M, d, d, W16(lp.w_out), d, d, P->bn_out);
-    if (rc) return rc;
-    g.p[0].bias = F32(lp.b_out);
-    g.p[0].rps_in = L;
-    g.p[0].rps_out = L;
-    g.p[0].row_scale = droppath_scale ? droppath_scale + (size_t)(2 * l) * P->B : nullptr;
-    g.p[0].out16 = T.br16;
-    g.p[0].ld16 = d;
-    rc = gemm_launch(P, g, P->bn_out, sms, st);
-    if (rc) return rc;
-    {
-      LnArgs a;
-      memset(&a, 0, sizeof(a));
-      a.in = T.x32;
-      a.ld_in = d;
-      a.add16 = T.br16;
-      a.ld_add16 = d;
-      a.sum_out = T.y1[l];
-      a.rows = M;
-      a.d = d;
-      a.gamma = F32(lp.n1w);
-      a.beta = F32(lp.n1b);
-      a.eps = 1e-5f;
-      a.fmt = fmt;
-      a.out32 = T.x1_32;
-      a.out16 = T.x1_16[l];
-      a.ld16 = d;
-      a.mean_out = T.mean1[l];
-      a.rstd_out = T.rstd1[l];
-      rc = launch_layernorm(a, st);
-      if (rc) return rc;
-    }
-    memset(&g, 0, sizeof(g));
-    g.num = 1;
-    g.fmt = fmt;
-    rc = setup_linear(g.p[0], T.x1_16[l], M, d, d, W16(lp.w1), ff, d, P->bn_ffn1);
-    if (rc) return rc;
-    g.p[0].bias = F32(lp.b1);
-    g.p[0].act = ACT_GELU;
-    g.p[0].out16 = T.h16[l];
-    g.p[0].ld16 = ff;
-    g.p[0].dact16 = T.dgelu16[l];
-    g.p[0].ld_dact = ff;
-    rc = gemm_launch(P, g, P->bn_ffn1, sms, st);
-    if (rc) return rc;
-    memset(&g, 0, sizeof(g));
-    g.num = 1;
-    g.fmt = fmt;
-    rc = setup_linear(g.p[0], T.h16[l], M, ff, ff, W16(lp.w2), d, ff, P->bn_ffn2);
-    if (rc) return rc;
-    g.p[0].bias = F32(lp.b2);
-    g.p[0].rps_in = L;
-    g.p[0].rps_out = L;
-    g.p[0].row_scale = droppath_scale ? droppath_scale + (size_t)(2 * l + 1) * P->B : nullptr;
-    g.p[0].out16 = T.br16;
-    g.p[0].ld16 = d;
-    rc = gemm_launch(P, g, P->bn_ffn2, sms, st);
-    if (rc) return rc;
-    {
-      LnArgs a;
-      memset(&a, 0, sizeof(a));
-      a.in = T.x1_32;
-      a.ld_in = d;
-      a.add16 = T.br16;
-      a.ld_add16 = d;
-      a.sum_out = T.y2[l];
-      a.rows = M;
-      a.d = d;
-      a.gamma = F32(lp.n2w);
-      a.beta = F32(lp.n2b);
-      a.eps = 1e-5f;
-      a.fmt = fmt;
-      a.L = L;
-      a.Lv = Lv;
-      a.out32 = T.x32;
-      a.out16 = T.xin16[l + 1];
-      a.out16p = T.xpos16[l + 1];
-      a.ld16 = d;
-      a.pos = T.pos;
-      a.mean_out = T.mean2[l];
-      a.rstd_out = T.rstd2[l];
-      if (l == c.enc_layers - 1) a.outc = T.hA;
-      rc = launch_layernorm(a, st);
-      if (rc) return rc;
-    }
-  }
-
-  // ---- heads ----
-  auto conv_problem = [&](GemmProblem& p, const uint16_t* A, int lda, const uint16_t* W, int N, const float* bias, uint16_t* out,
-                          int ldo, int bn) -> int {
-    init_problem(p);
-    p.M = Mh;
-    p.N = N;
-    p.taps = 3;
-    p.kblk_per_tap = d / 64;
-    p.ca = OperandCoord{0, 0, 0, 1, 0, 1, 1, 0};
-    p.cb = OperandCoord{0, 0, d, 1, 0, 1, 0, 0};
-    int r = make_tmap_2d(&p.tm_a, A, (uint64_t)Mh + 2, (uint64_t)d, (uint64_t)lda, GEMM_BM, 64);
-    r |= make_tmap_2d(&p.tm_b, W, (uint64_t)N, (uint64_t)3 * d, (uint64_t)3 * d, (uint32_t)bn, 64);
-    p.b_box_rows = bn;
-    p.bias = bias;
-    p.act = ACT_RELU;
-    p.rps_in = Lv + 1;
-    p.rps_out = Lv + 1;
-    p.row_off = 1;
-    p.zero_sep = 1;
-    p.out16 = out;
-    p.ld16 = ldo;
-    return r;
-  };
-  memset(&g, 0, sizeof(g));
-  g.num = 1;
-  g.fmt = fmt;
-  rc = conv_problem(g.p[0], T.hA, d, W16(Lw.conv1_w), 2 * d, F32(Lw.conv1_b), T.h1, 2 * d, P->bn_conv1);
-  if (rc) return rc;
-  rc = gemm_launch(P, g, P->bn_conv1, sms, st);
-  if (rc) return rc;
-  memset(&g, 0, sizeof(g));
-  g.num = 2;
-  g.fmt = fmt;
-  rc |= conv_problem(g.p[0], T.h1, 2 * d, W16(Lw.conv2c_w), d, F32(Lw.conv2c_b), T.hc2, d, P->bn_conv2);
-  rc |= conv_problem(g.p[1], T.h1 + d, 2 * d, W16(Lw.conv2s_w), d, F32(Lw.conv2s_b), T.hs2, d, P->bn_conv2);
-  if (rc) return rc;
-  rc = gemm_launch(P, g, P->bn_conv2, sms, st);
-  if (rc) return rc;
-  {
-    HeadFinalArgs a;
-    a.h_cls = T.hc2;
-    a.h_span = T.hs2;
-    a.w_cls = F32(Lw.conv3c_w);
-    a.w_span = F32(Lw.conv3s_w);
-    a.b_cls = F32(Lw.conv3c_b);
-    a.b_span = F32(Lw.conv3s_b);
-    a.pred_logits = pred_logits;
-    a.pred_spans = pred_spans;
-    a.B = P->B;
-    a.Lv = Lv;
-    a.d = d;
-    a.fmt = fmt;
-    rc = launch_conv_head_final(a, st);
-    if (rc) return rc;
-  }
-  {
-    PoolSalArgs a;
-    a.x_txt = T.txtproj32;
-    a.x_vid = vid_mem_proj;
-    a.txt_mask = src_txt_mask;
-    a.vid_mask = src_vid_mask;
-    a.w = F32(Lw.pool_w);
-    a.pooled = txt_mem_proj;
-    a.saliency = saliency_scores;
-    a.alpha_out = T.pool_alpha;
-    a.logits_ws = T.pool_logits;
-    a.B = P->B;
-    a.Lt = P->Lt;
-    a.Lv = Lv;
-    a.d = d;
-    rc = launch_pool_saliency(a, st);
-    if (rc) return rc;
-  }
-  // keep the small outputs the backward needs (the caller owns the returned tensors and may free them)
-  cudaMemcpyAsync(T.pred_logits, pred_logits, (size_t)Mv * 4, cudaMemcpyDeviceToDevice, st);
-  cudaMemcpyAsync(T.pred_spans, pred_spans, (size_t)Mv * 8, cudaMemcpyDeviceToDevice, st);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) {
     set_error("univtg_forward_train: %s", cudaGetErrorString(e));
@@ -638,7 +296,8 @@ int univtg_backward(univtg_plan* P, void* ws, const float* src_txt, const float*
       p.ksplit = t_cw.ksplit;
       return r;
     };
-    const int bn_c2d = bn_for(sms, 64, MNK{Mh, d, 3 * d}, MNK{Mh, d, 3 * d}), bn_c1d = bn_for(sms, 64, MNK{Mh, d, 6 * d});
+    const int bn_c2d = tile_for(sms, 64, 1, MNK{Mh, d, 3 * d}, MNK{Mh, d, 3 * d}).bn;
+    const int bn_c1d = tile_for(sms, 64, 1, MNK{Mh, d, 6 * d}).bn;
     // (splitting the k-blocks of the layer-1 dgrad - 76 tiles of 96 k-blocks - over idle SMs saves ~8 us but reduces into the stream
     // gradient with atomics, which makes every gradient upstream of the heads order-dependent in its last bits: not taken)
     const int bn_cw = t_cw.bn;
@@ -737,8 +396,8 @@ int univtg_backward(univtg_plan* P, void* ws, const float* src_txt, const float*
     const LayerPacked& lp = Lw.layer[l];
     const float* s1 = droppath_scale ? droppath_scale + (size_t)(2 * l) * B : nullptr;
     const float* s2 = droppath_scale ? droppath_scale + (size_t)(2 * l + 1) * B : nullptr;
-    const int bn_dff = bn_for(sms, 64, MNK{M, ff, d}), bn_dd1 = bn_for(sms, 64, MNK{M, d, ff}), bn_ddo = bn_for(sms, 64, MNK{M, d, d}),
-              bn_ddq = bn_for(sms, 64, MNK{M, d, 3 * d});
+    const int bn_dff = tile_for(sms, 64, 1, MNK{M, ff, d}).bn, bn_dd1 = tile_for(sms, 64, 1, MNK{M, d, ff}).bn,
+              bn_ddo = tile_for(sms, 64, 1, MNK{M, d, d}).bn, bn_ddq = tile_for(sms, 64, 1, MNK{M, d, 3 * d}).bn;
     const TileChoice t_wo = tile_for(sms, 64, 16, MNK{d, d, M}), t_wq = tile_for(sms, 64, 16, MNK{2 * d, d, M}, MNK{d, d, M}),
                      t_wf = tile_for(sms, 64, 16, MNK{d, ff, M}, MNK{ff, d, M});
     const int bn_wo = t_wo.bn, bn_wq = t_wq.bn;
@@ -1007,7 +666,7 @@ int univtg_backward(univtg_plan* P, void* ws, const float* src_txt, const float*
     const int nv = pad_v ? kpv : dinv;  // the operand a_vid[i] is zero beyond dinv
     const TileChoice t_pw = tile_for(sms, 64, 16, MNK{d, nv, Mv}, MNK{d, dint, Mt});
     const int bn = t_pw.bn;
-    const int bn_pd = bn_for(sms, 64, MNK{Mv, kpv, d}, MNK{Mt, kpt, d});
+    const int bn_pd = tile_for(sms, 64, 1, MNK{Mv, kpv, d}, MNK{Mt, kpt, d}).bn;
     rc |= setup_gemm(g.p[0], Mat16{T.dxv16, Mv, d, d}, 1, Mat16{T.a_vid[i], Mv, kpv, kpv}, 1, d, nv, Mv, bn);
     rc |= setup_gemm(g.p[1], Mat16{T.dxt16, Mt, d, d}, 1, Mat16{T.a_txt[i], Mt, kpt, kpt}, 1, d, dint, Mt, bn);
     if (rc) return rc;

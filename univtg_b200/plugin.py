@@ -88,7 +88,7 @@ def _uniform_(t, bound):
 
 
 class _PlanEntry:
-    """One (B, Lv, Lt, training) shape bucket: the C plan (tensor maps + launch descriptors over the shared workspace)."""
+    """One (B, Lv, Lt, training) shape bucket: the C plan (shape and tile widths, pointing into the shared workspace)."""
     __slots__ = ("handle", "shape", "key", "pins", "grad_events_owner")
 
     def __init__(self):
@@ -263,7 +263,7 @@ class Model(nn.Module):
         buf = self._packed.get(fmt)
         if buf is None or buf.device != dev or buf.numel() != nbytes:
             self._packed[fmt] = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-            self._drop_plans()  # plans hold tensor maps into the old buffer
+            self._drop_plans()  # plans point into the old buffer
         arr = (ctypes.c_void_p * len(params))(*[p.data_ptr() for p in params])
         _lib.check(lib.univtg_pack_weights(ctypes.byref(cfg), arr, len(params), _lib.ptr(self._packed[fmt]), _lib.stream_ptr()),
                    "univtg_pack_weights")
@@ -272,7 +272,7 @@ class Model(nn.Module):
     PLAN_CACHE = 32  # shape buckets kept (LRU); collate pads to the batch maximum, so a corpus produces many (B, Lv, Lt)
 
     def _drop_plans(self, keep_training=False):
-        """Destroy the cached plans (their tensor maps point into the packed-weight buffer and the shared workspace).
+        """Destroy the cached plans (they point into the packed-weight buffer and the shared workspace).
         keep_training: the shared workspace is being re-allocated - training plans never touch it (univtg_forward_train /
         univtg_backward work in a leased buffer) and may be held by live autograd contexts, so they stay."""
         lib = _lib.load_library()
@@ -295,7 +295,7 @@ class Model(nn.Module):
 
     def _shared_workspace(self, nbytes):
         """ONE inference workspace for all shape buckets, sized for the largest shape seen (grown geometrically; growing drops
-        the plans, whose tensor maps point into the old buffer)."""
+        the plans, which point into the old buffer)."""
         ws = self.__dict__.get("_ws_infer")
         if ws is None or ws.device != self._device() or ws.numel() < nbytes:
             self._drop_plans(keep_training=ws is not None and ws.device == self._device())
@@ -553,8 +553,8 @@ class Model(nn.Module):
 
     def profile_train_step(self, B, Lv, Lt, run):
         """CUDA-event timeline of ONE training step of shape (B, Lv, Lt): `run()` must execute forward + criterion + backward.
-        Returns [(kind, ms), ...]: kind 1 = one tensor-core GEMM launch, 2 = one attention launch (forward or backward), 3 = whatever
-        ran between two of those (row kernels, criterion, launch gaps)."""
+        Returns [(kind, ms), ...]: kind 0 = one row kernel of the forward, 1 = one tensor-core GEMM launch, 2 = one attention launch
+        (forward or backward), 3 = whatever else ran before a backward GEMM / attention launch (row kernels, criterion, launch gaps)."""
         lib = _lib.load_library()
         with torch.cuda.device(self._device()):
             self._ensure_packed(training=True)
