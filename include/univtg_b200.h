@@ -123,6 +123,14 @@ int univtg_forward_train(univtg_plan* plan, void* train_ws, const float* src_txt
  * scales [n_sites = 2*enc_layers, batch].  Parity tests hand them to the oracle. */
 int univtg_dropout_mask(const univtg_rng* rng, int32_t mask_index, size_t rows, size_t cols, float* out, void* stream);
 int univtg_droppath_scales(const univtg_rng* rng, int32_t n_sites, int32_t batch, float* out, void* stream);
+/* p of nn.MultiheadAttention's dropout (args.dropout) for the following univtg_forward_train / univtg_backward calls on this
+ * plan; 0 = off (default).  The masks come from rng->seed (Philox, csrc/philox.cuh); p > 0 with rng == NULL is an error.
+ * The value in effect at univtg_backward must be the one its forward ran with.  univtg_forward never applies it. */
+int univtg_plan_set_attention_dropout(univtg_plan* plan, float p);
+/* The multipliers (0 or 1/(1-p)) the kernels apply in encoder layer `layer`: out [B, H, L, L] f32, row = query, column = key
+ * (the reference's [B*H, L, L] layout).  Parity tests hand them to the oracle. */
+int univtg_attention_dropout_mask(const univtg_rng* rng, float p, int32_t layer, int32_t B, int32_t H, int32_t L,
+                                  float* out, void* stream);
 /* Backward of the last univtg_forward_train on (plan, train_ws).  g_*: upstream gradients of pred_logits [B,Lv,1],
  * pred_spans [B,Lv,2], vid_mem_proj [B,Lv,d], txt_mem_proj [B,1,d] (NULL = zero).  grads: HOST array of device pointers,
  * one ZERO-FILLED fp32 tensor per parameter in univtg_pack_weights order and in the parameter's own layout.

@@ -70,6 +70,8 @@ SIGNATURES = {
                                 c_void_p, c_void_p, c_void_p, c_void_p, c_float, ctypes.POINTER(c_void_p), c_int, c_void_p]),
     "univtg_dropout_mask": (c_int, [ctypes.POINTER(Rng), c_int, c_size_t, c_size_t, c_void_p, c_void_p]),
     "univtg_droppath_scales": (c_int, [ctypes.POINTER(Rng), c_int, c_int, c_void_p, c_void_p]),
+    "univtg_plan_set_attention_dropout": (c_int, [c_void_p, c_float]),
+    "univtg_attention_dropout_mask": (c_int, [ctypes.POINTER(Rng), c_float, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     "univtg_loss_scratch_bytes": (c_size_t, [c_int, c_int]),
     "univtg_loss_forward": (c_int, [c_void_p] * 10 + [c_int, c_int, c_int, c_float, c_float, c_void_p, c_void_p, c_void_p]),
     "univtg_loss_backward": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,

@@ -277,6 +277,15 @@ int univtg_plan_set_input_format(univtg_plan* plan, int32_t fmt) {
   return 0;
 }
 
+int univtg_plan_set_attention_dropout(univtg_plan* plan, float p) {
+  if (!plan || !(p >= 0.f && p < 1.f)) {
+    set_error("univtg_plan_set_attention_dropout: p must be in [0, 1), got %g", (double)p);
+    return 1;
+  }
+  plan->attn_dropout = p;
+  return 0;
+}
+
 int univtg_plan_set_profiling(univtg_plan* plan, int32_t enable) {
   if (!plan) return 1;
   plan->profiling = enable ? 1 : 0;
@@ -331,6 +340,7 @@ int run_forward(univtg_plan* P, const FwdBufs& W, const float* src_txt, const fl
   // train-mode randomness: explicit tensors (the caller drew them, e.g. with the reference's torch calls) win over `rng`
   const bool dp_rng = droppath_scale == nullptr && rng != nullptr && rng->droppath > 0.f;
   const bool drop_rng = drop_masks == nullptr && rng != nullptr && rng->input_dropout > 0.f;
+  const bool attn_rng = rng != nullptr && P->attn_dropout > 0.f;  // attention dropout: always in-kernel, training only
   prof_begin(P, st);
   rc = launch_sine_pos(src_vid_mask, src_txt_mask, P->dim_t, W.pos, W.key_mask, P->B, Lv, Lt, d, st, dp_rng ? W.dp_scale : nullptr,
                        W.dp_scale ? 2 * c.enc_layers : 0, rng ? rng->seed : 0ull, rng ? 1.0f - rng->droppath : 1.f);
@@ -431,6 +441,7 @@ int run_forward(univtg_plan* P, const FwdBufs& W, const float* src_txt, const fl
       a.dh = P->dh;
       a.d = d;
       a.fmt = fmt;
+      if (attn_rng) a.drop = make_drop_spec(rng->seed, (unsigned int)l, P->attn_dropout);
       if (P->dh == 64 || P->dh == 128) {
         if (make_tmap_2d(&a.tm_qkv, W.qkv16[l], (uint64_t)M, (uint64_t)3 * d, (uint64_t)3 * d, 128, 64)) return 1;
         rc = launch_attention(a, st);

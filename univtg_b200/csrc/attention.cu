@@ -35,7 +35,9 @@ __device__ __forceinline__ float quad_sum(float v) {
   return v + __shfl_xor_sync(0xffffffffu, v, 2);
 }
 
-template <int DH, int BF>
+// DROP = 1: attention dropout.  The multipliers of the tile are generated while the S product runs (one Philox call per 8
+// elements) and kept as keep-bits; P o M is what feeds P V, while the row sum, the running max and lse stay un-dropped.
+template <int DH, int BF, int DROP>
 __global__ void __launch_bounds__(256, 1) attention_wgmma_kernel(const __grid_constant__ AttnArgs a) {
   using Cfg = AttnCfg<DH>;
   extern __shared__ uint8_t smem_raw[];
@@ -115,6 +117,23 @@ __global__ void __launch_bounds__(256, 1) attention_wgmma_kernel(const __grid_co
                                      make_smem_desc_sw128(kbase + off, 16, 1024), ks > 0 ? 1u : 0u);
     }
     wgmma_commit();
+    // keep-bits of this thread's 64 probabilities of the tile: fragment (kc, q), element e -> bit 8 (kc & 3) + 2 q + e of
+    // mb[kc >> 2].  Query rows fr / fr + 8 and keys 16 kc + fc + {0, 1, 8, 9} are exactly one attn_drop_block call.
+    uint32_t mb[2] = {0u, 0u};
+    if constexpr (DROP != 0) {
+      const unsigned int bh = (unsigned int)(b * a.H + h), i0 = (unsigned int)(q0 + wg * 64 + fr);
+#pragma unroll
+      for (int kc = 0; kc < 8; ++kc) {
+        const uint4 rr = attn_drop_block(a.drop, bh, i0, (unsigned int)(j * 128 + 16 * kc + fc));
+        const uint32_t w[4] = {rr.x, rr.y, rr.z, rr.w};
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+          const uint32_t wq = w[2 * (q & 1) + (q >> 1)];  // row bit 3 = q & 1, key bit 3 = q >> 1
+          mb[kc >> 2] |= ((wq & 0xffffu) >= a.drop.thresh ? 1u : 0u) << (8 * (kc & 3) + 2 * q);
+          mb[kc >> 2] |= ((wq >> 16) >= a.drop.thresh ? 1u : 0u) << (8 * (kc & 3) + 2 * q + 1);
+        }
+      }
+    }
     wgmma_wait<0>();
 #pragma unroll
     for (int i = 0; i < 64; ++i) reg_fence(sacc[i]);
@@ -149,7 +168,12 @@ __global__ void __launch_bounds__(256, 1) attention_wgmma_kernel(const __grid_co
         const float p0 = exp2f(sacc[8 * kc + 2 * q] - m_use[r]);
         const float p1 = exp2f(sacc[8 * kc + 2 * q + 1] - m_use[r]);
         psum[r] += p0 + p1;
-        pf[kc][q] = cvt16x2(p0, p1, BF);
+        if constexpr (DROP != 0) {
+          const uint32_t bits = mb[kc >> 2] >> (8 * (kc & 3) + 2 * q);
+          pf[kc][q] = cvt16x2((bits & 1u) ? p0 * a.drop.scale : 0.f, (bits & 2u) ? p1 * a.drop.scale : 0.f, BF);
+        } else {
+          pf[kc][q] = cvt16x2(p0, p1, BF);
+        }
       }
     }
 #pragma unroll
@@ -200,8 +224,11 @@ struct AttnSimtArgs {
   float* lse;
   float scale;
   int B, L, H, dh, d, fmt;
+  DropSpec drop;
 };
 
+// DROP = 1: attention dropout, one Philox call per element (attn_drop_mul1); p o m is rounded to 16 bit where p is otherwise.
+template <int DROP>
 __global__ void __launch_bounds__(128) attention_simt_kernel(const AttnSimtArgs a) {
   pdl_prologue();
   extern __shared__ float s_sc[];  // [4 warps][L]
@@ -232,7 +259,9 @@ __global__ void __launch_bounds__(128) attention_simt_kernel(const AttnSimtArgs 
   for (int j = lane; j < a.L; j += 32) {
     const float p = expf(sc[j] - m_use);
     sum += p;
-    sc[j] = ld16(cvt16(p, a.fmt), a.fmt);  // same operand rounding as the tensor-core path
+    float pm = p;
+    if constexpr (DROP != 0) pm = p * attn_drop_mul1(a.drop, (unsigned int)(b * a.H + h), (unsigned int)i, (unsigned int)j);
+    sc[j] = ld16(cvt16(pm, a.fmt), a.fmt);  // same operand rounding as the tensor-core path
   }
   sum = warp_sum(sum);
   __syncwarp();
@@ -245,13 +274,13 @@ __global__ void __launch_bounds__(128) attention_simt_kernel(const AttnSimtArgs 
   if (lane == 0 && a.lse) a.lse[((size_t)b * a.H + h) * a.L + i] = mx + logf(sum);
 }
 
-template <int DH, int BF>
+template <int DH, int BF, int DROP>
 static int launch_tc(const AttnArgs& a, cudaStream_t stream) {
   using Cfg = AttnCfg<DH>;
   static bool attr_set = false;
   if (!attr_set) {
     cudaError_t e =
-        cudaFuncSetAttribute(attention_wgmma_kernel<DH, BF>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes);
+        cudaFuncSetAttribute(attention_wgmma_kernel<DH, BF, DROP>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes);
     if (e != cudaSuccess) {
       set_error("cudaFuncSetAttribute(attention): %s", cudaGetErrorString(e));
       return (int)e;
@@ -259,34 +288,58 @@ static int launch_tc(const AttnArgs& a, cudaStream_t stream) {
     attr_set = true;
   }
   dim3 grid((a.L + 127) / 128, a.H, a.B);
-  launch_k(attention_wgmma_kernel<DH, BF>, dim3(grid), dim3(256), Cfg::kSmemBytes, stream, a);
+  launch_k(attention_wgmma_kernel<DH, BF, DROP>, dim3(grid), dim3(256), Cfg::kSmemBytes, stream, a);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) set_error("attention launch failed: %s", cudaGetErrorString(e));
   return (int)e;
 }
 
+template <int DH, int BF>
+static int launch_tc_drop(const AttnArgs& a, cudaStream_t stream) {
+  return a.drop.on ? launch_tc<DH, BF, 1>(a, stream) : launch_tc<DH, BF, 0>(a, stream);
+}
+
 int launch_attention_simt(const AttnArgs& a, const uint16_t* qkv, cudaStream_t stream) {
-  AttnSimtArgs s{qkv, a.key_mask, a.out, a.lse, a.scale, a.B, a.L, a.H, a.dh, a.d, a.fmt};
+  AttnSimtArgs s{qkv, a.key_mask, a.out, a.lse, a.scale, a.B, a.L, a.H, a.dh, a.d, a.fmt, a.drop};
   const int warps = a.B * a.H * a.L;
   const size_t smem = (size_t)4 * a.L * sizeof(float);
+  auto kern = a.drop.on ? attention_simt_kernel<1> : attention_simt_kernel<0>;
   if (smem > 48 * 1024) {
-    cudaError_t e = cudaFuncSetAttribute(attention_simt_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) {
       set_error("attention_simt smem %zu: %s", smem, cudaGetErrorString(e));
       return (int)e;
     }
   }
-  launch_k(attention_simt_kernel, dim3((warps + 3) / 4), dim3(128), smem, stream, s);
+  launch_k(kern, dim3((warps + 3) / 4), dim3(128), smem, stream, s);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) set_error("attention_simt launch failed: %s", cudaGetErrorString(e));
   return (int)e;
 }
 
 int launch_attention(const AttnArgs& a, cudaStream_t stream) {
-  if (a.dh == 128) return a.fmt ? launch_tc<128, 1>(a, stream) : launch_tc<128, 0>(a, stream);
-  if (a.dh == 64) return a.fmt ? launch_tc<64, 1>(a, stream) : launch_tc<64, 0>(a, stream);
+  if (a.dh == 128) return a.fmt ? launch_tc_drop<128, 1>(a, stream) : launch_tc_drop<128, 0>(a, stream);
+  if (a.dh == 64) return a.fmt ? launch_tc_drop<64, 1>(a, stream) : launch_tc_drop<64, 0>(a, stream);
   set_error("launch_attention: tensor-core path needs dh in {64,128}, got %d", a.dh);
   return (int)cudaErrorInvalidValue;
+}
+
+// The attention-dropout multipliers of `spec` as dense [B, H, L, L] (parity tests; the kernels above never store them).
+__global__ void __launch_bounds__(256) attention_dropout_mask_kernel(const DropSpec spec, int L, size_t n, float* __restrict__ out) {
+  pdl_prologue();
+  for (size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x; idx < n; idx += (size_t)gridDim.x * blockDim.x) {
+    const unsigned int j = (unsigned int)(idx % L), i = (unsigned int)((idx / L) % L), bh = (unsigned int)(idx / ((size_t)L * L));
+    out[idx] = attn_drop_mul1(spec, bh, i, j);
+  }
+}
+
+int launch_attention_dropout_mask(const DropSpec& spec, int B, int H, int L, float* out, cudaStream_t stream) {
+  const size_t n = (size_t)B * H * L * L;
+  const unsigned int blocks = (unsigned int)((n + 255) / 256 < 65536 ? (n + 255) / 256 : 65536);
+  launch_k(attention_dropout_mask_kernel, dim3(blocks), dim3(256), 0, stream, spec, L, n, out);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) set_error("attention_dropout_mask launch failed: %s", cudaGetErrorString(e));
+  return (int)e;
 }
 
 }  // namespace uv

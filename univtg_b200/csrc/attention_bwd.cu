@@ -24,7 +24,9 @@ struct AttnBwdCfg {
   static constexpr int kSmemBytes = 1024 + 4 * kTile + kDS + 3 * 128 * 4 + 64;
 };
 
-template <int DH, int BF>
+// DROP = 1: the forward's attention dropout M is regenerated (attn_drop_block) and applied as dV += (P o M)^T dO and
+// dS^T = P^T o (M o dP^T - delta).  delta = rowsum(dO o O) needs no change: O is the dropped output.
+template <int DH, int BF, int DROP>
 __global__ void __launch_bounds__(256, 1) attention_bwd_wgmma_kernel(const __grid_constant__ AttnBwdArgs a) {
   using Cfg = AttnBwdCfg<DH>;
   extern __shared__ uint8_t smem_raw[];
@@ -106,6 +108,29 @@ __global__ void __launch_bounds__(256, 1) attention_bwd_wgmma_kernel(const __gri
 
 #pragma unroll 1
     for (int hq = 0; hq < 2; ++hq) {
+      // keep-bits of this thread's 32 elements of the half, packed before the accumulators are live: element (block c, key row
+      // fr + 8 r, query column 8 c + fc + e) -> bit 4 c + 2 r + e.  Call (c >> 1, e) covers queries {i0, i0 + 8} x keys
+      // {j0, j0 + 1, j0 + 8, j0 + 9}; this thread's keys differ in bit 3 (r) and share bit 0, so it uses 4 of the 8 lanes.
+      uint32_t mb = 0u;
+      if constexpr (DROP != 0) {
+        const unsigned int bh = (unsigned int)(b * a.H + h), key0 = (unsigned int)(j * 128 + wg * 64 + fr);
+        const unsigned int half = key0 & 1u;
+#pragma unroll
+        for (int cp = 0; cp < 4; ++cp) {
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const uint4 rr = attn_drop_block(a.drop, bh, (unsigned int)(i * 128 + hq * 64 + 16 * cp + fc + e), key0 & ~9u);
+            const uint32_t w[4] = {rr.x, rr.y, rr.z, rr.w};
+#pragma unroll
+            for (int cq = 0; cq < 2; ++cq)
+#pragma unroll
+              for (int r = 0; r < 2; ++r) {  // word 2 (query bit 3 = cq) + (key bit 3 = r), lane half = key bit 0
+                const uint32_t v = half ? (w[2 * cq + r] >> 16) : (w[2 * cq + r] & 0xffffu);
+                mb |= (v >= a.drop.thresh ? 1u : 0u) << (4 * (2 * cp + cq) + 2 * r + e);
+              }
+          }
+        }
+      }
       float st[32], dpt[32];
       wgmma_fence();
 #pragma unroll
@@ -139,7 +164,13 @@ __global__ void __launch_bounds__(256, 1) attention_bwd_wgmma_kernel(const __gri
           for (int e = 0; e < 2; ++e) {
             const int col = hq * 64 + 8 * c + fc + e;
             p[e] = exp2f(st[4 * c + 2 * r + e] * sc2 + kb2[r] - s_lse2[col]);
-            d[e] = p[e] == 0.f ? 0.f : p[e] * (dpt[4 * c + 2 * r + e] - s_dlt[col]) * a.scale;
+            if constexpr (DROP != 0) {
+              const bool keep = (mb >> (4 * c + 2 * r + e)) & 1u;
+              d[e] = p[e] == 0.f ? 0.f : p[e] * ((keep ? dpt[4 * c + 2 * r + e] * a.drop.scale : 0.f) - s_dlt[col]) * a.scale;
+              p[e] = keep ? p[e] * a.drop.scale : 0.f;  // P o M feeds the dV product
+            } else {
+              d[e] = p[e] == 0.f ? 0.f : p[e] * (dpt[4 * c + 2 * r + e] - s_dlt[col]) * a.scale;
+            }
           }
           // accumulator block c, row half r -> A-fragment k-chunk c / 2, register (c & 1) * 2 + r
           pf[c >> 1][(c & 1) * 2 + r] = cvt16x2(p[0], p[1], BF);
@@ -229,12 +260,12 @@ __global__ void __launch_bounds__(256, 1) attention_bwd_wgmma_kernel(const __gri
   }
 }
 
-template <int DH, int BF>
+template <int DH, int BF, int DROP>
 static int launch_bwd_tc(const AttnBwdArgs& a, cudaStream_t stream) {
   using Cfg = AttnBwdCfg<DH>;
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(attention_bwd_wgmma_kernel<DH, BF>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    cudaError_t e = cudaFuncSetAttribute(attention_bwd_wgmma_kernel<DH, BF, DROP>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                          Cfg::kSmemBytes);
     if (e != cudaSuccess) {
       set_error("cudaFuncSetAttribute(attention_bwd): %s", cudaGetErrorString(e));
@@ -243,10 +274,15 @@ static int launch_bwd_tc(const AttnBwdArgs& a, cudaStream_t stream) {
     attr_set = true;
   }
   dim3 grid((a.L + 127) / 128, a.H, a.B);
-  launch_k(attention_bwd_wgmma_kernel<DH, BF>, dim3(grid), dim3(256), Cfg::kSmemBytes, stream, a);
+  launch_k(attention_bwd_wgmma_kernel<DH, BF, DROP>, dim3(grid), dim3(256), Cfg::kSmemBytes, stream, a);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) set_error("attention_bwd launch failed: %s", cudaGetErrorString(e));
   return (int)e;
+}
+
+template <int DH, int BF>
+static int launch_bwd_tc_drop(const AttnBwdArgs& a, cudaStream_t stream) {
+  return a.drop.on ? launch_bwd_tc<DH, BF, 1>(a, stream) : launch_bwd_tc<DH, BF, 0>(a, stream);
 }
 
 int launch_attention_bwd(const AttnBwdArgs& a, cudaStream_t stream) {
@@ -255,8 +291,8 @@ int launch_attention_bwd(const AttnBwdArgs& a, cudaStream_t stream) {
     return (int)cudaErrorInvalidValue;
   }
   const bool bf = a.fmt_act != 0;
-  if (a.dh == 128) return bf ? launch_bwd_tc<128, 1>(a, stream) : launch_bwd_tc<128, 0>(a, stream);
-  if (a.dh == 64) return bf ? launch_bwd_tc<64, 1>(a, stream) : launch_bwd_tc<64, 0>(a, stream);
+  if (a.dh == 128) return bf ? launch_bwd_tc_drop<128, 1>(a, stream) : launch_bwd_tc_drop<128, 0>(a, stream);
+  if (a.dh == 64) return bf ? launch_bwd_tc_drop<64, 1>(a, stream) : launch_bwd_tc_drop<64, 0>(a, stream);
   set_error("launch_attention_bwd: tensor-core path needs dh in {64,128}, got %d", a.dh);
   return (int)cudaErrorInvalidValue;
 }

@@ -535,6 +535,8 @@ int launch_attn_delta(const uint16_t* dO, int fmt_do, const uint16_t* O, int fmt
 // ------------------------------------------------------------------------------------------------
 // SIMT attention backward (any head size).  One warp per (b, h, query i); dK / dV / dQ accumulate atomically in fp32.
 // ------------------------------------------------------------------------------------------------
+// DROP = 1: the forward's attention dropout m (attn_drop_mul1, one Philox call per element): dV takes p m, dS = p (m dp - delta).
+template <int DROP>
 __global__ void __launch_bounds__(128) attention_bwd_simt_kernel(const AttnBwdArgs a) {
   pdl_prologue();
   extern __shared__ float s_buf[];  // [4 warps][2][L]: p and ds
@@ -562,7 +564,13 @@ __global__ void __launch_bounds__(128) attention_bwd_simt_kernel(const AttnBwdAr
         dp += ld16(dorow[c], a.fmt_grad) * ld16(vrow[c], a.fmt_act);
       }
       p = expf(s * a.scale - lse);
-      ds = p * (dp - dlt) * a.scale;
+      if constexpr (DROP != 0) {
+        const float m = attn_drop_mul1(a.drop, (unsigned int)(b * a.H + h), (unsigned int)i, (unsigned int)j);
+        ds = p * (m * dp - dlt) * a.scale;
+        p *= m;
+      } else {
+        ds = p * (dp - dlt) * a.scale;
+      }
     }
     p_s[j] = p;
     ds_s[j] = ds;
@@ -587,14 +595,15 @@ __global__ void __launch_bounds__(128) attention_bwd_simt_kernel(const AttnBwdAr
 int launch_attention_bwd_simt(const AttnBwdArgs& a, cudaStream_t stream) {
   const int warps = a.B * a.H * a.L;
   const size_t smem = (size_t)4 * 2 * a.L * sizeof(float);
+  auto kern = a.drop.on ? attention_bwd_simt_kernel<1> : attention_bwd_simt_kernel<0>;
   if (smem > 48 * 1024) {
-    cudaError_t e = cudaFuncSetAttribute(attention_bwd_simt_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) {
       set_error("attention_bwd_simt smem %zu: %s", smem, cudaGetErrorString(e));
       return (int)e;
     }
   }
-  launch_k(attention_bwd_simt_kernel, dim3((warps + 3) / 4), dim3(128), smem, stream, a);
+  launch_k(kern, dim3((warps + 3) / 4), dim3(128), smem, stream, a);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) set_error("attention_bwd_simt launch failed: %s", cudaGetErrorString(e));
   return (int)e;

@@ -67,6 +67,7 @@ struct AttnBwdArgs {
   // Single-key-tile fast path (L <= 128, tensor-core kernel): write dQ | dK | dV directly as 16-bit operands of the in-projection
   // dgrad / wgrad GEMMs; dqkv32 is then not written (the in_proj_bias gradient comes from launch_colsum16 over this buffer).
   uint16_t* dqkv16;       // [B*L, 3d] or null
+  DropSpec drop;          // the forward's attention dropout (drop.on): dV += (P o M)^T dO, dS = P o (M o dP - delta)
 };
 int launch_attention_bwd(const AttnBwdArgs& a, cudaStream_t stream);       // wgmma, dh in {64, 128}
 int launch_attention_bwd_simt(const AttnBwdArgs& a, cudaStream_t stream);  // any dh; needs dqkv32 pre-zeroed

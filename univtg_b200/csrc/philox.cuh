@@ -2,6 +2,8 @@
 // (no mask tensors in HBM, regenerated bit-identically by the backward):
 //   * input dropout   nn.Dropout(p) of every LinearLayer (reference model/univtg.py:394,401): multiplier 0 or 1/(1-p) per element
 //   * DropPath        floor(keep + U[0,1)) / keep per sample and residual branch (model/transformer_encoder_droppath.py:154-167)
+//   * attention dropout  F.dropout of the softmax probabilities in every encoder layer's nn.MultiheadAttention (args.dropout):
+//                     multiplier 0 or 1/(1-p) per (layer, b, h, query, key), applied inside the attention kernels
 // Philox4x32-10 (Salmon et al., SC'11; the generator family torch's CUDA RNG uses), keyed by (seed, stream), counter = (row,
 // column / 8); one call yields eight 16-bit lanes = the dropout decisions of eight consecutive columns of a row.  The draws are NOT torch's draws for the same seed
 // (torch's element-to-counter mapping depends on its launch geometry); parity tests read the multipliers back through
@@ -75,6 +77,25 @@ __device__ __forceinline__ float droppath_scale(unsigned long long seed, unsigne
   const uint4 r = philox4x32_10(make_uint4(index, 0u, 0x64726f70u, 0x70617468u), make_uint2((unsigned int)seed, (unsigned int)(seed >> 32)));
   const float u = (float)(r.x >> 8) * (1.0f / 16777216.0f);
   return floorf(keep + u) / keep;
+}
+
+// ---- attention-probability dropout (F.dropout(attn, p) inside nn.MultiheadAttention, transformer_encoder_droppath.py:93) ----
+// One multiplier per (layer = s.stream, bh = b * H + h, query i, key j), same thresh / scale as input dropout.  One Philox call
+// covers query rows {i0, i0 + 8} x keys {j0, j0 + 1, j0 + 8, j0 + 9}, i0 = i with bit 3 cleared, j0 = j with bits 0 and 3
+// cleared; its word 2 * (bit 3 of i) + (bit 3 of j) holds key bit 0 = 0 in the low and = 1 in the high 16-bit lane.  That block
+// is exactly what one thread of the forward wgmma kernel holds for two adjacent 8-key accumulator blocks (one call per 8
+// elements); the key-major backward uses 4 of the 8 lanes of each call; the SIMT kernels and the materialiser make one call per
+// element.  The constant counter word 0x61740000 + layer keeps these streams apart from input dropout (0x756e6976) and DropPath.
+__device__ __forceinline__ uint4 attn_drop_block(const DropSpec& s, unsigned int bh, unsigned int i0, unsigned int j0) {
+  return philox4x32_10(make_uint4(j0, i0, bh, 0x61740000u + s.stream), make_uint2((unsigned int)s.seed, (unsigned int)(s.seed >> 32)));
+}
+// 16-bit lane of (i, j) in the call attn_drop_block(s, bh, i & ~8, j & ~9)
+__device__ __forceinline__ unsigned int attn_drop_lane(const uint4& r, unsigned int i, unsigned int j) {
+  return drop_lane(r, 4u * ((i >> 3) & 1u) + 2u * ((j >> 3) & 1u) + (j & 1u));
+}
+__device__ __forceinline__ float attn_drop_mul1(const DropSpec& s, unsigned int bh, unsigned int i, unsigned int j) {
+  const uint4 r = attn_drop_block(s, bh, i & ~8u, j & ~9u);
+  return attn_drop_lane(r, i, j) >= s.thresh ? s.scale : 0.f;
 }
 
 inline DropSpec make_drop_spec(unsigned long long seed, unsigned int stream, float p) {

@@ -296,6 +296,7 @@ struct univtg_plan {
   int num_sms;
   int in_fmt;       // src_vid / src_txt element type: 0 f32 (reference collate), 1 fp16, 2 bf16 (packed feature shards)
   int num_sms_bwd;  // SM budget of the backward's GEMM launches (0: num_sms); see univtg_plan_set_backward_sm_budget
+  float attn_dropout;  // p of the attention dropout of univtg_forward_train / univtg_backward (0: off); univtg_forward ignores it
   int B, Lv, Lt, L, d, ff, H, dh, M, Mv, Mt, Mh;
   int bn_proj[3];  // tile widths of the forward's GEMM launches (tile_for)
   int bn_qkv, bn_out, bn_ffn1, bn_ffn2, bn_conv1, bn_conv2;
@@ -458,8 +459,8 @@ bool check_shape(const univtg_shape* s) {
 }  // namespace
 
 // Reference Model.forward (model/univtg.py:105-155) over the buffers `W`, for univtg_forward and univtg_forward_train (api.cu).
-// drop_masks / rng: train-mode randomness as univtg_forward_train takes it (NULL at inference).  The training-only entries of `W`
-// that are non-null are written as well.
+// drop_masks / rng: train-mode randomness as univtg_forward_train takes it (NULL at inference; attention dropout applies only with
+// an rng, P->attn_dropout > 0).  The training-only entries of `W` that are non-null are written as well.
 int run_forward(univtg_plan* P, const FwdBufs& W, const float* src_txt, const float* src_txt_mask, const float* src_vid,
                 const float* src_vid_mask, const float* droppath_scale, const float* const* drop_masks, const univtg_rng* rng,
                 float* pred_logits, float* pred_spans, float* vid_mem_proj, float* txt_mem_proj, float* saliency_scores,

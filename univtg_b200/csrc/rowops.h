@@ -80,9 +80,12 @@ struct AttnArgs {
   uint16_t* out;          // [B*L, d] 16-bit attention output (heads concatenated)
   float* lse;             // [B, H, L] log-sum-exp per query row (training) or null
   int B, L, H, dh, d, fmt;
+  DropSpec drop;          // attention dropout (drop.on; stream = encoder layer): P o M feeds P V, the row sum and lse stay un-dropped
 };
 int launch_attention(const AttnArgs& a, cudaStream_t stream);
 // SIMT variant for head sizes outside {64,128}; reads qkv through a plain pointer.
 int launch_attention_simt(const AttnArgs& a, const uint16_t* qkv, cudaStream_t stream);
+// out [B, H, L, L] f32: the attention-dropout multipliers of `spec` (row = query, column = key), as the kernels apply them
+int launch_attention_dropout_mask(const DropSpec& spec, int B, int H, int L, float* out, cudaStream_t stream);
 
 }  // namespace uv

@@ -163,6 +163,10 @@ int univtg_forward_train(univtg_plan* P, void* ws, const float* src_txt, const f
     set_error("univtg_forward_train: null argument");
     return 1;
   }
+  if (P->attn_dropout > 0.f && !rng) {
+    set_error("univtg_forward_train: attention dropout p = %g needs an rng (its masks are drawn in-kernel)", (double)P->attn_dropout);
+    return 1;
+  }
   const TrainWs T = make_train_ws(P->cfg, P->shp, P->lay, reinterpret_cast<uint8_t*>(ws));
   const int rc = run_forward(P, T, src_txt, src_txt_mask, src_vid, src_vid_mask, droppath_scale, drop_masks, rng, pred_logits,
                              pred_spans, vid_mem_proj, txt_mem_proj, saliency_scores, (cudaStream_t)stream);
@@ -200,6 +204,10 @@ int univtg_backward(univtg_plan* P, void* ws, const float* src_txt, const float*
   const TrainWs T = make_train_ws(c, P->shp, Lw, reinterpret_cast<uint8_t*>(ws));
   if (droppath_scale == nullptr && rng != nullptr && rng->droppath > 0.f) droppath_scale = T.dp_scale;  // drawn by the forward
   const bool drop_rng = drop_masks == nullptr && rng != nullptr && rng->input_dropout > 0.f;
+  if (P->attn_dropout > 0.f && !rng) {
+    set_error("univtg_backward: attention dropout p = %g needs the forward's rng", (double)P->attn_dropout);
+    return 1;
+  }
   const int d = P->d, ff = P->ff, fmt = c.operand_format, M = P->M, Mv = P->Mv, Mt = P->Mt, Mh = P->Mh, L = P->L, Lv = P->Lv,
             Lt = P->Lt, B = P->B;
   // persistent GEMM grids assume every CTA is resident at once; when a gradient all-reduce runs beside the backward its CTAs
@@ -583,6 +591,7 @@ int univtg_backward(univtg_plan* P, void* ws, const float* src_txt, const float*
       a.d = d;
       a.fmt_act = fmt;
       a.fmt_grad = FMT_G;
+      if (P->attn_dropout > 0.f) a.drop = make_drop_spec(rng->seed, (unsigned int)l, P->attn_dropout);  // the forward's masks
       const bool tc = (P->dh == 64 || P->dh == 128);
       const int num_kv = (L + 127) / 128;
       a.dq_atomic = (!tc || num_kv > 1) ? 1 : 0;
@@ -870,6 +879,15 @@ int univtg_dropout_mask(const univtg_rng* rng, int32_t mask_index, size_t rows, 
   }
   return launch_dropout_mask(make_drop_spec(rng->seed, (unsigned int)mask_index, rng->input_dropout), rows * cols, cols, out,
                              (cudaStream_t)stream);
+}
+
+int univtg_attention_dropout_mask(const univtg_rng* rng, float p, int32_t layer, int32_t B, int32_t H, int32_t L, float* out,
+                                  void* stream) {
+  if (!rng || !out || layer < 0 || B < 1 || H < 1 || L < 1 || !(p >= 0.f && p < 1.f)) {
+    set_error("univtg_attention_dropout_mask: bad argument (p must be in [0, 1))");
+    return 1;
+  }
+  return launch_attention_dropout_mask(make_drop_spec(rng->seed, (unsigned int)layer, p), B, H, L, out, (cudaStream_t)stream);
 }
 
 int univtg_droppath_scales(const univtg_rng* rng, int32_t n_sites, int32_t batch, float* out, void* stream) {
