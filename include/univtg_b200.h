@@ -131,13 +131,33 @@ int univtg_plan_set_attention_dropout(univtg_plan* plan, float p);
  * (the reference's [B*H, L, L] layout).  Parity tests hand them to the oracle. */
 int univtg_attention_dropout_mask(const univtg_rng* rng, float p, int32_t layer, int32_t B, int32_t H, int32_t L,
                                   float* out, void* stream);
+/* Learned text positions (args.use_txt_pos; reference model/univtg.py:123, model/position_encoding.py:19-41): the text rows of
+ * q = k = x + pos in every encoder layer get pos_t = Dropout(LayerNorm(x_t + P[l])) instead of zeros, where x_t is the projected
+ * text token (token-type row included) and P the table.  The dropout is nn.Dropout(args.input_dropout) in training: in-kernel it
+ * is input-dropout mask index 2*n_input_proj of rng (univtg_dropout_mask(rng, 2*n_input_proj, B*Lt, d) reads it back); an explicit
+ * `drop_mul` takes precedence; univtg_forward never applies it.  univtg_plan_set_txt_pos(plan, NULL) switches the feature off
+ * (the default); the setting in effect at univtg_backward must be the one its forward ran with, including the same scratch. */
+typedef struct univtg_txt_pos {
+  const float* table;     /* txt_position_embed.position_embeddings.weight [max_q_l, d]; read at every forward (not packed) */
+  int32_t max_q_l;        /* rows of `table`: L_t > max_q_l is an error */
+  const float* ln_weight; /* txt_position_embed.LayerNorm.weight [d] */
+  const float* ln_bias;   /* txt_position_embed.LayerNorm.bias [d] */
+  const float* drop_mul;  /* NULL or [B*L_t, d] dropout multipliers (0 or 1/(1-p)) of a training forward */
+  void* scratch;          /* univtg_txt_pos_scratch_bytes(cfg, shape) bytes, owned by the caller; one per training forward
+                           * whose backward is pending (it carries pos_t's statistics from the forward to the backward) */
+} univtg_txt_pos;
+int univtg_plan_set_txt_pos(univtg_plan* plan, const univtg_txt_pos* txt_pos);
+/* Bytes of the scratch of univtg_txt_pos for (config, shape); shape->training selects the training layout. */
+size_t univtg_txt_pos_scratch_bytes(const univtg_config* cfg, const univtg_shape* shape);
+
 /* Backward of the last univtg_forward_train on (plan, train_ws).  g_*: upstream gradients of pred_logits [B,Lv,1],
  * pred_spans [B,Lv,2], vid_mem_proj [B,Lv,d], txt_mem_proj [B,1,d] (NULL = zero).  grads: HOST array of device pointers,
  * one ZERO-FILLED fp32 tensor per parameter in univtg_pack_weights order and in the parameter's own layout.
  * grad_scale: power-of-two loss scale S > 0.  Gradient GEMM operands share the plan's 16-bit format (one wgmma takes
  * A and B in one format); with fp16 operands the intermediate gradients are carried multiplied by S so they do not
  * underflow, and every parameter gradient is multiplied by 1/S where it is written (the results are unscaled).  Use 1 for
- * bf16 plans. */
+ * bf16 plans.  With text positions on (univtg_plan_set_txt_pos), n_grads is univtg_num_params + 3 and the last three tensors
+ * are txt_position_embed.{position_embeddings.weight, LayerNorm.weight, LayerNorm.bias}; any other count is an error. */
 int univtg_backward(univtg_plan* plan, void* train_ws, const float* src_txt, const float* src_vid, const float* droppath_scale,
                     const float* const* drop_masks, const univtg_rng* rng, const float* g_logits, const float* g_spans,
                     const float* g_vid_mem_proj, const float* g_txt_mem_proj, float grad_scale, float* const* grads,
@@ -152,7 +172,8 @@ int univtg_backward(univtg_plan* plan, void* train_ws, const float* src_txt, con
  * (univtg_pack_weights order; an empty second range is 0,0) and returns n (ranges == NULL: just returns n).
  * univtg_plan_set_grad_events installs n cudaEvent_t handles; univtg_backward records event k on its stream as soon as stage
  * k's gradients are final, so a communication stream can wait on it and reduce that slice while the backward continues.
- * n = 0 removes them.  (enc_layers <= 16, so n <= 19.) */
+ * n = 0 removes them.  (enc_layers <= 16, so n <= 19.)  With text positions on, the three appended gradients (indices
+ * univtg_num_params .. +3, not listed by univtg_backward_stages) are final at stage n-2. */
 int univtg_backward_stages(const univtg_config* cfg, int32_t* ranges, int32_t max_stages);
 /* The GEMM launches of univtg_backward are persistent grids of one CTA per SM.  When a collective (NCCL) runs beside the backward
  * its CTAs occupy some SMs; give the backward the number of SMs that are left (0 = all) so that its grids stay single-wave. */
@@ -217,8 +238,9 @@ int univtg_debug_choose_tile(const int32_t* Ms, const int32_t* Ns, const int32_t
  * finite - then NOTHING was updated (the skipped step of dynamic loss scaling; the fp16 gradient operands of univtg_backward can
  * overflow when grad_scale is too large), else 0.0.  write_clipped_grads != 0 also stores the clipped gradients back
  * (clip_grad_norm_ scales .grad in place).
- * cfg + packed (both non-NULL; the flat buffers must then hold exactly the config's parameters in univtg_pack_weights order, each
- * padded to a multiple of 4 floats): the kernel also refreshes the 16-bit copies of the GEMM weight matrices inside `packed` from the
+ * cfg + packed (both non-NULL; the flat buffers must then start with the config's parameters in univtg_pack_weights order, each
+ * padded to a multiple of 4 floats; floats beyond them - the text-position tensors of univtg_backward - are parameters without a
+ * 16-bit copy and are updated like the rest): the kernel also refreshes the 16-bit copies of the GEMM weight matrices inside `packed` from the
  * values it has just computed, so no separate re-packing pass re-reads the weights; call univtg_pack_vectors afterwards for the
  * fp32 vectors (LayerNorm terms, biases, token-type rows - a few hundred KB). */
 int univtg_adamw_step(float* params, float* grads, float* exp_avg, float* exp_avg_sq, size_t n, float lr, float beta1,

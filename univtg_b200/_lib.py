@@ -43,6 +43,13 @@ class Rng(ctypes.Structure):
     _fields_ = [("seed", ctypes.c_uint64), ("input_dropout", c_float), ("droppath", c_float)]
 
 
+class TxtPos(ctypes.Structure):
+    """univtg_txt_pos."""
+
+    _fields_ = [("table", c_void_p), ("max_q_l", c_int), ("ln_weight", c_void_p), ("ln_bias", c_void_p), ("drop_mul", c_void_p),
+                ("scratch", c_void_p)]
+
+
 # symbol -> (restype, argtypes); every symbol declared in include/univtg_b200.h must be listed here
 SIGNATURES = {
     "univtg_last_error": (ctypes.c_char_p, []),
@@ -71,6 +78,8 @@ SIGNATURES = {
     "univtg_dropout_mask": (c_int, [ctypes.POINTER(Rng), c_int, c_size_t, c_size_t, c_void_p, c_void_p]),
     "univtg_droppath_scales": (c_int, [ctypes.POINTER(Rng), c_int, c_int, c_void_p, c_void_p]),
     "univtg_plan_set_attention_dropout": (c_int, [c_void_p, c_float]),
+    "univtg_plan_set_txt_pos": (c_int, [c_void_p, ctypes.POINTER(TxtPos)]),
+    "univtg_txt_pos_scratch_bytes": (c_size_t, [ctypes.POINTER(Config), ctypes.POINTER(Shape)]),
     "univtg_attention_dropout_mask": (c_int, [ctypes.POINTER(Rng), c_float, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     "univtg_loss_scratch_bytes": (c_size_t, [c_int, c_int]),
     "univtg_loss_forward": (c_int, [c_void_p] * 10 + [c_int, c_int, c_int, c_float, c_float, c_void_p, c_void_p, c_void_p]),

@@ -189,7 +189,7 @@ int univtg_adamw_step(float* params, float* grads, float* exp_avg, float* exp_av
   PackSegTable t;
   const int total = make_pack_segments(*cfg, packed, t);
   if (total < 0) return 1;
-  if ((size_t)total != n) {
+  if ((size_t)total > n) {
     set_error("univtg_adamw_step: flat buffer has %zu floats, the config's parameters need %d", n, total);
     return 1;
   }
@@ -286,6 +286,38 @@ int univtg_plan_set_attention_dropout(univtg_plan* plan, float p) {
   return 0;
 }
 
+int univtg_plan_set_txt_pos(univtg_plan* plan, const univtg_txt_pos* tp) {
+  if (!plan) {
+    set_error("univtg_plan_set_txt_pos: null plan");
+    return 1;
+  }
+  if (tp == nullptr) {
+    plan->txt_pos_on = 0;
+    memset(&plan->txt_pos, 0, sizeof(plan->txt_pos));
+    return 0;
+  }
+  if (!tp->table || !tp->ln_weight || !tp->ln_bias || !tp->scratch) {
+    set_error("univtg_plan_set_txt_pos: null table, LayerNorm term or scratch");
+    return 1;
+  }
+  if (plan->Lt > tp->max_q_l) {
+    set_error("univtg_plan_set_txt_pos: %d text tokens but the position table has max_q_l = %d rows", plan->Lt, tp->max_q_l);
+    return 1;
+  }
+  if (plan->d % 64 != 0 || plan->d > 1024) {
+    set_error("univtg_plan_set_txt_pos: hidden_dim %d must be a multiple of 64 and <= 1024", plan->d);
+    return 1;
+  }
+  plan->txt_pos = *tp;
+  plan->txt_pos_on = 1;
+  return 0;
+}
+
+size_t univtg_txt_pos_scratch_bytes(const univtg_config* cfg, const univtg_shape* shape) {
+  if (!check_cfg(cfg) || !check_shape(shape)) return 0;
+  return make_txt_pos_ws(*cfg, *shape, nullptr).total;
+}
+
 int univtg_plan_set_profiling(univtg_plan* plan, int32_t enable) {
   if (!plan) return 1;
   plan->profiling = enable ? 1 : 0;
@@ -309,7 +341,7 @@ int univtg_plan_read_profile(univtg_plan* plan, float* ms, int32_t* kinds, int32
   return n;
 }
 
-int univtg_forward_num_launches(const univtg_plan* plan) { return plan ? plan->launches : -1; }
+int univtg_forward_num_launches(const univtg_plan* plan) { return plan ? plan->launches + (plan->txt_pos_on ? 1 : 0) : -1; }
 int64_t univtg_launch_count(void) { return (int64_t)*uv::launch_counter(); }
 
 }  // extern "C"
@@ -341,6 +373,9 @@ int run_forward(univtg_plan* P, const FwdBufs& W, const float* src_txt, const fl
   const bool dp_rng = droppath_scale == nullptr && rng != nullptr && rng->droppath > 0.f;
   const bool drop_rng = drop_masks == nullptr && rng != nullptr && rng->input_dropout > 0.f;
   const bool attn_rng = rng != nullptr && P->attn_dropout > 0.f;  // attention dropout: always in-kernel, training only
+  const bool training = W.mean1[0] != nullptr;
+  // learned text positions: pos_t of the text rows of q = k = x + pos (zeros when off)
+  const TxtPosWs TP = P->txt_pos_on ? make_txt_pos_ws(c, P->shp, P->txt_pos.scratch) : TxtPosWs{};
   prof_begin(P, st);
   rc = launch_sine_pos(src_vid_mask, src_txt_mask, P->dim_t, W.pos, W.key_mask, P->B, Lv, Lt, d, st, dp_rng ? W.dp_scale : nullptr,
                        W.dp_scale ? 2 * c.enc_layers : 0, rng ? rng->seed : 0ull, rng ? 1.0f - rng->droppath : 1.f);
@@ -409,6 +444,31 @@ int run_forward(univtg_plan* P, const FwdBufs& W, const float* src_txt, const fl
       pv.ld32_id = pt.ld32_id = d;
     }
     rc = marked(launch_gemm_group(g, bn, sms, st), 1);
+    if (rc) return rc;
+  }
+  if (P->txt_pos_on) {  // pos_t = Dropout(LayerNorm(x_t + P[l])); text rows of xpos16[0] := 16-bit(x_t + pos_t)
+    TxtPosArgs a;
+    memset(&a, 0, sizeof(a));
+    a.xt = W.txtproj32;
+    a.table = P->txt_pos.table;
+    a.gamma = P->txt_pos.ln_weight;
+    a.beta = P->txt_pos.ln_bias;
+    if (training) {
+      a.mul32 = P->txt_pos.drop_mul;
+      if (!a.mul32 && rng != nullptr && rng->input_dropout > 0.f)
+        a.drop = make_drop_spec(rng->seed, (unsigned int)(2 * c.n_input_proj), rng->input_dropout);
+      a.mean_out = TP.mean;
+      a.rstd_out = TP.rstd;
+    }
+    a.pos = TP.pos;
+    a.xpos16 = W.xpos16[0];
+    a.B = P->B;
+    a.Lt = Lt;
+    a.L = L;
+    a.Lv = Lv;
+    a.d = d;
+    a.fmt = fmt;
+    rc = marked(launch_txt_pos(a, st), 0);
     if (rc) return rc;
   }
 
@@ -529,6 +589,7 @@ int run_forward(univtg_plan* P, const FwdBufs& W, const float* src_txt, const fl
       a.out16p = W.xpos16[l + 1];
       a.ld16 = d;
       a.pos = W.pos;
+      a.pos_txt = TP.pos;
       a.mean_out = W.mean2[l];
       a.rstd_out = W.rstd2[l];
       if (l == c.enc_layers - 1) a.outc = W.hA;  // vid_mem = memory[:, :Lv] feeds the conv heads

@@ -379,8 +379,16 @@ int launch_layernorm_bwd(const LnBwdArgs& a, cudaStream_t stream) {
 // ------------------------------------------------------------------------------------------------
 // fp32 -> 16-bit conversion with optional column sums.  Block = 256 threads x 32 rows; thread = 4 columns.
 // ------------------------------------------------------------------------------------------------
+// text-row index of stream row r for the compact copy (TxtRows), or -1
+__device__ __forceinline__ long long txt_row(const TxtRows& t, int r) {
+  const int b = r / t.L, l = r - b * t.L;
+  return l >= t.Lv ? (long long)b * (t.L - t.Lv) + (l - t.Lv) : -1;
+}
+
+template <bool TXT>
 __global__ void __launch_bounds__(256) cvt16_colsum_kernel(const float* __restrict__ in32, int ld_in, uint16_t* __restrict__ out16,
-                                                          int ld_out, int rows, int cols, int fmt, float* __restrict__ colsum, float cscale) {
+                                                          int ld_out, int rows, int cols, int fmt, float* __restrict__ colsum, float cscale,
+                                                          const TxtRows txt) {
   pdl_prologue();
   const int c = (blockIdx.x * 256 + threadIdx.x) * 4;
   if (c >= cols) return;
@@ -388,7 +396,12 @@ __global__ void __launch_bounds__(256) cvt16_colsum_kernel(const float* __restri
   float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
   for (int r = r0; r < min(rows, r0 + 32); ++r) {
     const float4 v = *reinterpret_cast<const float4*>(in32 + (size_t)r * ld_in + c);
-    *reinterpret_cast<uint2*>(out16 + (size_t)r * ld_out + c) = make_uint2(cvt16x2(v.x, v.y, fmt), cvt16x2(v.z, v.w, fmt));
+    const uint2 h = make_uint2(cvt16x2(v.x, v.y, fmt), cvt16x2(v.z, v.w, fmt));
+    *reinterpret_cast<uint2*>(out16 + (size_t)r * ld_out + c) = h;
+    if constexpr (TXT) {
+      const long long tr = txt_row(txt, r);
+      if (tr >= 0 && c < txt.txt_cols) *reinterpret_cast<uint2*>(txt.txt16 + tr * txt.txt_cols + c) = h;
+    }
     s.x += v.x;
     s.y += v.y;
     s.z += v.z;
@@ -428,8 +441,9 @@ int launch_tap_interleave(const float* src, float* dst, int N, int C, cudaStream
 // written directly in 16-bit).  thread = 8 columns (128-bit loads), block = 1024 columns x 64 rows.
 constexpr int kColsumRows = 16;  // rows per block: all 16 loads of a thread are in flight at once (the first version walked 64
                                  // rows four loads at a time and sat at 13 us for 21 MB - latency, not bandwidth)
+template <bool TXT>
 __global__ void __launch_bounds__(128) colsum16_kernel(const uint16_t* __restrict__ in16, int ld, int rows, int cols, int fmt,
-                                                      float* __restrict__ colsum, float scale) {
+                                                      float* __restrict__ colsum, float scale, const TxtRows txt) {
   pdl_prologue();
   const int c = (blockIdx.x * 128 + threadIdx.x) * 8;
   if (c >= cols) return;
@@ -438,6 +452,15 @@ __global__ void __launch_bounds__(128) colsum16_kernel(const uint16_t* __restric
 #pragma unroll
   for (int k = 0; k < kColsumRows; ++k)
     q[k] = (r0 + k < rows) ? __ldg(reinterpret_cast<const uint4*>(in16 + (size_t)(r0 + k) * ld + c)) : make_uint4(0u, 0u, 0u, 0u);
+  if constexpr (TXT) {
+    if (c < txt.txt_cols) {
+#pragma unroll
+      for (int k = 0; k < kColsumRows; ++k) {
+        const long long tr = r0 + k < rows ? txt_row(txt, r0 + k) : -1;
+        if (tr >= 0) *reinterpret_cast<uint4*>(txt.txt16 + tr * txt.txt_cols + c) = q[k];
+      }
+    }
+  }
   float s[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
 #pragma unroll
   for (int k = 0; k < kColsumRows; ++k) {
@@ -452,26 +475,32 @@ __global__ void __launch_bounds__(128) colsum16_kernel(const uint16_t* __restric
   red_add_f32x4(colsum + c + 4, make_float4(s[4] * scale, s[5] * scale, s[6] * scale, s[7] * scale));
 }
 
-int launch_colsum16(const uint16_t* in16, int ld, int rows, int cols, int fmt, float* colsum, float scale, cudaStream_t stream) {
-  if (cols % 8 != 0 || ld % 8 != 0 || (reinterpret_cast<uintptr_t>(in16) & 15) != 0 || (reinterpret_cast<uintptr_t>(colsum) & 15) != 0) {
+int launch_colsum16(const uint16_t* in16, int ld, int rows, int cols, int fmt, float* colsum, float scale, cudaStream_t stream,
+                    TxtRows txt) {
+  if (cols % 8 != 0 || ld % 8 != 0 || (reinterpret_cast<uintptr_t>(in16) & 15) != 0 || (reinterpret_cast<uintptr_t>(colsum) & 15) != 0 ||
+      (txt.txt16 && (txt.txt_cols % 8 != 0 || (reinterpret_cast<uintptr_t>(txt.txt16) & 15) != 0))) {
     set_error("colsum16: columns / leading dimension must be multiples of 8 and the pointers 16-byte aligned");
     return (int)cudaErrorInvalidValue;
   }
-  launch_k(colsum16_kernel, dim3((cols / 8 + 127) / 128, (rows + kColsumRows - 1) / kColsumRows), dim3(128), 0, stream, in16, ld, rows, cols,
-           fmt, colsum, scale);
+  const dim3 grid((cols / 8 + 127) / 128, (rows + kColsumRows - 1) / kColsumRows);
+  if (txt.txt16) launch_k(colsum16_kernel<true>, grid, dim3(128), 0, stream, in16, ld, rows, cols, fmt, colsum, scale, txt);
+  else launch_k(colsum16_kernel<false>, grid, dim3(128), 0, stream, in16, ld, rows, cols, fmt, colsum, scale, txt);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) set_error("colsum16 launch failed: %s", cudaGetErrorString(e));
   return (int)e;
 }
 
 int launch_cvt16_colsum(const float* in32, int ld_in, uint16_t* out16, int ld_out, int rows, int cols, int fmt, float* colsum,
-                        float colsum_scale, cudaStream_t stream) {
-  if (cols % 4 != 0 || ld_in % 4 != 0 || ld_out % 4 != 0) {
+                        float colsum_scale, cudaStream_t stream, TxtRows txt) {
+  if (cols % 4 != 0 || ld_in % 4 != 0 || ld_out % 4 != 0 || (txt.txt16 && txt.txt_cols % 4 != 0)) {
     set_error("cvt16_colsum: dims must be multiples of 4");
     return (int)cudaErrorInvalidValue;
   }
   dim3 grid((cols / 4 + 255) / 256, (rows + 31) / 32);
-  launch_k(cvt16_colsum_kernel, dim3(grid), dim3(256), 0, stream, in32, ld_in, out16, ld_out, rows, cols, fmt, colsum, colsum_scale);
+  if (txt.txt16)
+    launch_k(cvt16_colsum_kernel<true>, dim3(grid), dim3(256), 0, stream, in32, ld_in, out16, ld_out, rows, cols, fmt, colsum, colsum_scale, txt);
+  else
+    launch_k(cvt16_colsum_kernel<false>, dim3(grid), dim3(256), 0, stream, in32, ld_in, out16, ld_out, rows, cols, fmt, colsum, colsum_scale, txt);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) set_error("cvt16_colsum launch failed: %s", cudaGetErrorString(e));
   return (int)e;
@@ -891,5 +920,87 @@ int launch_stream_gather(const float* dx_stream, int L, int off, const float* ex
   return (int)e;
 }
 
+
+// ------------------------------------------------------------------------------------------------
+// Learned text positions backward (TxtPosBwdArgs, backward.h).  One 128-thread CTA per position l; thread owns columns
+// tid + 128 i.  The position-table row l is this CTA's alone: no atomics for dtable.
+// ------------------------------------------------------------------------------------------------
+template <int EPT>
+__global__ void __launch_bounds__(128) txt_pos_bwd_kernel(const TxtPosBwdArgs a) {
+  pdl_prologue();
+  __shared__ float s_red[2][2][4];  // [parity of b][sum g, sum g * xhat][warp]
+  const int l = blockIdx.x;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const float* P = a.table + (size_t)l * a.d;
+  float acc_p[EPT], acc_g[EPT], acc_b[EPT], pv[EPT], gam[EPT];
+#pragma unroll
+  for (int i = 0; i < EPT; ++i) {
+    const int j = tid + 128 * i;
+    acc_p[i] = acc_g[i] = acc_b[i] = 0.f;
+    pv[i] = j < a.d ? P[j] : 0.f;
+    gam[i] = j < a.d ? a.gamma[j] : 0.f;
+  }
+  for (int b = 0; b < a.B; ++b) {
+    const size_t r = (size_t)b * a.Lt + l;
+    const float mean = a.mean[r], rstd = a.rstd[r];
+    float g[EPT], xh[EPT];
+    float s1 = 0.f, s2 = 0.f;
+#pragma unroll
+    for (int i = 0; i < EPT; ++i) {
+      const int j = tid + 128 * i;
+      g[i] = xh[i] = 0.f;
+      if (j < a.d) {
+        float go = a.dpos[r * a.d + j];
+        if (a.mul32) go *= a.mul32[r * a.d + j];
+        else if (a.drop.on) go *= drop_mul1(a.drop, (unsigned int)r, (unsigned int)j);
+        xh[i] = (a.xt[r * a.d + j] + pv[i] - mean) * rstd;
+        acc_g[i] += go * xh[i];
+        acc_b[i] += go;
+        g[i] = go * gam[i];
+        s1 += g[i];
+        s2 += g[i] * xh[i];
+      }
+    }
+    s1 = warp_sum(s1);
+    s2 = warp_sum(s2);
+    if (lane == 0) {
+      s_red[b & 1][0][warp] = s1;
+      s_red[b & 1][1][warp] = s2;
+    }
+    __syncthreads();  // (double-buffered by the parity of b: one barrier per sample)
+    const float m1 = (s_red[b & 1][0][0] + s_red[b & 1][0][1] + s_red[b & 1][0][2] + s_red[b & 1][0][3]) / (float)a.d;
+    const float m2 = (s_red[b & 1][1][0] + s_red[b & 1][1][1] + s_red[b & 1][1][2] + s_red[b & 1][1][3]) / (float)a.d;
+    float* dxr = a.dx + ((size_t)b * a.L + a.Lv + l) * a.d;
+#pragma unroll
+    for (int i = 0; i < EPT; ++i) {
+      const int j = tid + 128 * i;
+      if (j < a.d) {
+        const float du = rstd * (g[i] - m1 - xh[i] * m2);
+        acc_p[i] += du;
+        dxr[j] += du;
+      }
+    }
+  }
+#pragma unroll
+  for (int i = 0; i < EPT; ++i) {
+    const int j = tid + 128 * i;
+    if (j < a.d) {
+      a.dtable[(size_t)l * a.d + j] = acc_p[i] * a.pgrad_scale;
+      atomicAdd(a.dgamma + j, acc_g[i] * a.pgrad_scale);
+      atomicAdd(a.dbeta + j, acc_b[i] * a.pgrad_scale);
+    }
+  }
+}
+
+int launch_txt_pos_bwd(const TxtPosBwdArgs& a, cudaStream_t stream) {
+  if (a.d > 128 * 8) {
+    set_error("txt_pos_bwd: hidden_dim %d > 1024 not supported", a.d);
+    return (int)cudaErrorInvalidValue;
+  }
+  launch_k(txt_pos_bwd_kernel<8>, dim3(a.Lt), dim3(128), 0, stream, a);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) set_error("txt_pos_bwd launch failed: %s", cudaGetErrorString(e));
+  return (int)e;
+}
 
 }  // namespace uv

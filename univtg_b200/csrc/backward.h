@@ -37,15 +37,23 @@ struct LnBwdArgs {
 };
 int launch_layernorm_bwd(const LnBwdArgs& a, cudaStream_t stream);
 
+// Optional compact copy of the text rows (row r = b*L + l, l >= Lv) of the first txt_cols columns of the 16-bit output, as
+// [B*(L-Lv), txt_cols] (the [dq | dk] rows the learned text positions' gradient needs); txt16 == NULL: no copy.
+struct TxtRows {
+  uint16_t* txt16;
+  int L, Lv, txt_cols;
+};
+
 // out16[r, c] = cvt(in32[r, c]) (+ column sums), rows x cols with leading dims
 int launch_cvt16_colsum(const float* in32, int ld_in, uint16_t* out16, int ld_out, int rows, int cols, int fmt, float* colsum,
-                        float colsum_scale, cudaStream_t stream);
+                        float colsum_scale, cudaStream_t stream, TxtRows txt = TxtRows{nullptr, 0, 0, 0});
 
 // dst[n][c][t] = src[t][n][c], t < 3 (conv weight gradient planes -> reference [out, in, 3] layout)
 int launch_tap_interleave(const float* src, float* dst, int N, int C, cudaStream_t stream);
 
 // colsum[c] += scale * sum_r in16[r, c]
-int launch_colsum16(const uint16_t* in16, int ld, int rows, int cols, int fmt, float* colsum, float scale, cudaStream_t stream);
+int launch_colsum16(const uint16_t* in16, int ld, int rows, int cols, int fmt, float* colsum, float scale, cudaStream_t stream,
+                    TxtRows txt = TxtRows{nullptr, 0, 0, 0});
 
 // delta[b, h, i] = sum_c dO[b, i, h, c] * O[b, i, h, c]
 int launch_attn_delta(const uint16_t* dO, int fmt_do, const uint16_t* O, int fmt_o, float* delta, int B, int L, int H, int dh,
@@ -114,5 +122,25 @@ int launch_pool_bwd(const PoolBwdArgs& a, cudaStream_t stream);
 int launch_stream_gather(const float* dx_stream, int L, int off, const float* extra, float extra_scale, uint16_t* out16,
                          float* colsum, float colsum_scale, int B, int Ls, int d, int fmt, cudaStream_t stream);
 
+// Backward of the learned text positions (rowops.h TxtPosArgs): one CTA per position l, looping over the samples.
+//   g = drop(dpos[r]);  xhat = (xt[r] + table[l] - mean[r]) * rstd[r];  du = LayerNorm backward of g
+//   dx[b*L + Lv + l] += du (stream gradient of x_t);  dtable[l] = pgrad_scale * sum_b du;  dgamma / dbeta += pgrad_scale * ...
+struct TxtPosBwdArgs {
+  const float* dpos;   // [B*Lt, d] gradient of pos_t (summed over the encoder layers; loss-scaled)
+  const float* xt;     // [B*Lt, d] projected text tokens saved by the forward
+  const float* table;  // [max_q_l, d]
+  const float* gamma;  // [d]
+  const float* mean;   // [B*Lt]
+  const float* rstd;
+  const float* mul32;  // [B*Lt, d] dropout multipliers of the forward, or null
+  DropSpec drop;       // in-kernel regeneration (drop.on; ignored with mul32)
+  float* dx;           // [B*L, d] stream gradient (text rows accumulated)
+  float* dtable;       // [max_q_l, d]: rows < Lt written
+  float* dgamma;       // [d] atomically accumulated
+  float* dbeta;
+  float pgrad_scale;
+  int B, Lt, L, Lv, d;
+};
+int launch_txt_pos_bwd(const TxtPosBwdArgs& a, cudaStream_t stream);
 
 }  // namespace uv

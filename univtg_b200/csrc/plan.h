@@ -297,6 +297,8 @@ struct univtg_plan {
   int in_fmt;       // src_vid / src_txt element type: 0 f32 (reference collate), 1 fp16, 2 bf16 (packed feature shards)
   int num_sms_bwd;  // SM budget of the backward's GEMM launches (0: num_sms); see univtg_plan_set_backward_sm_budget
   float attn_dropout;  // p of the attention dropout of univtg_forward_train / univtg_backward (0: off); univtg_forward ignores it
+  int txt_pos_on;           // learned text positions (univtg_plan_set_txt_pos); 0: off
+  univtg_txt_pos txt_pos;
   int B, Lv, Lt, L, d, ff, H, dh, M, Mv, Mt, Mh;
   int bn_proj[3];  // tile widths of the forward's GEMM launches (tile_for)
   int bn_qkv, bn_out, bn_ffn1, bn_ffn2, bn_conv1, bn_conv2;
@@ -445,6 +447,32 @@ FwdBufs make_infer_ws(const univtg_config& c, const univtg_shape& s, const Packe
     w.x1_16[l] = x16;
     w.h16[l] = h16;
   }
+  return w;
+}
+
+// Scratch of the learned text positions (univtg_txt_pos.scratch, univtg_txt_pos_scratch_bytes): pos_t for the encoder layers'
+// q/k operands; training adds its LayerNorm statistics and the backward's accumulators.
+struct TxtPosWs {
+  float* pos;       // [Mt, d] pos_t
+  float *mean, *rstd;  // [Mt] (training)
+  float* dpos;      // [Mt, d] gradient of pos_t summed over the encoder layers (training)
+  uint16_t* dqk16;  // [Mt, 2d] text rows of [dq | dk] of the layer being differentiated (training)
+  size_t total;
+};
+inline TxtPosWs make_txt_pos_ws(const univtg_config& c, const univtg_shape& s, void* base_) {
+  TxtPosWs w;
+  memset(&w, 0, sizeof(w));
+  uint8_t* base = reinterpret_cast<uint8_t*>(base_);
+  Cursor cur;
+  const size_t d = c.hidden_dim, Mt = (size_t)s.batch * s.l_txt;
+  w.pos = reinterpret_cast<float*>(base + cur.take(Mt * d * 4));
+  if (s.training) {
+    w.mean = reinterpret_cast<float*>(base + cur.take(Mt * 4));
+    w.rstd = reinterpret_cast<float*>(base + cur.take(Mt * 4));
+    w.dpos = reinterpret_cast<float*>(base + cur.take(Mt * d * 4));
+    w.dqk16 = reinterpret_cast<uint16_t*>(base + cur.take(Mt * 2 * d * 2));
+  }
+  w.total = cur.off;
   return w;
 }
 

@@ -15,12 +15,15 @@ namespace uv {
 
 // ------------------------------------------------------------------------------------------------
 // LayerNorm over rows.  One warp per row.
+// TXT: the text rows of out16p also get a.pos_txt (learned text positions); a separate instantiation, so the kernels without
+// text positions are compiled exactly as before.
 // ------------------------------------------------------------------------------------------------
+template <bool TXT = false>
 struct LnStore {
   const LnArgs& a;
   int row, b, l;
   bool has_pos;
-  size_t prow, crow;
+  size_t prow, crow, trow;
   __device__ LnStore(const LnArgs& a_, int row_) : a(a_), row(row_) {
     b = 0;
     l = row;
@@ -31,6 +34,7 @@ struct LnStore {
     has_pos = (a.pos != nullptr) && (a.L > 0) && (l < a.Lv);
     prow = (size_t)b * a.Lv + l;
     crow = (size_t)1 + (size_t)b * (a.Lv + 1) + l;
+    trow = (size_t)b * (a.L - a.Lv) + (l - a.Lv);
   }
   __device__ __forceinline__ void store4(int j, float4 v) const {
     if (a.out32) *reinterpret_cast<float4*>(a.out32 + (size_t)row * a.d + j) = v;
@@ -52,6 +56,13 @@ struct LnStore {
         pp.x = cvt16x2(v.x + p.x, v.y + p.y, a.fmt);
         pp.y = cvt16x2(v.z + p.z, v.w + p.w, a.fmt);
       }
+      if constexpr (TXT) {
+        if (a.L > 0 && l >= a.Lv) {
+          const float4 p = *reinterpret_cast<const float4*>(a.pos_txt + trow * a.d + j);
+          pp.x = cvt16x2(v.x + p.x, v.y + p.y, a.fmt);
+          pp.y = cvt16x2(v.z + p.z, v.w + p.w, a.fmt);
+        }
+      }
       *reinterpret_cast<uint2*>(a.out16p + (size_t)row * a.ld16 + j) = pp;
     }
     if (a.outc && a.L > 0 && l < a.Lv) *reinterpret_cast<uint2*>(a.outc + crow * a.d + j) = pk;
@@ -62,13 +73,19 @@ struct LnStore {
     else if (a.drop.on) v *= drop_mul1(a.drop, (unsigned int)row, (unsigned int)j);
     const uint16_t h = cvt16(v, a.fmt);
     if (a.out16) a.out16[(size_t)row * a.ld16 + j] = h;
-    if (a.out16p) a.out16p[(size_t)row * a.ld16 + j] = has_pos ? cvt16(v + a.pos[prow * a.d + j], a.fmt) : h;
+    if (a.out16p) {
+      uint16_t hp = has_pos ? cvt16(v + a.pos[prow * a.d + j], a.fmt) : h;
+      if constexpr (TXT) {
+        if (a.L > 0 && l >= a.Lv) hp = cvt16(v + a.pos_txt[trow * a.d + j], a.fmt);
+      }
+      a.out16p[(size_t)row * a.ld16 + j] = hp;
+    }
     if (a.outc && a.L > 0 && l < a.Lv) a.outc[crow * a.d + j] = h;
   }
 };
 
 // d == NV * 128: the row lives in registers (NV float4 per lane), one global read.
-template <int NV>
+template <int NV, bool TXT>
 __global__ void __launch_bounds__(256) layernorm_rows_vec_kernel(const LnArgs a) {
   pdl_prologue();
   const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
@@ -109,7 +126,7 @@ __global__ void __launch_bounds__(256) layernorm_rows_vec_kernel(const LnArgs a)
     if (a.mean_out) a.mean_out[warp] = mean;
     if (a.rstd_out) a.rstd_out[warp] = rstd;
   }
-  const LnStore st(a, warp);
+  const LnStore<TXT> st(a, warp);
 #pragma unroll
   for (int i = 0; i < NV; ++i) {
     const int j = (i * 32 + lane) * 4;
@@ -147,7 +164,7 @@ __global__ void __launch_bounds__(256) layernorm_rows_generic_kernel(const LnArg
     if (a.mean_out) a.mean_out[warp] = mean;
     if (a.rstd_out) a.rstd_out[warp] = rstd;
   }
-  const LnStore st(a, warp);
+  const LnStore<> st(a, warp);
   for (int j = lane; j < a.d; j += 32) st.store1(j, (X(j) - mean) * rstd * a.gamma[j] + a.beta[j]);
   // zero the K padding of the 16-bit operand row (columns d .. ld16)
   if (a.out16)
@@ -155,7 +172,7 @@ __global__ void __launch_bounds__(256) layernorm_rows_generic_kernel(const LnArg
 }
 
 // arbitrary d <= 128*EPT: one 128-thread block per row, the row lives in registers (single HBM read).
-template <int EPT>
+template <int EPT, bool TXT>
 __global__ void __launch_bounds__(128) layernorm_rows_block_kernel(const LnArgs a) {
   pdl_prologue();
   __shared__ float s_red[4];
@@ -201,7 +218,7 @@ __global__ void __launch_bounds__(128) layernorm_rows_block_kernel(const LnArgs 
   }
   __syncthreads();
   const float rstd = s_stat[1];
-  const LnStore st(a, row);
+  const LnStore<TXT> st(a, row);
 #pragma unroll
   for (int i = 0; i < EPT; ++i) {
     const int j = tid + 128 * i;
@@ -299,16 +316,26 @@ int launch_layernorm(const LnArgs& a, cudaStream_t stream) {
   const int blocks = (a.rows * 32 + threads - 1) / threads;
   const bool vec_ok = (a.ld_in % 4 == 0) && (a.ld16 == a.d) &&
                       (a.in16 ? (reinterpret_cast<uintptr_t>(a.in16) & 7) == 0 : (reinterpret_cast<uintptr_t>(a.in) & 15) == 0);
-  if (vec_ok && a.d == 1024) launch_k(layernorm_rows_vec_kernel<8>, dim3(blocks), dim3(threads), 0, stream, a);
-  else if (vec_ok && a.d == 512) launch_k(layernorm_rows_vec_kernel<4>, dim3(blocks), dim3(threads), 0, stream, a);
-  else if (vec_ok && a.d == 256) launch_k(layernorm_rows_vec_kernel<2>, dim3(blocks), dim3(threads), 0, stream, a);
+  if (a.pos_txt != nullptr) {  // LayerNorm 2 of an encoder layer with learned text positions (out16p of the next layer)
+    if (!a.out16p || a.L <= 0 || a.d > 128 * 24) {
+      set_error("layernorm: text positions need the structured q/k operand and d <= 3072");
+      return (int)cudaErrorInvalidValue;
+    }
+    if (vec_ok && a.d == 1024) launch_k(layernorm_rows_vec_kernel<8, true>, dim3(blocks), dim3(threads), 0, stream, a);
+    else if (vec_ok && a.d == 512) launch_k(layernorm_rows_vec_kernel<4, true>, dim3(blocks), dim3(threads), 0, stream, a);
+    else if (vec_ok && a.d == 256) launch_k(layernorm_rows_vec_kernel<2, true>, dim3(blocks), dim3(threads), 0, stream, a);
+    else if (a.d <= 128 * 8) launch_k(layernorm_rows_block_kernel<8, true>, dim3(a.rows), dim3(128), 0, stream, a);
+    else launch_k(layernorm_rows_block_kernel<24, true>, dim3(a.rows), dim3(128), 0, stream, a);
+  } else if (vec_ok && a.d == 1024) launch_k(layernorm_rows_vec_kernel<8, false>, dim3(blocks), dim3(threads), 0, stream, a);
+  else if (vec_ok && a.d == 512) launch_k(layernorm_rows_vec_kernel<4, false>, dim3(blocks), dim3(threads), 0, stream, a);
+  else if (vec_ok && a.d == 256) launch_k(layernorm_rows_vec_kernel<2, false>, dim3(blocks), dim3(threads), 0, stream, a);
   else if (a.d > 1024 && a.d <= 1024 * 3 && a.d % 2 == 0 && a.ld_in % 2 == 0 && a.ld16 % 2 == 0 && a.out16 && !a.out32 &&
            !a.out16p && !a.outc && !a.add16 && (a.in16 ? (reinterpret_cast<uintptr_t>(a.in16) & 3) == 0 : (reinterpret_cast<uintptr_t>(a.in) & 7) == 0) &&
            (reinterpret_cast<uintptr_t>(a.gamma) & 7) == 0 && (reinterpret_cast<uintptr_t>(a.beta) & 7) == 0 &&
            (!a.mul32 || (reinterpret_cast<uintptr_t>(a.mul32) & 7) == 0))
     launch_k(layernorm_rows_block2_kernel<12>, dim3(a.rows), dim3(128), 0, stream, a);
-  else if (a.d <= 128 * 8) launch_k(layernorm_rows_block_kernel<8>, dim3(a.rows), dim3(128), 0, stream, a);
-  else if (a.d <= 128 * 24) launch_k(layernorm_rows_block_kernel<24>, dim3(a.rows), dim3(128), 0, stream, a);
+  else if (a.d <= 128 * 8) launch_k(layernorm_rows_block_kernel<8, false>, dim3(a.rows), dim3(128), 0, stream, a);
+  else if (a.d <= 128 * 24) launch_k(layernorm_rows_block_kernel<24, false>, dim3(a.rows), dim3(128), 0, stream, a);
   else {
     if (a.add16) {
       set_error("layernorm: fused branch add needs d <= 3072");
@@ -318,6 +345,81 @@ int launch_layernorm(const LnArgs& a, cudaStream_t stream) {
   }
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) set_error("layernorm launch failed: %s", cudaGetErrorString(e));
+  return (int)e;
+}
+
+// ------------------------------------------------------------------------------------------------
+// Learned text positions (TxtPosArgs, rowops.h).  One warp per text row; lane owns columns 2 (lane + 32 i), i < d / 64.
+// ------------------------------------------------------------------------------------------------
+constexpr int kTxtPosMaxPairs = 16;  // d <= 64 * 16
+__global__ void __launch_bounds__(256) txt_pos_rows_kernel(const TxtPosArgs a) {
+  pdl_prologue();
+  const int row = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (row >= a.B * a.Lt) return;
+  const int b = row / a.Lt, l = row - b * a.Lt;
+  const int npairs = a.d >> 6;
+  const float* x = a.xt + (size_t)row * a.d;
+  const float* P = a.table + (size_t)l * a.d;
+  float2 u[kTxtPosMaxPairs];
+  float s = 0.f;
+#pragma unroll
+  for (int i = 0; i < kTxtPosMaxPairs; ++i) {
+    if (i < npairs) {
+      const int j = 2 * (lane + 32 * i);
+      const float2 xv = *reinterpret_cast<const float2*>(x + j);
+      const float2 pv = *reinterpret_cast<const float2*>(P + j);
+      u[i] = make_float2(xv.x + pv.x, xv.y + pv.y);
+      s += u[i].x + u[i].y;
+    }
+  }
+  const float mean = warp_sum(s) / (float)a.d;
+  float q = 0.f;
+#pragma unroll
+  for (int i = 0; i < kTxtPosMaxPairs; ++i) {
+    if (i < npairs) {
+      const float dx = u[i].x - mean, dy = u[i].y - mean;
+      q += dx * dx + dy * dy;
+    }
+  }
+  const float rstd = rsqrtf(warp_sum(q) / (float)a.d + 1e-5f);
+  if (lane == 0 && a.mean_out) {
+    a.mean_out[row] = mean;
+    a.rstd_out[row] = rstd;
+  }
+  uint16_t* xp = a.xpos16 + ((size_t)b * a.L + a.Lv + l) * a.d;
+#pragma unroll
+  for (int i = 0; i < kTxtPosMaxPairs; ++i) {
+    if (i < npairs) {
+      const int j = 2 * (lane + 32 * i);
+      const float2 g = *reinterpret_cast<const float2*>(a.gamma + j);
+      const float2 be = *reinterpret_cast<const float2*>(a.beta + j);
+      float ox = (u[i].x - mean) * rstd * g.x + be.x;
+      float oy = (u[i].y - mean) * rstd * g.y + be.y;
+      if (a.mul32) {
+        const float2 m = *reinterpret_cast<const float2*>(a.mul32 + (size_t)row * a.d + j);
+        ox *= m.x;
+        oy *= m.y;
+      } else if (a.drop.on) {
+        ox *= drop_mul1(a.drop, (unsigned int)row, (unsigned int)j);
+        oy *= drop_mul1(a.drop, (unsigned int)row, (unsigned int)(j + 1));
+      }
+      *reinterpret_cast<float2*>(a.pos + (size_t)row * a.d + j) = make_float2(ox, oy);
+      const float2 xv = *reinterpret_cast<const float2*>(x + j);
+      *reinterpret_cast<uint32_t*>(xp + j) = cvt16x2(xv.x + ox, xv.y + oy, a.fmt);
+    }
+  }
+}
+
+int launch_txt_pos(const TxtPosArgs& a, cudaStream_t stream) {
+  if (a.d % 64 != 0 || a.d > 64 * kTxtPosMaxPairs) {
+    set_error("text positions: hidden_dim %d must be a multiple of 64 and <= %d", a.d, 64 * kTxtPosMaxPairs);
+    return (int)cudaErrorInvalidValue;
+  }
+  const int rows = a.B * a.Lt;
+  launch_k(txt_pos_rows_kernel, dim3((rows * 32 + 255) / 256), dim3(256), 0, stream, a);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) set_error("txt_pos launch failed: %s", cudaGetErrorString(e));
   return (int)e;
 }
 

@@ -28,6 +28,7 @@ struct LnArgs {
   uint16_t* out16p;    // [rows, ld16] 16-bit(x + pos) for video rows, 16-bit(x) for text rows
   int ld16;
   const float* pos;    // [B*Lv, d] fp32 sine table (row b*Lv + l)
+  const float* pos_txt;  // [B*Lt, d] fp32 learned text positions (row b*Lt + l - Lv) added to out16p's text rows, or null
   uint16_t* outc;      // conv-head layout: row 1 + b*(Lv+1) + l of a [B*(Lv+1)+2, d] buffer (video rows only)
   const float* mul32;  // [rows, d] multiplier applied to the 16-bit outputs only (input-dropout mask incl. 1/(1-p)), or null
   DropSpec drop;       // in-kernel input dropout (drop.on; ignored when mul32 is given): same multiplier semantics
@@ -35,6 +36,23 @@ struct LnArgs {
   float* rstd_out;     // [rows]
 };
 int launch_layernorm(const LnArgs& a, cudaStream_t stream);
+
+// Learned text positions (txt_position_embed, reference model/position_encoding.py:19-41), one warp per text row r = b*Lt + l:
+//   pos[r] = drop(LayerNorm(xt[r] + table[l])) (eps 1e-5), and the text row b*L + Lv + l of xpos16 becomes 16-bit(xt[r] + pos[r])
+struct TxtPosArgs {
+  const float* xt;      // [B*Lt, d] projected text tokens incl. the token-type row (x_t: the text rows of the stream)
+  const float* table;   // [max_q_l, d] position_embeddings.weight
+  const float* gamma;   // [d]
+  const float* beta;    // [d]
+  const float* mul32;   // [B*Lt, d] dropout multipliers, or null
+  DropSpec drop;        // in-kernel dropout (drop.on; ignored when mul32 is given)
+  float* pos;           // [B*Lt, d] out
+  float* mean_out;      // [B*Lt] (training) or null
+  float* rstd_out;
+  uint16_t* xpos16;     // [B*L, d] q/k operand of encoder layer 0
+  int B, Lt, L, Lv, d, fmt;
+};
+int launch_txt_pos(const TxtPosArgs& a, cudaStream_t stream);
 
 // pos [B*Lv, d] sine table + key_mask [B, Lv+Lt] = cat(vid_mask, txt_mask)
 // dp_out (optional): [dp_sites, B] DropPath scales floor(keep + u) / keep drawn in-kernel from (dp_seed, site * B + b)

@@ -192,8 +192,10 @@ int univtg_backward(univtg_plan* P, void* ws, const float* src_txt, const float*
     return 1;
   }
   const univtg_config& c = P->cfg;
-  if (n_grads != univtg_num_params(&c)) {
-    set_error("univtg_backward: expected %d gradient tensors, got %d", univtg_num_params(&c), n_grads);
+  const int n_params = univtg_num_params(&c) + (P->txt_pos_on ? 3 : 0);  // + txt_position_embed.* with learned text positions
+  if (n_grads != n_params) {
+    set_error("univtg_backward: expected %d gradient tensors (text positions %s), got %d", n_params, P->txt_pos_on ? "on" : "off",
+              n_grads);
     return 1;
   }
   cudaStream_t st = (cudaStream_t)stream;
@@ -229,6 +231,9 @@ int univtg_backward(univtg_plan* P, void* ws, const float* src_txt, const float*
   auto G_span = [&](int k) { return grads[hb + k]; };
   auto G_cls = [&](int k) { return grads[hb + 6 + k]; };
   float* G_pool = grads[hb + 12];
+  const bool txt_pos = P->txt_pos_on != 0;
+  const TxtPosWs TP = txt_pos ? make_txt_pos_ws(c, P->shp, P->txt_pos.scratch) : TxtPosWs{};
+  const TxtRows txt_rows = txt_pos ? TxtRows{TP.dqk16, L, Lv, 2 * d} : TxtRows{nullptr, 0, 0, 0};
 
   cudaMemsetAsync(T.dx, 0, (size_t)M * d * 4, st);
 
@@ -609,8 +614,9 @@ int univtg_backward(univtg_plan* P, void* ws, const float* src_txt, const float*
       }
       if (rc) return rc;
     }
-    if (!fused16) rc = launch_cvt16_colsum(T.dqkv32, 3 * d, T.dqkv16, 3 * d, M, 3 * d, FMT_G, G_layer(l, 1), INV, st);
-    else rc = launch_colsum16(T.dqkv16, 3 * d, M, 3 * d, FMT_G, G_layer(l, 1), INV, st);  // in_proj_bias gradient
+    // (with text positions the same pass also copies the text rows of [dq | dk] into TP.dqk16)
+    if (!fused16) rc = launch_cvt16_colsum(T.dqkv32, 3 * d, T.dqkv16, 3 * d, M, 3 * d, FMT_G, G_layer(l, 1), INV, st, txt_rows);
+    else rc = launch_colsum16(T.dqkv16, 3 * d, M, 3 * d, FMT_G, G_layer(l, 1), INV, st, txt_rows);  // in_proj_bias gradient
     if (rc) return rc;
     // ---- in-projections: dgrad dx = dy + [dq|dk|dv] [Wq;Wk;Wv]; wgrad dWqk = [dq|dk]^T (x+pos), dWv = dv^T x ----
     auto qkv_dgrad = [&](GemmProblem& p, int bnn) -> int {
@@ -642,6 +648,18 @@ int univtg_backward(univtg_plan* P, void* ws, const float* src_txt, const float*
       g.fmt = fmt;
       rc = qkv_dgrad(g.p[0], bn_ddq);
       if (rc) return rc;
+      if (txt_pos) {  // d(pos_t) += [dq | dk] [Wq; Wk] over the text rows (the first layer differentiated overwrites)
+        g.num = 2;
+        GemmProblem& p = g.p[1];
+        rc = setup_gemm(p, Mat16{TP.dqk16, Mt, 2 * d, 2 * d}, 0, Mat16{W16(lp.w_in), 2 * d, d, d}, 1, Mt, d, 2 * d, bn_ddq);
+        if (rc) return rc;
+        p.a_fmt = FMT_G;
+        p.b_fmt = fmt;
+        p.resid = l == c.enc_layers - 1 ? nullptr : TP.dpos;
+        p.ld_resid = d;
+        p.out32 = TP.dpos;
+        p.ld32 = d;
+      }
       rc = gemm_launch(P, g, bn_ddq, sms, st);
       if (rc) return rc;
       memset(&g, 0, sizeof(g));
@@ -656,6 +674,32 @@ int univtg_backward(univtg_plan* P, void* ws, const float* src_txt, const float*
   }
 
   // ================================================ projectors ================================================
+  if (txt_pos) {  // LayerNorm (+ dropout) backward of pos_t: its three parameter gradients, and du into the text rows of dx
+    const int base = univtg_num_params(&c);
+    TxtPosBwdArgs a;
+    memset(&a, 0, sizeof(a));
+    a.dpos = TP.dpos;
+    a.xt = T.txtproj32;
+    a.table = P->txt_pos.table;
+    a.gamma = P->txt_pos.ln_weight;
+    a.mean = TP.mean;
+    a.rstd = TP.rstd;
+    a.mul32 = P->txt_pos.drop_mul;
+    if (!a.mul32 && rng != nullptr && rng->input_dropout > 0.f)
+      a.drop = make_drop_spec(rng->seed, (unsigned int)(2 * np), rng->input_dropout);
+    a.dx = T.dx;
+    a.dtable = grads[base];
+    a.dgamma = grads[base + 1];
+    a.dbeta = grads[base + 2];
+    a.pgrad_scale = INV;
+    a.B = B;
+    a.Lt = Lt;
+    a.L = L;
+    a.Lv = Lv;
+    a.d = d;
+    rc = launch_txt_pos_bwd(a, st);
+    if (rc) return rc;
+  }
   // gradient w.r.t. the projected tokens = stream gradient rows + direct (saliency-loss) gradients (dxt_pool: written up front)
   // column sums = bias gradient of the last projector layer AND the token-type embedding rows
   rc = launch_stream_gather(T.dx, L, 0, g_vid_mem_proj, GS, T.dxv16, G_type + d, INV, B, Lv, d, FMT_G, st);

@@ -43,7 +43,8 @@ def make_flat_allreduce_hook(group=None):
 
 def grad_stage_slices(model):
     """[(stage, [(lo, hi), ...]), ...]: slices of the flat gradient buffer that become final at each backward stage
-    (univtg_backward_stages), in completion order.  Together they cover every parameter exactly once."""
+    (univtg_backward_stages), in completion order.  Together they cover every parameter exactly once: with use_txt_pos the three
+    txt_position_embed gradients appended after the C-ABI list are final at stage n - 2 (include/univtg_b200.h)."""
     import ctypes
 
     from . import _lib
@@ -64,6 +65,8 @@ def grad_stage_slices(model):
             first, last = arr[4 * k + j], arr[4 * k + j + 1]
             if last > first:
                 sl.append((offs[first], offs[last]))
+        if model.use_txt_pos and k == n - 2:
+            sl.append((offs[-4], offs[-1]))
         out.append((k, sl))
     return out
 

@@ -53,7 +53,8 @@ class FlatAdamW(torch.optim.Optimizer):
                         decoupled_weight_decay=True)
         # the group lists what the reference hands its AdamW (main/config.py:345-350): every trainable parameter in
         # named_parameters() order - state_dict() numbers parameters by their position in this list.  Parameters outside the
-        # C-ABI list (txt_position_embed.*: never used by the univtg path) receive no gradient here or there and keep no state.
+        # C-ABI list (txt_position_embed.* unless use_txt_pos: then they sit at the end of the flat buffers and are clipped and
+        # updated like the rest) receive no gradient here or there and keep no state.
         torch.optim.Optimizer.__init__(self, [{"params": [p for _, p in model.named_parameters() if p.requires_grad]}], defaults)
 
     # the hyper-parameters live in the (single) parameter group, where torch's lr schedulers write them
@@ -141,7 +142,7 @@ class FlatAdamW(torch.optim.Optimizer):
                        "univtg_adamw_step")
             arr = self.__dict__.get("_ptr_array")
             if arr is None or self.__dict__.get("_ptr_array_base") != self._flat_p.data_ptr():
-                params = model._abi_params()
+                params = model._packed_params()
                 arr = (ctypes.c_void_p * len(params))(*[p.data_ptr() for p in params])
                 self.__dict__["_ptr_array"], self.__dict__["_ptr_array_base"] = arr, self._flat_p.data_ptr()
             _lib.check(lib.univtg_pack_vectors(ctypes.byref(cfg), arr, len(arr), _lib.ptr(packed), _lib.stream_ptr()),

@@ -61,7 +61,7 @@ class _Transformer(nn.Module):
         self.nhead = nhead
 
 
-class _TxtPos(nn.Module):  # TrainablePositionalEncoding keys (unused unless --use_txt_pos; never receives gradients)
+class _TxtPos(nn.Module):  # TrainablePositionalEncoding keys (used with --use_txt_pos; otherwise they receive no gradient)
     def __init__(self, max_q_l, d):
         super().__init__()
         self.position_embeddings = _Params(weight=(max_q_l, d))
@@ -89,9 +89,10 @@ def _uniform_(t, bound):
 
 class _PlanEntry:
     """One (B, Lv, Lt, training) shape bucket: the C plan (shape and tile widths, pointing into the shared workspace)."""
-    __slots__ = ("handle", "shape", "key", "pins", "grad_events_owner")
+    __slots__ = ("handle", "shape", "key", "pins", "grad_events_owner", "txt_pos_scratch")
 
     def __init__(self):
+        self.txt_pos_scratch = None    # inference plans with learned text positions: pos_t (lives as long as the plan)
         self.handle = None
         self.shape = None
         self.key = None
@@ -149,12 +150,11 @@ class Model(nn.Module):
             raise ValueError(f"not supported {args.position_embedding}")
         if not 1 <= self.n_input_proj <= 3:
             raise ValueError("n_input_proj must be 1, 2 or 3")
-        if self.use_txt_pos:
-            raise NotImplementedError("use_txt_pos=True (learned text positions) is outside the accelerated path")
 
         # registration order == reference Model.__init__ (keeps state_dict / optimizer parameter order identical)
         self.transformer = _Transformer(d, self.dim_feedforward, self.enc_layers, self.nheads)
-        self.txt_position_embed = _TxtPos(int(args.max_q_l), d)
+        self.max_q_l = int(args.max_q_l)
+        self.txt_position_embed = _TxtPos(self.max_q_l, d)
         self.token_type_embeddings = _Params(weight=(2, d))
         self.span_embed = _ConvHead(d, 2 if self.span_loss_type == "l1" else self.max_v_l * 2)
         self.class_embed = _ConvHead(d, 1)
@@ -215,8 +215,9 @@ class Model(nn.Module):
         return super()._apply(fn, *args, **kwargs)
 
     def _abi_params(self):
-        """Parameters in the order include/univtg_b200.h documents for univtg_pack_weights (the list is cached: the Parameter
-        objects of this module never change identity; the hot loop asks for it several times per step)."""
+        """Parameters in the order include/univtg_b200.h documents for univtg_pack_weights, followed with use_txt_pos by the three
+        txt_position_embed tensors (univtg_backward's appended gradients).  The list is cached: the Parameter objects of this
+        module never change identity; the hot loop asks for it several times per step."""
         cached = self.__dict__.get("_abi_cache")
         if cached is not None:
             return cached
@@ -233,8 +234,43 @@ class Model(nn.Module):
             for c in head.layers:
                 ps += [c.weight, c.bias]
         ps.append(self.weightedpool.weight)
+        if self.use_txt_pos:
+            tp = self.txt_position_embed
+            ps += [tp.position_embeddings.weight, tp.LayerNorm.weight, tp.LayerNorm.bias]
         self.__dict__["_abi_cache"] = ps
         return ps
+
+    def _packed_params(self):
+        """The univtg_pack_weights prefix of _abi_params() (the text-position tensors are read as they are, never packed)."""
+        ps = self._abi_params()
+        return ps[:-3] if self.use_txt_pos else ps
+
+    def _arm_txt_pos(self, plan, drop_mul=None, scratch=None):
+        """Install the learned text positions on `plan` (univtg_plan_set_txt_pos) with the parameters' CURRENT storage.  Inference
+        plans own their scratch; a training forward passes its own (it carries statistics to its backward)."""
+        if not self.use_txt_pos:
+            return
+        lib = _lib.load_library()
+        if scratch is None:
+            nbytes = lib.univtg_txt_pos_scratch_bytes(ctypes.byref(self._cfg), ctypes.byref(plan.shape))
+            if plan.txt_pos_scratch is None or plan.txt_pos_scratch.device != self._device():
+                plan.txt_pos_scratch = torch.empty(nbytes, dtype=torch.uint8, device=self._device())
+            scratch = plan.txt_pos_scratch
+        tp = self.txt_position_embed
+        for t in (tp.position_embeddings.weight, tp.LayerNorm.weight, tp.LayerNorm.bias):
+            if t.dtype != torch.float32 or not t.is_contiguous() or t.device != self._device():
+                raise RuntimeError("univtg_b200: txt_position_embed parameters must be contiguous float32 tensors on the model's device")
+        st = _lib.TxtPos(tp.position_embeddings.weight.data_ptr(), tp.position_embeddings.weight.shape[0],
+                         tp.LayerNorm.weight.data_ptr(), tp.LayerNorm.bias.data_ptr(),
+                         drop_mul.data_ptr() if drop_mul is not None else None, scratch.data_ptr())
+        _lib.check(lib.univtg_plan_set_txt_pos(plan.handle, ctypes.byref(st)), "univtg_plan_set_txt_pos")
+
+    def _txt_pos_ptrs(self):
+        """Storage of the text-position tensors a captured graph has baked in (FlatAdamW re-seats parameters)."""
+        if not self.use_txt_pos:
+            return None
+        tp = self.txt_position_embed
+        return tuple(t.data_ptr() for t in (tp.position_embeddings.weight, tp.LayerNorm.weight, tp.LayerNorm.bias))
 
     def _device(self):
         return self.weightedpool.weight.device
@@ -247,7 +283,7 @@ class Model(nn.Module):
         lib = _lib.load_library()
         fmt = self._fmt(training)
         cfg = self._cfgs[fmt]
-        params = self._abi_params()
+        params = self._packed_params()
         dev = self._device()
         if dev.type != "cuda":
             raise RuntimeError("univtg_b200: the model must live on a CUDA device (no CPU path); call model.to('cuda')")
@@ -445,6 +481,8 @@ class Model(nn.Module):
             raise ValueError("src_vid / src_txt must be [B, L, D] with the same batch size")
         if src_vid.shape[2] != self.vid_dim or src_txt.shape[2] != self.txt_dim:
             raise ValueError(f"feature dims ({src_vid.shape[2]}, {src_txt.shape[2]}) != model ({self.vid_dim}, {self.txt_dim})")
+        if self.use_txt_pos and src_txt.shape[1] > self.max_q_l:  # the reference's embedding lookup raises IndexError here
+            raise ValueError(f"use_txt_pos: {src_txt.shape[1]} text tokens exceed max_q_l = {self.max_q_l} learned positions")
         dev = self._device()
         if src_vid.device != dev:
             raise RuntimeError(f"inputs on {src_vid.device}, model on {dev}")
@@ -475,6 +513,9 @@ class Model(nn.Module):
             self._ensure_packed()
             cache = self.__dict__.setdefault("_graphs", {})  # _ensure_packed may have dropped plans + graphs
             ent = cache.get(key)
+            if ent is not None and ent["txt_pos"] != self._txt_pos_ptrs():
+                del cache[key]  # the graph baked in text-position tensors that have been re-seated since
+                ent = None
             if ent is None:
                 if len(cache) >= 4:
                     cache.pop(next(iter(cache)))
@@ -491,7 +532,7 @@ class Model(nn.Module):
                 graph = torch.cuda.CUDAGraph()
                 with torch.cuda.graph(graph):
                     outs = self._forward_inference(**static)
-                ent = {"graph": graph, "static": static, "outs": outs}
+                ent = {"graph": graph, "static": static, "outs": outs, "txt_pos": self._txt_pos_ptrs()}
                 cache[key] = ent
             st = ent["static"]
             st["src_txt"].copy_(src_txt, non_blocking=True)
@@ -514,6 +555,7 @@ class Model(nn.Module):
             self._ensure_packed()
             plan = self._get_plan(B, Lv, Lt, False)
             self._activate(plan)
+            self._arm_txt_pos(plan)
             txt, vid = self._feature_inputs(lib, plan, src_txt, src_vid)
             tmask = src_txt_mask.detach().to(torch.float32).contiguous()
             vmask = src_vid_mask.detach().to(torch.float32).contiguous()
@@ -576,7 +618,9 @@ class Model(nn.Module):
         lib = _lib.load_library()
         with torch.cuda.device(self._device()):
             self._ensure_packed()
-            return int(lib.univtg_forward_num_launches(self._get_plan(B, Lv, Lt, False).handle))
+            plan = self._get_plan(B, Lv, Lt, False)
+            self._arm_txt_pos(plan)
+            return int(lib.univtg_forward_num_launches(plan.handle))
 
 
 def build_model(args):
