@@ -218,6 +218,151 @@ int univtg_op_gemm(const void* a, const void* b, int32_t M, int32_t N, int32_t K
 int univtg_op_gemm_cluster(const void* a, const void* b, int32_t M, int32_t N, int32_t K, int32_t a_mn, int32_t b_mn,
                            int32_t fmt, int32_t bn, int32_t ksplit, const float* bias, int32_t act, float alpha, float* out32,
                            void* out16, void* stream);
+/* One problem of univtg_op_gemm_group: C[M,N] = epilogue(sum_k A(m,k) B(n,k)) with the epilogue univtg_backward and the
+ * training forward use.  16-bit formats: 0 fp16, 1 bf16, -1 = the group's `fmt`; A and B must resolve to the same format.
+ *   conv = 0: a [M,K] (a_mn=0) or [K,M] (a_mn=1), b [N,K] (b_mn=0) or [K,N] (b_mn=1), pitches lda / ldb (multiples of 8).
+ *   conv = 1: k=3 Conv1d data gradient in the conv-head layout (buffer row = logical row + 1, rows 0 and M+1 zero): a = dY
+ *             [M+2, K] (K = out channels, multiple of 64), b = packed weight [K, 3N] with b[o, t*N + c] = W[o, c, t] (ldb = 3N);
+ *             row m of the result is sum_t dY[m - t + 1] W[:, :, t].  a_mn = 0, b_mn = 1.
+ *   conv = 2: weight gradient of tap `tap`: a = dY [K+2, M], b = X [K+2, N] (same layout); C[n, c] = sum_m dY[m, n] X[m + tap - 1, c]
+ *             over the K logical rows.  a_mn = b_mn = 1.
+ * Epilogue: v = act(acc + bias[n]) * alpha * row_scale[m / rps_in]; out row = (m / rps_in) * rps_out + m % rps_in + row_off
+ * (identity when rps_in = 0); zero_sep stores v = 0 and skip_sep stores nothing on rows with m % rps_in == rps_in - 1;
+ * v += resid[out row]; mask16 (indexed like out16, group fmt) zeroes v where mask16 <= 0, or multiplies v by it (mask_mul = 1);
+ * out32 at out rows (accumulate = 1: out32 += v), out32_id at row m, out16 at out rows, out16p = 16-bit(v + addtab[m]) at out rows
+ * (pitch ld16), dact16 = GELU'(acc + bias) with act = 2; colsum[n] += colsum_scale * sum of the stored v.  ksplit > 1 splits the K
+ * loop into partial sums added into a pre-zeroed out32; ksplit > 1 and accumulate are rejected with act, resid, out16, out16p,
+ * out32_id or dact16.  vec_ok is an output: 0 scalar, 1 128-bit, 2 256-bit epilogue accesses. */
+typedef struct univtg_gemm_problem {
+  const void* a;
+  int32_t lda, a_mn;
+  const void* b;
+  int32_t ldb, b_mn;
+  int32_t M, N, K, ksplit;
+  int32_t a_fmt, b_fmt, out_fmt;
+  int32_t conv, tap;
+  const float* bias;
+  int32_t act; /* 0 none, 1 ReLU, 2 GELU (erf) */
+  float alpha;
+  const float* row_scale;
+  int32_t rps_in, rps_out, row_off, zero_sep, skip_sep;
+  const float* resid;
+  int32_t ld_resid;
+  const float* addtab;
+  int32_t ld_addtab;
+  float* out32;
+  int32_t ld32;
+  float* out32_id;
+  int32_t ld32_id;
+  void* out16;
+  void* out16p;
+  int32_t ld16, accumulate;
+  const void* mask16;
+  int32_t ld_mask, mask_mul;
+  void* dact16;
+  int32_t ld_dact;
+  float* colsum;
+  float colsum_scale;
+  int32_t vec_ok; /* written */
+} univtg_gemm_problem;
+/* 1 <= num <= 4 problems in one persistent launch (tiles interleaved over the SMs).  bn: tile width (multiple of 16 in [32,256];
+ * of 64 when a B operand is MN-major); cluster = 2 launches 2-CTA clusters (K-major B only).  full (optional) receives 1 when the
+ * FULL epilogue variant ran, 0 for the lean one. */
+int univtg_op_gemm_group(univtg_gemm_problem* problems, int32_t num, int32_t fmt, int32_t bn, int32_t cluster, int32_t* full,
+                         void* stream);
+
+/* LayerNorm backward over rows (the kernels of univtg_backward):  xhat = (y - mean) * rstd, g = dout' * gamma with
+ * dout' = dout * (dout_mul or the in-kernel dropout of (rng, mask_index), as univtg_dropout_mask reads it back),
+ *   dy = rstd * (g - mean_j g - xhat * mean_j(g xhat)), zeroed where y <= 0 when relu_mask_y;  dy32 = dy;
+ *   dbr16 = 16-bit(dy * row_scale[row / L]) with columns [d, ld16) set to 0;  dgamma += pgrad_scale * sum_rows dout' xhat;
+ *   dbeta += pgrad_scale * sum_rows dout';  colsum += pgrad_scale * sum_rows dy * row_scale (fp32, before rounding).
+ * With dy32 = dbr16 = NULL only the parameter gradients are formed, and y may be given as 16-bit (y16, y_fmt). */
+typedef struct univtg_ln_bwd {
+  const float* dout;
+  int32_t ld_dout;
+  const float* y;
+  int32_t ld_y;
+  const void* y16;
+  int32_t y_fmt;
+  const float* mean;
+  const float* rstd;
+  const float* gamma;
+  int32_t rows, d;
+  const float* row_scale;
+  int32_t L, relu_mask_y;
+  float* dy32;
+  void* dbr16;
+  int32_t ld16, fmt16;
+  float* dgamma;
+  float* dbeta;
+  float* colsum;
+  float pgrad_scale;
+  const float* dout_mul;
+} univtg_ln_bwd;
+/* rng == NULL or rng->input_dropout == 0: no in-kernel dropout.  kernel_used (optional) receives the instantiation that ran:
+ * 0 parameters only, 1/2/3 warp-per-row d = 256/512/1024, 4/5 128-bit d <= 512 / <= 1024, 6/7 row-per-block d <= 1024 / <= 3072. */
+int univtg_op_layernorm_bwd(const univtg_ln_bwd* args, const univtg_rng* rng, int32_t mask_index, int32_t* kernel_used, void* stream);
+
+/* Last conv layer of the heads, backward (d % 8 == 0; activations in the conv-head layout [B*(Lv+1)+2, d], fmt_act):
+ *   dz = pre-sigmoid gradients * in_scale [B*(Lv+1)+2, 4] (scratch, written); dh_cls / dh_span = ReLU'(h) * conv-transpose of dz
+ *   (fmt_grad, separator rows 0); gw_* ([o, d, 3]), gb_*, cs_* (column sums of dh_*, both or neither) += pgrad_scale * ... */
+typedef struct univtg_head_final_bwd {
+  const float* g_logits;
+  const float* g_spans;
+  const float* pred_logits;
+  const float* pred_spans;
+  const void* h_cls;
+  const void* h_span;
+  const float* w_cls;  /* [3][d] */
+  const float* w_span; /* [2][3][d] */
+  float* dz;
+  void* dh_cls;
+  void* dh_span;
+  float* gw_cls;
+  float* gb_cls;
+  float* gw_span;
+  float* gb_span;
+  float* cs_cls;
+  float* cs_span;
+  float in_scale, pgrad_scale;
+  int32_t B, Lv, d, fmt_act, fmt_grad;
+} univtg_head_final_bwd;
+int univtg_op_head_final_bwd(const univtg_head_final_bwd* args, void* stream);
+/* colsum[c] += scale * sum_r in16[r, c] (the stored 16-bit values).  txt16 != NULL also copies the text rows (r % L >= Lv) of the
+ * first txt_cols columns into txt16 [rows / L * (L - Lv), txt_cols].  cols, ld, txt_cols multiples of 8, pointers 16-byte aligned. */
+int univtg_op_colsum16(const void* in16, int32_t ld, int32_t rows, int32_t cols, int32_t fmt, float* colsum, float scale, void* txt16,
+                       int32_t L, int32_t Lv, int32_t txt_cols, void* stream);
+/* out16 = 16-bit(in32); colsum (optional) += colsum_scale * column sums of in32 (fp32, before rounding); txt16 as above.
+ * cols, pitches, txt_cols multiples of 4; in32 16-byte, out16 / txt16 8-byte aligned. */
+int univtg_op_cvt16_colsum(const float* in32, int32_t ld_in, void* out16, int32_t ld_out, int32_t rows, int32_t cols, int32_t fmt,
+                           float* colsum, float colsum_scale, void* txt16, int32_t L, int32_t Lv, int32_t txt_cols, void* stream);
+/* out16[b*Ls + l] = 16-bit(dx[b*L + off + l] + extra_scale * extra[b*Ls + l]) (extra optional), colsum (optional) += colsum_scale *
+ * column sums of the fp32 values.  d % 4 == 0, off + Ls <= L, dx / extra 16-byte and out16 8-byte aligned. */
+int univtg_op_stream_gather(const float* dx, int32_t L, int32_t off, const float* extra, float extra_scale, void* out16, float* colsum,
+                            float colsum_scale, int32_t B, int32_t Ls, int32_t d, int32_t fmt, void* stream);
+/* Weighted-pool backward: pooled = sum_l alpha_l x_l; dx_txt [B,Lt,d] = out_scale * (alpha g + dlogit w) (written);
+ * gw [d] += sum dlogit x (unscaled). */
+int univtg_op_pool_bwd(const float* x_txt, const float* alpha, const float* w, const float* g_pooled, float* dx_txt, float* gw,
+                       float out_scale, int32_t B, int32_t Lt, int32_t d, void* stream);
+/* Learned text positions backward (d <= 1024): g = dpos * (mul32 or the dropout of (rng, mask_index)); LayerNorm backward of
+ * u = xt + table[l] with the given mean / rstd; dx[b*L + Lv + l] += du; dtable rows < Lt = pgrad_scale * sum_b du (written);
+ * dgamma / dbeta += pgrad_scale * ... */
+typedef struct univtg_txt_pos_bwd {
+  const float* dpos;
+  const float* xt;
+  const float* table;
+  const float* gamma;
+  const float* mean;
+  const float* rstd;
+  const float* mul32;
+  float* dx;
+  float* dtable;
+  float* dgamma;
+  float* dbeta;
+  float pgrad_scale;
+  int32_t B, Lt, L, Lv, d;
+} univtg_txt_pos_bwd;
+int univtg_op_txt_pos_bwd(const univtg_txt_pos_bwd* args, const univtg_rng* rng, int32_t mask_index, void* stream);
 /* Profiling aid: when `buf` (device, >= num_SMs*8 uint64) is non-NULL every following GEMM launch stamps %globaltimer per CTA:
  * [0] entry, [1] setup done, [2] all TMA issued, [3] first stage landed, [4] last MMA of the first tile retired, [5] unused,
  * [6] epilogue done, [7] exit.  Pass NULL to switch it off. */

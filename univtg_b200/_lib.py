@@ -50,6 +50,43 @@ class TxtPos(ctypes.Structure):
                 ("scratch", c_void_p)]
 
 
+class GemmProblem(ctypes.Structure):
+    """univtg_gemm_problem (one problem of univtg_op_gemm_group)."""
+
+    _fields_ = [("a", c_void_p), ("lda", c_int), ("a_mn", c_int), ("b", c_void_p), ("ldb", c_int), ("b_mn", c_int), ("M", c_int),
+                ("N", c_int), ("K", c_int), ("ksplit", c_int), ("a_fmt", c_int), ("b_fmt", c_int), ("out_fmt", c_int), ("conv", c_int),
+                ("tap", c_int), ("bias", c_void_p), ("act", c_int), ("alpha", c_float), ("row_scale", c_void_p), ("rps_in", c_int),
+                ("rps_out", c_int), ("row_off", c_int), ("zero_sep", c_int), ("skip_sep", c_int), ("resid", c_void_p),
+                ("ld_resid", c_int), ("addtab", c_void_p), ("ld_addtab", c_int), ("out32", c_void_p), ("ld32", c_int),
+                ("out32_id", c_void_p), ("ld32_id", c_int), ("out16", c_void_p), ("out16p", c_void_p), ("ld16", c_int),
+                ("accumulate", c_int), ("mask16", c_void_p), ("ld_mask", c_int), ("mask_mul", c_int), ("dact16", c_void_p),
+                ("ld_dact", c_int), ("colsum", c_void_p), ("colsum_scale", c_float), ("vec_ok", c_int)]
+
+
+class LnBwd(ctypes.Structure):
+    """univtg_ln_bwd."""
+
+    _fields_ = [("dout", c_void_p), ("ld_dout", c_int), ("y", c_void_p), ("ld_y", c_int), ("y16", c_void_p), ("y_fmt", c_int),
+                ("mean", c_void_p), ("rstd", c_void_p), ("gamma", c_void_p), ("rows", c_int), ("d", c_int), ("row_scale", c_void_p),
+                ("L", c_int), ("relu_mask_y", c_int), ("dy32", c_void_p), ("dbr16", c_void_p), ("ld16", c_int), ("fmt16", c_int),
+                ("dgamma", c_void_p), ("dbeta", c_void_p), ("colsum", c_void_p), ("pgrad_scale", c_float), ("dout_mul", c_void_p)]
+
+
+class HeadFinalBwd(ctypes.Structure):
+    """univtg_head_final_bwd."""
+
+    _fields_ = [(n, c_void_p) for n in ("g_logits", "g_spans", "pred_logits", "pred_spans", "h_cls", "h_span", "w_cls", "w_span", "dz",
+                                        "dh_cls", "dh_span", "gw_cls", "gb_cls", "gw_span", "gb_span", "cs_cls", "cs_span")] + \
+        [("in_scale", c_float), ("pgrad_scale", c_float), ("B", c_int), ("Lv", c_int), ("d", c_int), ("fmt_act", c_int), ("fmt_grad", c_int)]
+
+
+class TxtPosBwd(ctypes.Structure):
+    """univtg_txt_pos_bwd."""
+
+    _fields_ = [(n, c_void_p) for n in ("dpos", "xt", "table", "gamma", "mean", "rstd", "mul32", "dx", "dtable", "dgamma", "dbeta")] + \
+        [("pgrad_scale", c_float), ("B", c_int), ("Lt", c_int), ("L", c_int), ("Lv", c_int), ("d", c_int)]
+
+
 # symbol -> (restype, argtypes); every symbol declared in include/univtg_b200.h must be listed here
 SIGNATURES = {
     "univtg_last_error": (ctypes.c_char_p, []),
@@ -101,6 +138,16 @@ SIGNATURES = {
                                c_float, c_void_p, c_void_p, c_void_p]),
     "univtg_op_gemm_cluster": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_int,
                                        c_float, c_void_p, c_void_p, c_void_p]),
+    "univtg_op_gemm_group": (c_int, [ctypes.POINTER(GemmProblem), c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
+    "univtg_op_layernorm_bwd": (c_int, [ctypes.POINTER(LnBwd), ctypes.POINTER(Rng), c_int, c_void_p, c_void_p]),
+    "univtg_op_head_final_bwd": (c_int, [ctypes.POINTER(HeadFinalBwd), c_void_p]),
+    "univtg_op_colsum16": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_float, c_void_p, c_int, c_int, c_int, c_void_p]),
+    "univtg_op_cvt16_colsum": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_float, c_void_p, c_int, c_int,
+                                       c_int, c_void_p]),
+    "univtg_op_stream_gather": (c_int, [c_void_p, c_int, c_int, c_void_p, c_float, c_void_p, c_void_p, c_float, c_int, c_int, c_int,
+                                        c_int, c_void_p]),
+    "univtg_op_pool_bwd": (c_int, [c_void_p] * 6 + [c_float, c_int, c_int, c_int, c_void_p]),
+    "univtg_op_txt_pos_bwd": (c_int, [ctypes.POINTER(TxtPosBwd), ctypes.POINTER(Rng), c_int, c_void_p]),
     "univtg_debug_gemm_timeline": (c_int, [c_void_p]),
     "univtg_debug_choose_tile": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     "univtg_op_layernorm": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_float, c_int, c_void_p, c_void_p, c_int,

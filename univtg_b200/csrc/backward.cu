@@ -325,9 +325,10 @@ __global__ void __launch_bounds__(256) layernorm_bwd_params_kernel(const LnBwdAr
   if (in && a.dbeta) atomicAdd(a.dbeta + j, ab * a.pgrad_scale);
 }
 
-int launch_layernorm_bwd(const LnBwdArgs& a, cudaStream_t stream) {
+int launch_layernorm_bwd(const LnBwdArgs& a, cudaStream_t stream, int* kernel_used) {
   if (a.rows <= 0) return 0;
   if (a.dy32 == nullptr && a.dbr16 == nullptr) {
+    if (kernel_used) *kernel_used = LNB_PARAMS;
     launch_k(layernorm_bwd_params_kernel, dim3(dim3((a.d + 255) / 256, (a.rows + kLnParamRows - 1) / kLnParamRows)), dim3(256), 0, stream, a);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) set_error("layernorm_bwd launch failed: %s", cudaGetErrorString(e));
@@ -363,11 +364,20 @@ int launch_layernorm_bwd(const LnBwdArgs& a, cudaStream_t stream) {
     if (a.d == 1024) launch_k(layernorm_bwd_warp_kernel<8>, dim3(wgrid), dim3(256), smem, stream, a);
     else if (a.d == 512) launch_k(layernorm_bwd_warp_kernel<4>, dim3(wgrid), dim3(256), smem, stream, a);
     else launch_k(layernorm_bwd_warp_kernel<2>, dim3(wgrid), dim3(256), smem, stream, a);
-  } else if (vec && a.d <= 512) launch_k(layernorm_bwd_vec_kernel<1>, dim3(grid), dim3(128), 0, stream, a);
-  else if (vec && a.d <= 1024) launch_k(layernorm_bwd_vec_kernel<2>, dim3(grid), dim3(128), 0, stream, a);
-  else if (a.d <= 128 * 8) launch_k(layernorm_bwd_kernel<8>, dim3(grid), dim3(128), 0, stream, a);
-  else if (a.d <= 128 * 24) launch_k(layernorm_bwd_kernel<24>, dim3(grid), dim3(128), 0, stream, a);
-  else {
+    if (kernel_used) *kernel_used = a.d == 1024 ? LNB_WARP8 : (a.d == 512 ? LNB_WARP4 : LNB_WARP2);
+  } else if (vec && a.d <= 512) {
+    launch_k(layernorm_bwd_vec_kernel<1>, dim3(grid), dim3(128), 0, stream, a);
+    if (kernel_used) *kernel_used = LNB_VEC1;
+  } else if (vec && a.d <= 1024) {
+    launch_k(layernorm_bwd_vec_kernel<2>, dim3(grid), dim3(128), 0, stream, a);
+    if (kernel_used) *kernel_used = LNB_VEC2;
+  } else if (a.d <= 128 * 8) {
+    launch_k(layernorm_bwd_kernel<8>, dim3(grid), dim3(128), 0, stream, a);
+    if (kernel_used) *kernel_used = LNB_ROW8;
+  } else if (a.d <= 128 * 24) {
+    launch_k(layernorm_bwd_kernel<24>, dim3(grid), dim3(128), 0, stream, a);
+    if (kernel_used) *kernel_used = LNB_ROW24;
+  } else {
     set_error("layernorm_bwd: d %d > 3072 not supported", a.d);
     return (int)cudaErrorInvalidValue;
   }

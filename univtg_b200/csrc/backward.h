@@ -35,7 +35,9 @@ struct LnBwdArgs {
   const float* dout_mul;   // optional [rows, d] multiplier applied to dout on load (input-dropout mask incl. 1/(1-p))
   DropSpec drop;           // in-kernel regeneration of the forward's input-dropout multipliers (drop.on; ignored with dout_mul)
 };
-int launch_layernorm_bwd(const LnBwdArgs& a, cudaStream_t stream);
+// kernel_used (optional): which instantiation ran (LnbKernel; the same numbering as univtg_op_layernorm_bwd reports)
+enum LnbKernel { LNB_PARAMS = 0, LNB_WARP2 = 1, LNB_WARP4 = 2, LNB_WARP8 = 3, LNB_VEC1 = 4, LNB_VEC2 = 5, LNB_ROW8 = 6, LNB_ROW24 = 7 };
+int launch_layernorm_bwd(const LnBwdArgs& a, cudaStream_t stream, int* kernel_used = nullptr);
 
 // Optional compact copy of the text rows (row r = b*L + l, l >= Lv) of the first txt_cols columns of the 16-bit output, as
 // [B*(L-Lv), txt_cols] (the [dq | dk] rows the learned text positions' gradient needs); txt16 == NULL: no copy.

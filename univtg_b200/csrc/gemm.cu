@@ -687,7 +687,7 @@ int make_tmap_b_mn(GemmProblem& p, const void* base, uint64_t rows, uint64_t col
   return 0;
 }
 
-int launch_gemm_group(GemmGroup& g, int bn, int num_sms, cudaStream_t stream) {
+int launch_gemm_group(GemmGroup& g, int bn, int num_sms, cudaStream_t stream, int* used_full) {
   using Cfg = GemmCfg<1>;
   static_assert(GemmCfg<1>::kSmemBytes == GemmCfg<2>::kSmemBytes, "both variants use the same dynamic shared memory size");
   if (g.num < 1 || g.num > GEMM_MAX_GROUP) {
@@ -741,6 +741,17 @@ int launch_gemm_group(GemmGroup& g, int bn, int num_sms, cudaStream_t stream) {
       set_error("gemm problem %d: MN-major B needs BN %% %d == 0 (got %d)", p, 64 * cl, bn);
       return (int)cudaErrorInvalidValue;
     }
+    // split-K tiles and `accumulate` add partial sums into out32: only options that are linear in the accumulator (bias is added by
+    // split 0 alone) may run on a partial sum; an activation, a residual or a 16-bit / identity-row store of one would be wrong
+    if (pr.ksplit > 1 || pr.accumulate) {
+      const char* bad = pr.dact16 ? "dact16" : pr.act != ACT_NONE ? "act" : pr.resid ? "resid" : pr.out16 ? "out16"
+                        : pr.out16p ? "out16p" : pr.out32_id ? "out32_id" : nullptr;
+      if (bad != nullptr) {
+        set_error("gemm problem %d: %s cannot be combined with %s (each split would apply it to a partial sum)", p, bad,
+                  pr.ksplit > 1 ? "ksplit > 1" : "accumulate");
+        return (int)cudaErrorInvalidValue;
+      }
+    }
     const int fa = pr.a_fmt < 0 ? g.fmt : pr.a_fmt, fb = pr.b_fmt < 0 ? g.fmt : pr.b_fmt;
     if (fa != fb) {
       set_error("gemm problem %d: A and B must share one 16-bit format (wgmma), got %d and %d", p, fa, fb);
@@ -774,6 +785,7 @@ int launch_gemm_group(GemmGroup& g, int bn, int num_sms, cudaStream_t stream) {
     const GemmProblem& pr = g.p[p];
     full = full || pr.vec_ok != 2 || pr.pre32 || pr.dact16 || pr.aux32 || pr.mask16 || pr.accumulate || pr.ksplit > 1 || pr.out32_id || pr.colsum || pr.cs32 > 1;
   }
+  if (used_full) *used_full = full ? 1 : 0;
   g.bn = bn;
   g.dbg = g_timeline;
   cudaError_t e;

@@ -36,7 +36,9 @@ struct GemmProblem {
   int M, N;
   int taps;          // 1 = plain; 3 = k=3 conv expressed as 3 K segments
   int kblk_per_tap;  // 64-wide k-blocks per tap
-  int ksplit;        // >=1; k-blocks are split over `ksplit` tiles that accumulate atomically into out32
+  int ksplit;        // >=1; k-blocks are split over `ksplit` tiles that accumulate atomically into out32, which the caller must have
+                     // zeroed (or filled with what the sum should be added to).  ksplit > 1 and `accumulate` are rejected together
+                     // with act, resid, out16, out16p, out32_id or dact16, which are not additive over partial sums.
   // ---- epilogue:  v = act(acc + bias[n]) * alpha * row_scale[b(m)]  (+ resid[orow, n]) ----
   const float* bias;
   float alpha;
@@ -89,8 +91,8 @@ struct GemmGroup {
 };
 
 // bn: tile width, multiple of 16 in [32, 256] (multiple of 64 when a problem has an MN-major B).  A and B of a problem must share
-// one 16-bit format.  Returns cudaError_t as int.
-int launch_gemm_group(GemmGroup& g, int bn, int num_sms, cudaStream_t stream);
+// one 16-bit format.  Returns cudaError_t as int.  used_full (optional): 1 when the FULL epilogue variant was launched, 0 for the lean one.
+int launch_gemm_group(GemmGroup& g, int bn, int num_sms, cudaStream_t stream, int* used_full = nullptr);
 // Tile width minimising waves x tile-time for problems that share a launch (step 16: K-major B, 64: MN-major B).
 struct TileChoice {
   int bn, ksplit;

@@ -385,6 +385,45 @@ int setup_gemm(GemmProblem& p, Mat16 A, int a_mn, Mat16 B, int b_mn, int M, int 
   return rc;
 }
 
+// k=3 Conv1d backward in the conv-head layout (buffer row = logical row + 1; rows 0, Mh + 1 and every sample's separator row are
+// zeros).  fmt_g / fmt_w: formats of the gradient / weight-or-activation operand.
+// dgrad: dX[m] = sum_t' dY[m + t' - 1] W[:, :, 2 - t'] over Mh logical rows.  A = dY [Mh + 2, Kc] (pitch ldy, K-major, row-shifted
+// by the tap), B = packed W [Kc, 3 * Cin] (MN-major, w2[o, t * Cin + c] = W[o, c, t]); N = Cin, K = 3 taps x Kc (Kc % 64 == 0).
+int conv_dgrad_problem(GemmProblem& p, int Mh, const uint16_t* dY, int ldy, int Kc, const uint16_t* Wp, int Cin, int bn, int fmt_g,
+                       int fmt_w) {
+  init_problem(p);
+  p.M = Mh;
+  p.N = Cin;
+  p.taps = 3;
+  p.kblk_per_tap = Kc / 64;
+  p.b_mn = 1;
+  p.a_fmt = fmt_g;
+  p.b_fmt = fmt_w;
+  p.ca = OperandCoord{0, 0, 0, 1, 0, 1, 1, 0};           // rows m0 + t', cols k
+  p.cb = OperandCoord{2 * Cin, 1, -Cin, 0, 0, 0, 0, 1};  // cols n0 + (2 - t') * Cin, rows k (out channel)
+  int r = make_tmap_2d(&p.tm_a, dY, (uint64_t)Mh + 2, (uint64_t)Kc, (uint64_t)ldy, GEMM_BM, 64);
+  r |= make_tmap_b_mn(p, Wp, (uint64_t)Kc, (uint64_t)3 * Cin, (uint64_t)3 * Cin, bn);
+  return r;
+}
+// wgrad of tap t: dW[n, c, t] = sum_m dY[m, n] X[m + t - 1, c] over Mh logical rows.  A = dY [Mh + 2, Nc] (pitch ldy, MN-major),
+// B = X [Mh + 2, Cin] (pitch ldx, MN-major, row-shifted by t); M = Nc, N = Cin, K = Mh.
+int conv_wgrad_problem(GemmProblem& p, int Mh, const uint16_t* dY, int ldy, int Nc, const uint16_t* X, int ldx, int Cin, int t, int bn,
+                       int fmt_g, int fmt_w) {
+  init_problem(p);
+  p.M = Nc;
+  p.N = Cin;
+  p.a_mn = 1;
+  p.b_mn = 1;
+  p.a_fmt = fmt_g;
+  p.b_fmt = fmt_w;
+  p.kblk_per_tap = (Mh + 63) / 64;
+  p.ca = OperandCoord{0, 1, 0, 0, 1, 0, 0, 1};  // cols m0 (out channel), rows 1 + k
+  p.cb = OperandCoord{0, 1, 0, 0, t, 0, 0, 1};  // cols n0 (in channel), rows t + k
+  int r = make_tmap_2d(&p.tm_a, dY, (uint64_t)Mh + 2, (uint64_t)Nc, (uint64_t)ldy, 64, 64);
+  r |= make_tmap_b_mn(p, X, (uint64_t)Mh + 2, (uint64_t)Cin, (uint64_t)ldx, bn);
+  return r;
+}
+
 // K-major linear problem: A [M, K] (pitch lda), W [N, K] (pitch ldw).
 inline int setup_linear(GemmProblem& p, const uint16_t* A, int M, int K, int lda, const uint16_t* W, int N, int ldw, int bn) {
   return setup_gemm(p, Mat16{A, M, K, lda}, 0, Mat16{W, N, K, ldw}, 0, M, N, K, bn);

@@ -268,41 +268,14 @@ int univtg_backward(univtg_plan* P, void* ws, const float* src_txt, const float*
     rc = launch_head_final_bwd(a, st);
     if (rc) return rc;
 
-    // conv layout helpers: buffer row = logical row + 1
-    // dgrad of a k=3 conv: dX[m] = sum_t' dY[m + t' - 1] W[:, :, 2 - t']  (A = dY K-major with row shift, B = packed W MN-major)
+    // conv layout helpers (conv_dgrad_problem / conv_wgrad_problem, plan.h): buffer row = logical row + 1
     auto conv_dgrad = [&](GemmProblem& p, const uint16_t* dY, int ldy, int Kc /*out channels*/, const uint16_t* Wp /*[Kc, 3*Cin]*/,
-                          int Cin, int bnn) -> int {
-      init_problem(p);
-      p.M = Mh;
-      p.N = Cin;
-      p.taps = 3;
-      p.kblk_per_tap = Kc / 64;
-      p.b_mn = 1;
-      p.a_fmt = FMT_G;
-      p.b_fmt = fmt;
-      p.ca = OperandCoord{0, 0, 0, 1, 0, 1, 1, 0};              // rows m0 + t', cols k
-      p.cb = OperandCoord{2 * Cin, 1, -Cin, 0, 0, 0, 0, 1};     // cols n0 + (2 - t') * Cin, rows k (out channel)
-      int r = make_tmap_2d(&p.tm_a, dY, (uint64_t)Mh + 2, (uint64_t)Kc, (uint64_t)ldy, GEMM_BM, 64);
-      r |= make_tmap_b_mn(p, Wp, (uint64_t)Kc, (uint64_t)3 * Cin, (uint64_t)3 * Cin, bnn);
-      return r;
-    };
-    // wgrad of one tap: dW[n, c, t] = sum_m dY[m, n] X[m + t - 1, c]  -> written with column stride 3 into [N, C, 3]
+                          int Cin, int bnn) -> int { return conv_dgrad_problem(p, Mh, dY, ldy, Kc, Wp, Cin, bnn, FMT_G, fmt); };
+    // wgrad of one tap, written as a tap-major plane of T.wtap (launch_tap_interleave then builds the [N, C, 3] layout with 256-bit
+    // stores here instead of stride-3 scalars)
     const TileChoice t_cw = tile_for(sms, 64, 8, MNK{d, d, Mh}, MNK{d, d, Mh}, MNK{d, d, Mh});
-    auto conv_wgrad = [&](GemmProblem& p, const uint16_t* dY, int ldy, int Nc, const uint16_t* X, int ldx, int Cin, int t,
-                          float* gw) -> int {
-      init_problem(p);
-      p.M = Nc;
-      p.N = Cin;
-      p.a_mn = 1;
-      p.b_mn = 1;
-      p.a_fmt = FMT_G;
-      p.b_fmt = fmt;
-      p.kblk_per_tap = (Mh + 63) / 64;
-      p.ca = OperandCoord{0, 1, 0, 0, 1, 0, 0, 1};      // cols m0 (out channel), rows 1 + k
-      p.cb = OperandCoord{0, 1, 0, 0, t, 0, 0, 1};      // cols n0 (in channel), rows t + k
-      int r = make_tmap_2d(&p.tm_a, dY, (uint64_t)Mh + 2, (uint64_t)Nc, (uint64_t)ldy, 64, 64);
-      r |= make_tmap_b_mn(p, X, (uint64_t)Mh + 2, (uint64_t)Cin, (uint64_t)ldx, t_cw.bn);
-      (void)gw;  // written by launch_tap_interleave from the tap-major planes (256-bit stores here instead of stride-3 scalars)
+    auto conv_wgrad = [&](GemmProblem& p, const uint16_t* dY, int ldy, int Nc, const uint16_t* X, int ldx, int Cin, int t) -> int {
+      const int r = conv_wgrad_problem(p, Mh, dY, ldy, Nc, X, ldx, Cin, t, t_cw.bn, FMT_G, fmt);
       p.out32 = T.wtap + (size_t)t * Nc * Cin;
       p.ld32 = Cin;
       p.alpha = INV;
@@ -344,7 +317,7 @@ int univtg_backward(univtg_plan* P, void* ws, const float* src_txt, const float*
       g.num = 3;
       g.fmt = fmt;
       for (int t = 0; t < 3; ++t)
-        rc |= conv_wgrad(g.p[t], s == 0 ? T.dhc2 : T.dhs2, d, d, T.h1 + s * d, 2 * d, d, t, s == 0 ? G_cls(2) : G_span(2));
+        rc |= conv_wgrad(g.p[t], s == 0 ? T.dhc2 : T.dhs2, d, d, T.h1 + s * d, 2 * d, d, t);
       if (rc) return rc;
       if (t_cw.ksplit > 1) cudaMemsetAsync(T.wtap, 0, (size_t)3 * d * d * 4, st);  // split-K accumulates into the planes
       rc = gemm_launch(P, g, bn_cw, sms, st);
@@ -371,7 +344,7 @@ int univtg_backward(univtg_plan* P, void* ws, const float* src_txt, const float*
       memset(&g, 0, sizeof(g));
       g.num = 3;
       g.fmt = fmt;
-      for (int t = 0; t < 3; ++t) rc |= conv_wgrad(g.p[t], T.dh1 + s * d, 2 * d, d, T.hA, d, d, t, s == 0 ? G_cls(0) : G_span(0));
+      for (int t = 0; t < 3; ++t) rc |= conv_wgrad(g.p[t], T.dh1 + s * d, 2 * d, d, T.hA, d, d, t);
       if (rc) return rc;
       if (t_cw.ksplit > 1) cudaMemsetAsync(T.wtap, 0, (size_t)3 * d * d * 4, st);
       rc = gemm_launch(P, g, bn_cw, sms, st);
@@ -915,6 +888,316 @@ int univtg_op_attention_bwd(const void* qkv, const void* dO, const void* O, cons
   if (make_tmap_2d(&a.tm_do, dO, (uint64_t)M, (uint64_t)d, (uint64_t)d, 128, 64)) return 1;
   return launch_attention_bwd(a, st);
 }
+
+// ---- single backward operators: thin wrappers over the launchers univtg_backward uses.  Each checks on the host what its kernel
+// assumes (null pointers, vector widths, alignment, size limits) and names the offending argument before anything is launched. ----
+#define UV_REQ(cond, ...)      \
+  do {                         \
+    if (!(cond)) {             \
+      set_error(__VA_ARGS__);  \
+      return 1;                \
+    }                          \
+  } while (0)
+static bool al_(const void* p, int bytes) { return (reinterpret_cast<uintptr_t>(p) & (uintptr_t)(bytes - 1)) == 0; }
+
+int univtg_op_gemm_group(univtg_gemm_problem* problems, int32_t num, int32_t fmt, int32_t bn, int32_t cluster, int32_t* full,
+                         void* stream) {
+  const char* fn = "univtg_op_gemm_group";
+  UV_REQ(problems != nullptr && num >= 1 && num <= GEMM_MAX_GROUP, "%s: problems must hold 1..%d entries", fn, GEMM_MAX_GROUP);
+  UV_REQ(fmt == 0 || fmt == 1, "%s: fmt %d (0 fp16, 1 bf16)", fn, fmt);
+  UV_REQ(bn >= 32 && bn <= 256 && bn % 16 == 0, "%s: bn %d (multiple of 16 in [32, 256])", fn, bn);
+  UV_REQ(cluster == 1 || cluster == 2, "%s: cluster %d (1 or 2)", fn, cluster);
+  GemmGroup g;
+  memset(&g, 0, sizeof(g));
+  g.num = num;
+  g.fmt = fmt;
+  g.cluster = cluster;
+  for (int i = 0; i < num; ++i) {
+    const univtg_gemm_problem& q = problems[i];
+    GemmProblem& p = g.p[i];
+    UV_REQ(q.a && q.b, "%s: problem %d: null a or b", fn, i);
+    UV_REQ(q.M >= 1 && q.N >= 1 && q.K >= 1, "%s: problem %d: M, N, K must be >= 1", fn, i);
+    UV_REQ(q.lda % 8 == 0 && q.ldb % 8 == 0 && al_(q.a, 16) && al_(q.b, 16), "%s: problem %d: lda / ldb must be multiples of 8 and a / b 16-byte aligned", fn, i);
+    UV_REQ(q.ksplit >= 1, "%s: problem %d: ksplit %d", fn, i, q.ksplit);
+    for (int f : {q.a_fmt, q.b_fmt, q.out_fmt}) UV_REQ(f >= -1 && f <= 1, "%s: problem %d: 16-bit format %d (-1, 0, 1)", fn, i, f);
+    UV_REQ(q.act >= ACT_NONE && q.act <= ACT_GELU, "%s: problem %d: act %d", fn, i, q.act);
+    UV_REQ(!q.dact16 || q.act == ACT_GELU, "%s: problem %d: dact16 needs act = 2 (GELU)", fn, i);
+    UV_REQ(!q.mask_mul || q.mask16, "%s: problem %d: mask_mul needs mask16", fn, i);
+    UV_REQ(!(q.zero_sep || q.skip_sep) || q.rps_in > 0, "%s: problem %d: zero_sep / skip_sep need rps_in > 0", fn, i);
+    UV_REQ(q.rps_in >= 0 && (q.rps_in == 0 || q.rps_out >= q.rps_in) && q.row_off >= 0, "%s: problem %d: rps_in %d / rps_out %d / row_off %d",
+           fn, i, q.rps_in, q.rps_out, q.row_off);
+    UV_REQ(!q.addtab || q.out16p, "%s: problem %d: addtab is only used with out16p", fn, i);
+    UV_REQ(!q.out32 || q.ld32 >= q.N, "%s: problem %d: ld32 %d < N %d", fn, i, q.ld32, q.N);
+    UV_REQ(!q.out32_id || q.ld32_id >= q.N, "%s: problem %d: ld32_id %d < N %d", fn, i, q.ld32_id, q.N);
+    UV_REQ(!(q.out16 || q.out16p) || q.ld16 >= q.N, "%s: problem %d: ld16 %d < N %d", fn, i, q.ld16, q.N);
+    UV_REQ(!q.resid || q.ld_resid >= q.N, "%s: problem %d: ld_resid %d < N %d", fn, i, q.ld_resid, q.N);
+    UV_REQ(!q.addtab || q.ld_addtab >= q.N, "%s: problem %d: ld_addtab %d < N %d", fn, i, q.ld_addtab, q.N);
+    UV_REQ(!q.mask16 || q.ld_mask >= q.N, "%s: problem %d: ld_mask %d < N %d", fn, i, q.ld_mask, q.N);
+    UV_REQ(!q.dact16 || q.ld_dact >= q.N, "%s: problem %d: ld_dact %d < N %d", fn, i, q.ld_dact, q.N);
+    // scalar-path stores are element-wise; the vector paths are chosen by launch_gemm_group only where alignment allows them
+    UV_REQ(al_(q.out32, 4) && al_(q.out32_id, 4) && al_(q.resid, 4) && al_(q.addtab, 4) && al_(q.colsum, 4) && al_(q.out16, 2) &&
+               al_(q.out16p, 2) && al_(q.mask16, 2) && al_(q.dact16, 2),
+           "%s: problem %d: misaligned epilogue pointer", fn, i);
+    const int fg = q.a_fmt < 0 ? fmt : q.a_fmt, fw = q.b_fmt < 0 ? fmt : q.b_fmt;
+    int rc = 0;
+    if (q.conv == 1) {
+      UV_REQ(!q.a_mn && q.b_mn && q.K % 64 == 0, "%s: problem %d: conv dgrad needs a_mn = 0, b_mn = 1 and K %% 64 == 0", fn, i);
+      UV_REQ(q.ldb == 3 * q.N, "%s: problem %d: conv dgrad weight pitch ldb must be 3 N", fn, i);
+      rc = conv_dgrad_problem(p, q.M, reinterpret_cast<const uint16_t*>(q.a), q.lda, q.K, reinterpret_cast<const uint16_t*>(q.b), q.N, bn,
+                              fg, fw);
+    } else if (q.conv == 2) {
+      UV_REQ(q.a_mn && q.b_mn && q.tap >= 0 && q.tap <= 2, "%s: problem %d: conv wgrad needs a_mn = b_mn = 1 and tap in 0..2", fn, i);
+      rc = conv_wgrad_problem(p, q.K, reinterpret_cast<const uint16_t*>(q.a), q.lda, q.M, reinterpret_cast<const uint16_t*>(q.b), q.ldb,
+                              q.N, q.tap, bn, fg, fw);
+    } else {
+      UV_REQ(q.conv == 0, "%s: problem %d: conv %d (0 plain, 1 dgrad, 2 wgrad)", fn, i, q.conv);
+      const Mat16 A = q.a_mn ? Mat16{reinterpret_cast<const uint16_t*>(q.a), q.K, q.M, q.lda}
+                             : Mat16{reinterpret_cast<const uint16_t*>(q.a), q.M, q.K, q.lda};
+      const Mat16 Bm = q.b_mn ? Mat16{reinterpret_cast<const uint16_t*>(q.b), q.K, q.N, q.ldb}
+                              : Mat16{reinterpret_cast<const uint16_t*>(q.b), q.N, q.K, q.ldb};
+      UV_REQ(A.ld >= A.cols && Bm.ld >= Bm.cols, "%s: problem %d: lda / ldb smaller than the operand's row length", fn, i);
+      rc = setup_gemm(p, A, q.a_mn, Bm, q.b_mn, q.M, q.N, q.K, cluster == 2 && !q.b_mn ? bn / 2 : bn);
+      p.a_fmt = q.a_fmt;
+      p.b_fmt = q.b_fmt;
+    }
+    if (rc) return rc;
+    p.ksplit = q.ksplit;
+    p.out_fmt = q.out_fmt;
+    p.bias = q.bias;
+    p.act = q.act;
+    p.alpha = q.alpha;
+    p.row_scale = q.row_scale;
+    p.rps_in = q.rps_in;
+    p.rps_out = q.rps_out;
+    p.row_off = q.row_off;
+    p.zero_sep = q.zero_sep;
+    p.skip_sep = q.skip_sep;
+    p.resid = q.resid;
+    p.ld_resid = q.ld_resid;
+    p.addtab = q.addtab;
+    p.ld_addtab = q.ld_addtab;
+    p.out32 = q.out32;
+    p.ld32 = q.ld32;
+    p.out32_id = q.out32_id;
+    p.ld32_id = q.ld32_id;
+    p.out16 = reinterpret_cast<uint16_t*>(q.out16);
+    p.out16p = reinterpret_cast<uint16_t*>(q.out16p);
+    p.ld16 = q.ld16;
+    p.accumulate = q.accumulate;
+    p.mask16 = reinterpret_cast<const uint16_t*>(q.mask16);
+    p.ld_mask = q.ld_mask;
+    p.mask_mul = q.mask_mul;
+    p.dact16 = reinterpret_cast<uint16_t*>(q.dact16);
+    p.ld_dact = q.ld_dact;
+    p.colsum = q.colsum;
+    p.colsum_scale = q.colsum_scale;
+  }
+  int dev = 0, sms = 0;
+  cudaGetDevice(&dev);
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  int used_full = 0;
+  const int rc = launch_gemm_group(g, bn, sms, (cudaStream_t)stream, &used_full);
+  for (int i = 0; i < num; ++i) problems[i].vec_ok = g.p[i].vec_ok;
+  if (full) *full = used_full;
+  return rc;
+}
+
+int univtg_op_layernorm_bwd(const univtg_ln_bwd* q, const univtg_rng* rng, int32_t mask_index, int32_t* kernel_used, void* stream) {
+  const char* fn = "univtg_op_layernorm_bwd";
+  UV_REQ(q != nullptr, "%s: null args", fn);
+  UV_REQ(q->dout && (q->y || q->y16) && q->mean && q->rstd && q->gamma, "%s: null dout, y / y16, mean, rstd or gamma", fn);
+  UV_REQ(q->rows >= 1 && q->d >= 1 && q->d <= 3072, "%s: rows %d / d %d (d <= 3072)", fn, q->rows, q->d);
+  UV_REQ(q->ld_dout >= q->d && q->ld_y >= q->d, "%s: ld_dout %d / ld_y %d smaller than d %d", fn, q->ld_dout, q->ld_y, q->d);
+  UV_REQ(!q->dbr16 || q->ld16 >= q->d, "%s: ld16 %d smaller than d %d", fn, q->ld16, q->d);
+  UV_REQ(!q->y16 || (!q->dy32 && !q->dbr16), "%s: a 16-bit y (y16) is only supported for parameter gradients (dy32 = dbr16 = NULL)", fn);
+  UV_REQ(!q->row_scale || q->L >= 1, "%s: row_scale needs L >= 1", fn);
+  UV_REQ(q->fmt16 == 0 || q->fmt16 == 1, "%s: fmt16 %d", fn, q->fmt16);
+  UV_REQ(q->y_fmt == 0 || q->y_fmt == 1, "%s: y_fmt %d", fn, q->y_fmt);
+  UV_REQ(al_(q->dout, 4) && al_(q->y, 4) && al_(q->y16, 2) && al_(q->dbr16, 2) && al_(q->dy32, 4) && al_(q->dgamma, 4) &&
+             al_(q->dbeta, 4) && al_(q->colsum, 4) && al_(q->dout_mul, 4),
+         "%s: misaligned pointer", fn);
+  UV_REQ(!rng || !(rng->input_dropout > 0.f) || mask_index >= 0, "%s: mask_index %d", fn, mask_index);
+  LnBwdArgs a;
+  memset(&a, 0, sizeof(a));
+  a.dout = q->dout;
+  a.ld_dout = q->ld_dout;
+  a.y = q->y16 ? reinterpret_cast<const float*>(q->y16) : q->y;
+  a.ld_y = q->ld_y;
+  a.y16 = reinterpret_cast<const uint16_t*>(q->y16);
+  a.y_fmt = q->y_fmt;
+  a.mean = q->mean;
+  a.rstd = q->rstd;
+  a.gamma = q->gamma;
+  a.rows = q->rows;
+  a.d = q->d;
+  a.row_scale = q->row_scale;
+  a.L = q->L;
+  a.relu_mask_y = q->relu_mask_y;
+  a.dy32 = q->dy32;
+  a.dbr16 = reinterpret_cast<uint16_t*>(q->dbr16);
+  a.ld16 = q->ld16;
+  a.fmt16 = q->fmt16;
+  a.dgamma = q->dgamma;
+  a.dbeta = q->dbeta;
+  a.colsum = q->colsum;
+  a.pgrad_scale = q->pgrad_scale;
+  a.dout_mul = q->dout_mul;
+  if (!a.dout_mul && rng && rng->input_dropout > 0.f) a.drop = make_drop_spec(rng->seed, (unsigned int)mask_index, rng->input_dropout);
+  int used = -1;
+  const int rc = launch_layernorm_bwd(a, (cudaStream_t)stream, &used);
+  if (kernel_used) *kernel_used = used;
+  return rc;
+}
+
+int univtg_op_head_final_bwd(const univtg_head_final_bwd* q, void* stream) {
+  const char* fn = "univtg_op_head_final_bwd";
+  UV_REQ(q != nullptr, "%s: null args", fn);
+  UV_REQ(q->g_logits && q->g_spans && q->pred_logits && q->pred_spans && q->h_cls && q->h_span && q->w_cls && q->w_span && q->dz &&
+             q->dh_cls && q->dh_span && q->gw_cls && q->gb_cls && q->gw_span && q->gb_span,
+         "%s: null pointer argument", fn);
+  UV_REQ((q->cs_cls == nullptr) == (q->cs_span == nullptr), "%s: cs_cls and cs_span must both be given or both be NULL", fn);
+  UV_REQ(q->B >= 1 && q->Lv >= 1, "%s: B %d / Lv %d", fn, q->B, q->Lv);
+  UV_REQ(q->d >= 8 && q->d % 8 == 0, "%s: d %d must be a positive multiple of 8 (128-bit loads)", fn, q->d);
+  UV_REQ((q->fmt_act == 0 || q->fmt_act == 1) && (q->fmt_grad == 0 || q->fmt_grad == 1), "%s: fmt_act / fmt_grad", fn);
+  UV_REQ(al_(q->h_cls, 16) && al_(q->h_span, 16) && al_(q->dh_cls, 16) && al_(q->dh_span, 16) && al_(q->dz, 16) && al_(q->gw_cls, 16) &&
+             al_(q->gw_span, 16) && al_(q->cs_cls, 16) && al_(q->cs_span, 16),
+         "%s: h_*, dh_*, dz, gw_* and cs_* must be 16-byte aligned", fn);
+  UV_REQ(al_(q->g_logits, 4) && al_(q->g_spans, 4) && al_(q->pred_logits, 4) && al_(q->pred_spans, 4) && al_(q->w_cls, 4) &&
+             al_(q->w_span, 4) && al_(q->gb_cls, 4) && al_(q->gb_span, 4),
+         "%s: misaligned fp32 pointer", fn);
+  HeadFinalBwdArgs a;
+  memset(&a, 0, sizeof(a));
+  a.g_logits = q->g_logits;
+  a.g_spans = q->g_spans;
+  a.pred_logits = q->pred_logits;
+  a.pred_spans = q->pred_spans;
+  a.h_cls = reinterpret_cast<const uint16_t*>(q->h_cls);
+  a.h_span = reinterpret_cast<const uint16_t*>(q->h_span);
+  a.w_cls = q->w_cls;
+  a.w_span = q->w_span;
+  a.dz = q->dz;
+  a.dh_cls = reinterpret_cast<uint16_t*>(q->dh_cls);
+  a.dh_span = reinterpret_cast<uint16_t*>(q->dh_span);
+  a.gw_cls = q->gw_cls;
+  a.gb_cls = q->gb_cls;
+  a.gw_span = q->gw_span;
+  a.gb_span = q->gb_span;
+  a.cs_cls = q->cs_cls;
+  a.cs_span = q->cs_span;
+  a.in_scale = q->in_scale;
+  a.pgrad_scale = q->pgrad_scale;
+  a.B = q->B;
+  a.Lv = q->Lv;
+  a.d = q->d;
+  a.fmt_act = q->fmt_act;
+  a.fmt_grad = q->fmt_grad;
+  return launch_head_final_bwd(a, (cudaStream_t)stream);
+}
+
+// text-row copy arguments shared by the two column-sum operators
+static int txt_rows_arg(const char* fn, void* txt16, int L, int Lv, int txt_cols, int rows, int cols, int vec, TxtRows& t) {
+  t = TxtRows{nullptr, 0, 0, 0};
+  if (!txt16) return 0;
+  UV_REQ(L >= 1 && Lv >= 0 && Lv < L && rows % L == 0, "%s: text rows need 0 <= Lv < L and rows %% L == 0 (L %d, Lv %d, rows %d)", fn, L,
+         Lv, rows);
+  UV_REQ(txt_cols >= vec && txt_cols <= cols && txt_cols % vec == 0, "%s: txt_cols %d must be a multiple of %d in [%d, cols]", fn, txt_cols,
+         vec, vec);
+  UV_REQ(al_(txt16, 2 * vec), "%s: txt16 must be %d-byte aligned", fn, 2 * vec);
+  t = TxtRows{reinterpret_cast<uint16_t*>(txt16), L, Lv, txt_cols};
+  return 0;
+}
+
+int univtg_op_colsum16(const void* in16, int32_t ld, int32_t rows, int32_t cols, int32_t fmt, float* colsum, float scale, void* txt16,
+                       int32_t L, int32_t Lv, int32_t txt_cols, void* stream) {
+  const char* fn = "univtg_op_colsum16";
+  UV_REQ(in16 && colsum, "%s: null in16 or colsum", fn);
+  UV_REQ(rows >= 1 && cols >= 8 && cols % 8 == 0 && ld >= cols && ld % 8 == 0, "%s: rows %d / cols %d / ld %d (multiples of 8, ld >= cols)", fn,
+         rows, cols, ld);
+  UV_REQ(al_(in16, 16) && al_(colsum, 16), "%s: in16 and colsum must be 16-byte aligned", fn);
+  UV_REQ(fmt == 0 || fmt == 1, "%s: fmt %d", fn, fmt);
+  TxtRows t;
+  if (txt_rows_arg(fn, txt16, L, Lv, txt_cols, rows, cols, 8, t)) return 1;
+  return launch_colsum16(reinterpret_cast<const uint16_t*>(in16), ld, rows, cols, fmt, colsum, scale, (cudaStream_t)stream, t);
+}
+
+int univtg_op_cvt16_colsum(const float* in32, int32_t ld_in, void* out16, int32_t ld_out, int32_t rows, int32_t cols, int32_t fmt,
+                           float* colsum, float colsum_scale, void* txt16, int32_t L, int32_t Lv, int32_t txt_cols, void* stream) {
+  const char* fn = "univtg_op_cvt16_colsum";
+  UV_REQ(in32 && out16, "%s: null in32 or out16", fn);
+  UV_REQ(rows >= 1 && cols >= 4 && cols % 4 == 0 && ld_in >= cols && ld_in % 4 == 0 && ld_out >= cols && ld_out % 4 == 0,
+         "%s: rows %d / cols %d / ld_in %d / ld_out %d (multiples of 4, pitches >= cols)", fn, rows, cols, ld_in, ld_out);
+  UV_REQ(al_(in32, 16) && al_(out16, 8) && al_(colsum, 4), "%s: in32 must be 16-byte, out16 8-byte aligned", fn);
+  UV_REQ(fmt == 0 || fmt == 1, "%s: fmt %d", fn, fmt);
+  TxtRows t;
+  if (txt_rows_arg(fn, txt16, L, Lv, txt_cols, rows, cols, 4, t)) return 1;
+  return launch_cvt16_colsum(in32, ld_in, reinterpret_cast<uint16_t*>(out16), ld_out, rows, cols, fmt, colsum, colsum_scale,
+                             (cudaStream_t)stream, t);
+}
+
+int univtg_op_stream_gather(const float* dx, int32_t L, int32_t off, const float* extra, float extra_scale, void* out16, float* colsum,
+                            float colsum_scale, int32_t B, int32_t Ls, int32_t d, int32_t fmt, void* stream) {
+  const char* fn = "univtg_op_stream_gather";
+  UV_REQ(dx && out16, "%s: null dx or out16", fn);
+  UV_REQ(B >= 1 && Ls >= 1 && off >= 0 && off + Ls <= L, "%s: B %d / Ls %d / off %d / L %d (off + Ls <= L)", fn, B, Ls, off, L);
+  UV_REQ(d >= 4 && d % 4 == 0, "%s: d %d must be a positive multiple of 4", fn, d);
+  UV_REQ(al_(dx, 16) && al_(extra, 16) && al_(out16, 8) && al_(colsum, 4), "%s: dx / extra must be 16-byte, out16 8-byte aligned", fn);
+  UV_REQ(fmt == 0 || fmt == 1, "%s: fmt %d", fn, fmt);
+  return launch_stream_gather(dx, L, off, extra, extra_scale, reinterpret_cast<uint16_t*>(out16), colsum, colsum_scale, B, Ls, d, fmt,
+                              (cudaStream_t)stream);
+}
+
+int univtg_op_pool_bwd(const float* x_txt, const float* alpha, const float* w, const float* g_pooled, float* dx_txt, float* gw,
+                       float out_scale, int32_t B, int32_t Lt, int32_t d, void* stream) {
+  const char* fn = "univtg_op_pool_bwd";
+  UV_REQ(x_txt && alpha && w && g_pooled && dx_txt && gw, "%s: null pointer argument", fn);
+  UV_REQ(B >= 1 && d >= 1 && Lt >= 1 && (size_t)Lt * sizeof(float) <= 48 * 1024, "%s: B %d / Lt %d / d %d (Lt <= 12288)", fn, B, Lt, d);
+  UV_REQ(al_(x_txt, 4) && al_(alpha, 4) && al_(w, 4) && al_(g_pooled, 4) && al_(dx_txt, 4) && al_(gw, 4), "%s: misaligned pointer", fn);
+  PoolBwdArgs a;
+  a.x_txt = x_txt;
+  a.alpha = alpha;
+  a.w = w;
+  a.g_pooled = g_pooled;
+  a.dx_txt = dx_txt;
+  a.gw = gw;
+  a.out_scale = out_scale;
+  a.B = B;
+  a.Lt = Lt;
+  a.d = d;
+  return launch_pool_bwd(a, (cudaStream_t)stream);
+}
+
+int univtg_op_txt_pos_bwd(const univtg_txt_pos_bwd* q, const univtg_rng* rng, int32_t mask_index, void* stream) {
+  const char* fn = "univtg_op_txt_pos_bwd";
+  UV_REQ(q != nullptr, "%s: null args", fn);
+  UV_REQ(q->dpos && q->xt && q->table && q->gamma && q->mean && q->rstd && q->dx && q->dtable && q->dgamma && q->dbeta,
+         "%s: null pointer argument", fn);
+  UV_REQ(q->B >= 1 && q->Lt >= 1 && q->Lv >= 0 && q->Lv + q->Lt <= q->L, "%s: B %d / Lt %d / Lv %d / L %d (Lv + Lt <= L)", fn, q->B, q->Lt,
+         q->Lv, q->L);
+  UV_REQ(q->d >= 1 && q->d <= 1024, "%s: d %d (1..1024)", fn, q->d);
+  UV_REQ(!rng || !(rng->input_dropout > 0.f) || mask_index >= 0, "%s: mask_index %d", fn, mask_index);
+  TxtPosBwdArgs a;
+  memset(&a, 0, sizeof(a));
+  a.dpos = q->dpos;
+  a.xt = q->xt;
+  a.table = q->table;
+  a.gamma = q->gamma;
+  a.mean = q->mean;
+  a.rstd = q->rstd;
+  a.mul32 = q->mul32;
+  if (!a.mul32 && rng && rng->input_dropout > 0.f) a.drop = make_drop_spec(rng->seed, (unsigned int)mask_index, rng->input_dropout);
+  a.dx = q->dx;
+  a.dtable = q->dtable;
+  a.dgamma = q->dgamma;
+  a.dbeta = q->dbeta;
+  a.pgrad_scale = q->pgrad_scale;
+  a.B = q->B;
+  a.Lt = q->Lt;
+  a.L = q->L;
+  a.Lv = q->Lv;
+  a.d = q->d;
+  return launch_txt_pos_bwd(a, (cudaStream_t)stream);
+}
+#undef UV_REQ
 
 int univtg_dropout_mask(const univtg_rng* rng, int32_t mask_index, size_t rows, size_t cols, float* out, void* stream) {
   if (!rng || !out || mask_index < 0 || cols == 0) {
