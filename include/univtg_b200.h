@@ -35,7 +35,14 @@ typedef struct univtg_config {
   int32_t n_input_proj;     /* args.n_input_proj in {1,2,3}    */
   int32_t v_feat_dim;       /* args.v_feat_dim (already +2 TEF)*/
   int32_t t_feat_dim;       /* args.t_feat_dim                 */
-  int32_t operand_format;   /* 0 = fp16 MMA operands (default), 1 = bf16; accumulation/LN/softmax/heads are fp32 */
+  int32_t operand_format;   /* 0 = fp16 MMA operands (default), 1 = bf16; accumulation/LN/softmax/heads are fp32.
+                             * 2 = fp16x3 (inference only): every 16-bit buffer holds hi = fp16(v) and a lo plane fp16(v - hi),
+                             * and every product is A_hi B_hi + A_lo B_hi + A_hi B_lo.  The packed weights and the inference
+                             * workspace are then twice their format-0 size: the first half is the format-0 layout (hi planes),
+                             * and the lo plane of each 16-bit buffer lies exactly half the buffer size after its hi plane
+                             * (the fp32 entries of the second half are unused).  univtg_prepare_workspace zeroes the separator
+                             * rows of both planes.  univtg_forward_train, univtg_backward, univtg_train_workspace_bytes,
+                             * univtg_adamw_step and the backward-only univtg_op_* entry points refuse it. */
 } univtg_config;
 
 /* Problem shape of one batch (reference Model.forward arguments, model/univtg.py:105). */
@@ -213,6 +220,10 @@ int univtg_plan_read_profile(univtg_plan* plan, float* ms, int32_t* kinds, int32
 int univtg_op_gemm(const void* a, const void* b, int32_t M, int32_t N, int32_t K, int32_t a_mn, int32_t b_mn, int32_t fmt,
                    int32_t bn, int32_t ksplit, const float* bias, int32_t act, float alpha, float* out32, void* out16,
                    void* stream);
+/* fmt = 2 (fp16x3) for univtg_op_gemm, univtg_op_layernorm and univtg_op_attention: every 16-bit argument is a hi plane
+ * followed directly by its lo plane of the same shape (a: lo at a + M*K, b: b + N*K, out16: out16 + M*N; layernorm out16:
+ * out16 + rows*ld16; attention qkv: qkv + B*L*3d, out: out + B*L*d).  The GEMM needs a_mn = b_mn = 0, N % 16 == 0,
+ * 32-byte aligned outputs and lo planes, and no ksplit with out16. */
 /* Same GEMM launched as 2-CTA clusters: vertically adjacent tiles share a K-major B tile through TMA multicast (half the
  * L2 -> SM traffic of B).  bn multiple of 32; b_mn must be 0 (an MN-major B is rejected with an error). */
 int univtg_op_gemm_cluster(const void* a, const void* b, int32_t M, int32_t N, int32_t K, int32_t a_mn, int32_t b_mn,

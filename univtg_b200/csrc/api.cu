@@ -22,7 +22,7 @@ int univtg_num_params(const univtg_config* cfg) {
 
 size_t univtg_packed_bytes(const univtg_config* cfg) {
   if (!check_cfg(cfg)) return 0;
-  return make_layout(*cfg).total;
+  return planes(*cfg) * make_layout(*cfg).total;
 }
 
 // mode 0: everything; mode 1: only the fp32 vectors / small fp32 tensors (the 16-bit matrices are kept current by univtg_adamw_step)
@@ -42,7 +42,8 @@ static int pack_impl(const univtg_config* cfg, const float* const* params, int32
   const int d = cfg->hidden_dim, ff = cfg->dim_feedforward;
   Packer pk;
   pk.base = reinterpret_cast<uint8_t*>(packed);
-  pk.fmt = cfg->operand_format;
+  pk.fmt = kernel_fmt(*cfg);
+  pk.lo = is_split(*cfg) ? (long long)L.total : 0;
   pk.st = (cudaStream_t)stream;
   pk.tab.n = 0;
   pk.skip_matrices = mode == 1;
@@ -185,7 +186,7 @@ int univtg_adamw_step(float* params, float* grads, float* exp_avg, float* exp_av
   if (cfg == nullptr || packed == nullptr)
     return uv::adamw_step_impl(params, grads, exp_avg, exp_avg_sq, n, lr, beta1, beta2, eps, weight_decay, step, max_grad_norm,
                                write_clipped_grads, scratch3, nullptr, stream);
-  if (!check_cfg(cfg)) return 1;
+  if (!check_cfg(cfg) || refuse_split(*cfg, "univtg_adamw_step")) return 1;
   PackSegTable t;
   const int total = make_pack_segments(*cfg, packed, t);
   if (total < 0) return 1;
@@ -203,7 +204,7 @@ extern "C" {
 
 size_t univtg_workspace_bytes(const univtg_config* cfg, const univtg_shape* shape) {
   if (!check_cfg(cfg) || !check_shape(shape)) return 0;
-  return make_infer_ws(*cfg, *shape, make_layout(*cfg), nullptr).total;
+  return planes(*cfg) * make_infer_ws(*cfg, *shape, make_layout(*cfg), nullptr).total;
 }
 
 int univtg_plan_create(const univtg_config* cfg, const univtg_shape* shape, const void* packed, void* workspace,
@@ -242,20 +243,24 @@ int univtg_plan_create(const univtg_config* cfg, const univtg_shape* shape, cons
   P->Mv = P->B * P->Lv;
   P->Mt = P->B * P->Lt;
   P->Mh = P->B * (P->Lv + 1);
+  if (is_split(*cfg)) {
+    P->pk_lo = (long long)(P->lay.total / 2);
+    P->ws_lo = (long long)(make_infer_ws(*cfg, *shape, P->lay, nullptr).total / 2);
+  }
   if (univtg_prepare_workspace(cfg, shape, workspace, 0, stream) != 0) {  // zero rows of the conv-head buffers
     delete P;
     return 1;
   }
-  // per-launch tile widths: fill the SMs with as little wave quantisation as possible
-  const int sms = P->num_sms, M = P->M, Mh = P->Mh;
+  // per-launch tile widths: fill the SMs with as little wave quantisation as possible (fp16x3 walks every K three times)
+  const int sms = P->num_sms, M = P->M, Mh = P->Mh, kx = is_split(*cfg) ? 3 : 1;
   for (int i = 0; i < cfg->n_input_proj; ++i)
-    P->bn_proj[i] = tile_for(sms, 16, 1, MNK{P->Mv, d, P->lay.vid[i].kpad}, MNK{P->Mt, d, P->lay.txt[i].kpad}).bn;
-  P->bn_qkv = tile_for(sms, 16, 1, MNK{M, 2 * d, d}, MNK{M, d, d}).bn;
-  P->bn_out = tile_for(sms, 16, 1, MNK{M, d, d}).bn;
-  P->bn_ffn1 = tile_for(sms, 16, 1, MNK{M, ff, d}).bn;
-  P->bn_ffn2 = tile_for(sms, 16, 1, MNK{M, d, ff}).bn;
-  P->bn_conv1 = tile_for(sms, 16, 1, MNK{Mh, 2 * d, 3 * d}).bn;
-  P->bn_conv2 = tile_for(sms, 16, 1, MNK{Mh, d, 3 * d}, MNK{Mh, d, 3 * d}).bn;
+    P->bn_proj[i] = tile_for(sms, 16, 1, MNK{P->Mv, d, kx * P->lay.vid[i].kpad}, MNK{P->Mt, d, kx * P->lay.txt[i].kpad}).bn;
+  P->bn_qkv = tile_for(sms, 16, 1, MNK{M, 2 * d, kx * d}, MNK{M, d, kx * d}).bn;
+  P->bn_out = tile_for(sms, 16, 1, MNK{M, d, kx * d}).bn;
+  P->bn_ffn1 = tile_for(sms, 16, 1, MNK{M, ff, kx * d}).bn;
+  P->bn_ffn2 = tile_for(sms, 16, 1, MNK{M, d, kx * ff}).bn;
+  P->bn_conv1 = tile_for(sms, 16, 1, MNK{Mh, 2 * d, kx * 3 * d}).bn;
+  P->bn_conv2 = tile_for(sms, 16, 1, MNK{Mh, d, kx * 3 * d}, MNK{Mh, d, kx * 3 * d}).bn;
   P->launches = 1 + 3 * cfg->n_input_proj + 7 * cfg->enc_layers + 6;
   *out = P;
   return 0;
@@ -355,13 +360,18 @@ int run_forward(univtg_plan* P, const FwdBufs& W, const float* src_txt, const fl
   const uint8_t* pk = P->packed;
   auto W16 = [&](size_t off) { return reinterpret_cast<const uint16_t*>(pk + off); };
   auto F32 = [&](size_t off) { return reinterpret_cast<const float*>(pk + off); };
-  const int d = P->d, ff = P->ff, fmt = c.operand_format, M = P->M, L = P->L, Lv = P->Lv, Lt = P->Lt, sms = P->num_sms;
+  const int d = P->d, ff = P->ff, fmt = kernel_fmt(c), M = P->M, L = P->L, Lv = P->Lv, Lt = P->Lt, sms = P->num_sms;
+  // fp16x3: element offsets of the lo planes of the packed weights and of the workspace's 16-bit buffers (0: one plane)
+  const int split = is_split(c) ? 1 : 0;
+  const long long pk_lo = P->pk_lo, ws_lo = P->ws_lo;
   int rc = 0;
   GemmGroup g;
   auto group = [&](int num) {
     memset(&g, 0, sizeof(g));
     g.num = num;
     g.fmt = fmt;
+    g.split = split;
+    g.lo16 = ws_lo;
   };
   // every launch is followed by a profiling mark of its kind: 0 row kernel, 1 tensor-core GEMM, 2 attention
   auto marked = [&](int r, int kind) {
@@ -401,6 +411,8 @@ int run_forward(univtg_plan* P, const FwdBufs& W, const float* src_txt, const fl
       a.beta = F32(pp.ln_b);
       a.eps = 1e-5f;
       a.fmt = fmt;
+      a.split = split;
+      a.lo = ws_lo;
       a.out16 = s == 0 ? W.a_vid[i] : W.a_txt[i];
       a.ld16 = pp.kpad;
       a.mul32 = drop_masks ? drop_masks[s * c.n_input_proj + i] : nullptr;
@@ -415,8 +427,8 @@ int run_forward(univtg_plan* P, const FwdBufs& W, const float* src_txt, const fl
     const int bn = P->bn_proj[i];
     GemmProblem& pv = g.p[0];
     GemmProblem& pt = g.p[1];
-    rc |= setup_linear(pv, W.a_vid[i], P->Mv, Lw.vid[i].kpad, Lw.vid[i].kpad, W16(Lw.vid[i].w16), d, Lw.vid[i].kpad, bn);
-    rc |= setup_linear(pt, W.a_txt[i], P->Mt, Lw.txt[i].kpad, Lw.txt[i].kpad, W16(Lw.txt[i].w16), d, Lw.txt[i].kpad, bn);
+    rc |= setup_linear(pv, W.a_vid[i], P->Mv, Lw.vid[i].kpad, Lw.vid[i].kpad, W16(Lw.vid[i].w16), d, Lw.vid[i].kpad, bn, ws_lo, pk_lo);
+    rc |= setup_linear(pt, W.a_txt[i], P->Mt, Lw.txt[i].kpad, Lw.txt[i].kpad, W16(Lw.txt[i].w16), d, Lw.txt[i].kpad, bn, ws_lo, pk_lo);
     if (rc) return rc;
     pv.bias = F32(Lw.vid[i].bias);
     pt.bias = F32(Lw.txt[i].bias);
@@ -468,6 +480,8 @@ int run_forward(univtg_plan* P, const FwdBufs& W, const float* src_txt, const fl
     a.Lv = Lv;
     a.d = d;
     a.fmt = fmt;
+    a.split = split;
+    a.lo = ws_lo;
     rc = marked(launch_txt_pos(a, st), 0);
     if (rc) return rc;
   }
@@ -477,8 +491,8 @@ int run_forward(univtg_plan* P, const FwdBufs& W, const float* src_txt, const fl
     const LayerPacked& lp = Lw.layer[l];
     // q = k = x + pos -> columns [0, 2d) of qkv16; v = x -> columns [2d, 3d)   (in_proj rows: Wq, Wk, Wv)
     group(2);
-    rc |= setup_linear(g.p[0], W.xpos16[l], M, d, d, W16(lp.w_in), 2 * d, d, P->bn_qkv);
-    rc |= setup_linear(g.p[1], W.xin16[l], M, d, d, W16(lp.w_in) + (size_t)2 * d * d, d, d, P->bn_qkv);
+    rc |= setup_linear(g.p[0], W.xpos16[l], M, d, d, W16(lp.w_in), 2 * d, d, P->bn_qkv, ws_lo, pk_lo);
+    rc |= setup_linear(g.p[1], W.xin16[l], M, d, d, W16(lp.w_in) + (size_t)2 * d * d, d, d, P->bn_qkv, ws_lo, pk_lo);
     if (rc) return rc;
     g.p[0].bias = F32(lp.b_in);
     g.p[0].out16 = W.qkv16[l];
@@ -501,9 +515,11 @@ int run_forward(univtg_plan* P, const FwdBufs& W, const float* src_txt, const fl
       a.dh = P->dh;
       a.d = d;
       a.fmt = fmt;
+      a.split = split;
+      a.lo_qkv = a.lo_out = ws_lo;
       if (attn_rng) a.drop = make_drop_spec(rng->seed, (unsigned int)l, P->attn_dropout);
       if (P->dh == 64 || P->dh == 128) {
-        if (make_tmap_2d(&a.tm_qkv, W.qkv16[l], (uint64_t)M, (uint64_t)3 * d, (uint64_t)3 * d, 128, 64)) return 1;
+        if (make_tmap_op(&a.tm_qkv, W.qkv16[l], (uint64_t)M, (uint64_t)3 * d, (uint64_t)3 * d, 128, 64, ws_lo)) return 1;
         rc = launch_attention(a, st);
       } else {
         rc = launch_attention_simt(a, W.qkv16[l], st);
@@ -512,7 +528,7 @@ int run_forward(univtg_plan* P, const FwdBufs& W, const float* src_txt, const fl
       if (rc) return rc;
     }
     group(1);
-    rc = setup_linear(g.p[0], W.attn16[l], M, d, d, W16(lp.w_out), d, d, P->bn_out);
+    rc = setup_linear(g.p[0], W.attn16[l], M, d, d, W16(lp.w_out), d, d, P->bn_out, ws_lo, pk_lo);
     if (rc) return rc;
     g.p[0].bias = F32(lp.b_out);
     g.p[0].rps_in = L;
@@ -536,6 +552,8 @@ int run_forward(univtg_plan* P, const FwdBufs& W, const float* src_txt, const fl
       a.beta = F32(lp.n1b);
       a.eps = 1e-5f;
       a.fmt = fmt;
+      a.split = split;
+      a.lo = ws_lo;
       a.out32 = W.x1_32;
       a.out16 = W.x1_16[l];
       a.ld16 = d;
@@ -545,7 +563,7 @@ int run_forward(univtg_plan* P, const FwdBufs& W, const float* src_txt, const fl
       if (rc) return rc;
     }
     group(1);
-    rc = setup_linear(g.p[0], W.x1_16[l], M, d, d, W16(lp.w1), ff, d, P->bn_ffn1);
+    rc = setup_linear(g.p[0], W.x1_16[l], M, d, d, W16(lp.w1), ff, d, P->bn_ffn1, ws_lo, pk_lo);
     if (rc) return rc;
     g.p[0].bias = F32(lp.b1);
     g.p[0].act = ACT_GELU;
@@ -558,7 +576,7 @@ int run_forward(univtg_plan* P, const FwdBufs& W, const float* src_txt, const fl
     rc = marked(launch_gemm_group(g, P->bn_ffn1, sms, st), 1);
     if (rc) return rc;
     group(1);
-    rc = setup_linear(g.p[0], W.h16[l], M, ff, ff, W16(lp.w2), d, ff, P->bn_ffn2);
+    rc = setup_linear(g.p[0], W.h16[l], M, ff, ff, W16(lp.w2), d, ff, P->bn_ffn2, ws_lo, pk_lo);
     if (rc) return rc;
     g.p[0].bias = F32(lp.b2);
     g.p[0].rps_in = L;
@@ -582,6 +600,8 @@ int run_forward(univtg_plan* P, const FwdBufs& W, const float* src_txt, const fl
       a.beta = F32(lp.n2b);
       a.eps = 1e-5f;
       a.fmt = fmt;
+      a.split = split;
+      a.lo = ws_lo;
       a.L = L;
       a.Lv = Lv;
       a.out32 = W.x32;
@@ -610,8 +630,8 @@ int run_forward(univtg_plan* P, const FwdBufs& W, const float* src_txt, const fl
     p.ca = OperandCoord{0, 0, 0, 1, 0, 1, 1, 0};
     // W2 [N, 3d]: column tap*d + k
     p.cb = OperandCoord{0, 0, d, 1, 0, 1, 0, 0};
-    int r = make_tmap_2d(&p.tm_a, A, (uint64_t)P->Mh + 2, (uint64_t)d, (uint64_t)lda, GEMM_BM, 64);
-    r |= make_tmap_2d(&p.tm_b, Wc, (uint64_t)N, (uint64_t)3 * d, (uint64_t)3 * d, (uint32_t)bn, 64);
+    int r = make_tmap_op(&p.tm_a, A, (uint64_t)P->Mh + 2, (uint64_t)d, (uint64_t)lda, GEMM_BM, 64, ws_lo);
+    r |= make_tmap_op(&p.tm_b, Wc, (uint64_t)N, (uint64_t)3 * d, (uint64_t)3 * d, (uint32_t)bn, 64, pk_lo);
     p.b_box_rows = bn;
     p.bias = bias;
     p.act = ACT_RELU;
@@ -648,6 +668,8 @@ int run_forward(univtg_plan* P, const FwdBufs& W, const float* src_txt, const fl
     a.Lv = Lv;
     a.d = d;
     a.fmt = fmt;
+    a.split = split;
+    a.lo = ws_lo;
     rc = marked(launch_conv_head_final(a, st), 0);
     if (rc) return rc;
   }
@@ -704,11 +726,22 @@ static int op_gemm_impl(const void* a, const void* b, int32_t M, int32_t N, int3
     set_error("univtg_op_gemm_cluster: cluster launches need a K-major B operand (b_mn = 0)");
     return 1;
   }
+  const bool split = fmt == 2;
+  if (split && (a_mn || b_mn || cluster == 2)) {
+    set_error("univtg_op_gemm: fmt 2 (fp16x3) needs K-major A and B (a_mn = b_mn = 0) and no cluster");
+    return 1;
+  }
+  if (split && ksplit > 1 && out16) {
+    set_error("univtg_op_gemm: fmt 2 (fp16x3) out16 cannot be combined with ksplit > 1");
+    return 1;
+  }
   GemmGroup g;
   memset(&g, 0, sizeof(g));
   g.num = 1;
-  g.fmt = fmt;
+  g.fmt = split ? 0 : fmt;
   g.cluster = cluster;
+  g.split = split ? 1 : 0;
+  g.lo16 = split ? (long long)M * N : 0;
   GemmProblem& p = g.p[0];
   init_problem(p);
   p.M = M;
@@ -719,13 +752,14 @@ static int op_gemm_impl(const void* a, const void* b, int32_t M, int32_t N, int3
   p.ksplit = ksplit < 1 ? 1 : ksplit;
   int rc = 0;
   if (!a_mn) {
-    rc |= make_tmap_2d(&p.tm_a, a, (uint64_t)M, (uint64_t)K, (uint64_t)K, GEMM_BM, 64);
+    rc |= make_tmap_op(&p.tm_a, a, (uint64_t)M, (uint64_t)K, (uint64_t)K, GEMM_BM, 64, split ? (long long)M * K : 0);
   } else {
     rc |= make_tmap_2d(&p.tm_a, a, (uint64_t)K, (uint64_t)M, (uint64_t)M, 64, 64);
     p.ca = OperandCoord{0, 1, 0, 0, 0, 0, 0, 1};  // c0 = m0, c1 = k
   }
   if (!b_mn) {
-    rc |= make_tmap_2d(&p.tm_b, b, (uint64_t)N, (uint64_t)K, (uint64_t)K, (uint32_t)(cluster == 2 ? bn / 2 : bn), 64);
+    rc |= make_tmap_op(&p.tm_b, b, (uint64_t)N, (uint64_t)K, (uint64_t)K, (uint32_t)(cluster == 2 ? bn / 2 : bn), 64,
+                       split ? (long long)N * K : 0);
     p.b_box_rows = cluster == 2 ? bn / 2 : bn;
   } else {
     rc |= make_tmap_b_mn(p, b, (uint64_t)K, (uint64_t)N, (uint64_t)N, bn);
@@ -789,10 +823,12 @@ int univtg_op_layernorm(const float* in, int32_t rows, int32_t d, const float* g
   a.gamma = gamma;
   a.beta = beta;
   a.eps = eps;
-  a.fmt = fmt;
+  a.fmt = fmt == 2 ? 0 : fmt;
   a.out32 = out32;
   a.out16 = reinterpret_cast<uint16_t*>(out16);
   a.ld16 = out16 ? ld16 : d;
+  a.split = fmt == 2;
+  a.lo = fmt == 2 ? (long long)rows * a.ld16 : 0;
   return launch_layernorm(a, (cudaStream_t)stream);
 }
 
@@ -814,9 +850,14 @@ int univtg_op_attention(const void* qkv, const float* key_mask, void* out, float
   a.H = H;
   a.dh = dh;
   a.d = d;
-  a.fmt = fmt;
+  a.fmt = fmt == 2 ? 0 : fmt;
+  a.split = fmt == 2;
+  if (a.split) {
+    a.lo_qkv = (long long)B * L * 3 * d;
+    a.lo_out = (long long)B * L * d;
+  }
   if (impl == 1) return launch_attention_simt(a, reinterpret_cast<const uint16_t*>(qkv), (cudaStream_t)stream);
-  if (make_tmap_2d(&a.tm_qkv, qkv, (uint64_t)B * L, (uint64_t)3 * d, (uint64_t)3 * d, 128, 64)) return 1;
+  if (make_tmap_op(&a.tm_qkv, qkv, (uint64_t)B * L, (uint64_t)3 * d, (uint64_t)3 * d, 128, 64, a.lo_qkv)) return 1;
   return launch_attention(a, (cudaStream_t)stream);
 }
 

@@ -52,7 +52,7 @@ struct TileInfo {
 
 // CL = 1: `t` is this CTA's tile index.  CL = 2: `t` indexes a 256-row PAIR tile made of two vertically adjacent 128-row tiles
 // (m_blk = 2*pair + rank, same n_blk).  The odd tail tile of a problem is a phantom whose rows are all out of range.
-template <int CL>
+template <int CL, bool SPLIT>
 __device__ __forceinline__ bool decode_tile(const GemmGroup& g, int bn, int t, int rank, TileInfo& ti) {
   for (int p = 0; p < g.num; ++p) {
     const GemmProblem& pr = g.p[p];
@@ -66,7 +66,7 @@ __device__ __forceinline__ bool decode_tile(const GemmGroup& g, int bn, int t, i
       const int rest = t / tn;
       ti.m_blk = (rest % tm) * CL + rank;
       ti.split = rest / tm;
-      const int total_kb = pr.taps * pr.kblk_per_tap;
+      const int total_kb = pr.taps * pr.kblk_per_tap * (SPLIT ? 3 : 1);
       const int per = (total_kb + pr.ksplit - 1) / pr.ksplit;
       ti.kb0 = ti.split * per;
       ti.kb1 = min(total_kb, ti.kb0 + per);
@@ -165,8 +165,11 @@ __device__ __forceinline__ void ld16f(const float* p, float (&v)[16]) {
 // FULL = false drops the training-only epilogue options at compile time (pre-activation save, aux / mask multiplies, atomic and
 // strided fp32 stores, second fp32 output, column sums, scalar fallback); the host picks the variant per launch.
 // v: accumulator + bias of columns [n0, n0 + 16) of this thread's row.  n0 is warp-uniform (column sums use the whole warp).
-template <bool FULL>
-__device__ __forceinline__ void epi_step(const GemmProblem& pr, const EpiRow& r, float (&v)[16], int n0, int fmt, int lane) {
+// SPLIT: out16 / out16p are fp16x3 pairs; the lo plane of each lies `lo16` elements after the hi plane.  The split variant is
+// lean plus out32_id (the projector's vid_mem_proj output).
+template <bool FULL, bool SPLIT>
+__device__ __forceinline__ void epi_step(const GemmProblem& pr, const EpiRow& r, float (&v)[16], int n0, int fmt, int lane,
+                                         long long lo16) {
   const int pN = pr.N;
   const int act = pr.act;
   const int ofmt = pr.out_fmt < 0 ? fmt : pr.out_fmt;
@@ -261,7 +264,7 @@ __device__ __forceinline__ void epi_step(const GemmProblem& pr, const EpiRow& r,
           st_global_256f(r.o32_row + n0 + 8, v[8], v[9], v[10], v[11], v[12], v[13], v[14], v[15]);
         }
       }
-      if (FULL && r.o32i_row != nullptr) {
+      if ((FULL || SPLIT) && r.o32i_row != nullptr) {
         st_global_256f(r.o32i_row + n0, v[0], v[1], v[2], v[3], v[4], v[5], v[6], v[7]);
         st_global_256f(r.o32i_row + n0 + 8, v[8], v[9], v[10], v[11], v[12], v[13], v[14], v[15]);
       }
@@ -270,6 +273,11 @@ __device__ __forceinline__ void epi_step(const GemmProblem& pr, const EpiRow& r,
 #pragma unroll
         for (int q = 0; q < 8; ++q) w8[q] = cvt16x2(v[2 * q], v[2 * q + 1], ofmt);
         st_global_256(r.o16_row + n0, w8);
+        if constexpr (SPLIT) {
+#pragma unroll
+          for (int q = 0; q < 8; ++q) w8[q] = cvt16x2_lo(v[2 * q], v[2 * q + 1]);
+          st_global_256(r.o16_row + lo16 + n0, w8);
+        }
       }
       if (r.o16p_row != nullptr) {
         float p[16];
@@ -285,6 +293,11 @@ __device__ __forceinline__ void epi_step(const GemmProblem& pr, const EpiRow& r,
 #pragma unroll
         for (int q = 0; q < 8; ++q) w8[q] = cvt16x2(p[2 * q], p[2 * q + 1], ofmt);
         st_global_256(r.o16p_row + n0, w8);
+        if constexpr (SPLIT) {
+#pragma unroll
+          for (int q = 0; q < 8; ++q) w8[q] = cvt16x2_lo(p[2 * q], p[2 * q + 1]);
+          st_global_256(r.o16p_row + lo16 + n0, w8);
+        }
       }
     } else {
 #pragma unroll
@@ -310,8 +323,15 @@ __device__ __forceinline__ void epi_step(const GemmProblem& pr, const EpiRow& r,
           else *dst = x;
         }
         if (r.o32i_row != nullptr) r.o32i_row[n] = x;
-        if (r.o16_row != nullptr) r.o16_row[n] = cvt16(x, ofmt);
-        if (r.o16p_row != nullptr) r.o16p_row[n] = cvt16(x + (r.add_row ? r.add_row[n] : 0.f), ofmt);
+        if (r.o16_row != nullptr) {
+          r.o16_row[n] = cvt16(x, ofmt);
+          if constexpr (SPLIT) r.o16_row[lo16 + n] = cvt16_lo(x);
+        }
+        if (r.o16p_row != nullptr) {
+          const float xp = x + (r.add_row ? r.add_row[n] : 0.f);
+          r.o16p_row[n] = cvt16(xp, ofmt);
+          if constexpr (SPLIT) r.o16p_row[lo16 + n] = cvt16_lo(xp);
+        }
       } else {
         x = 0.f;
       }
@@ -324,7 +344,10 @@ __device__ __forceinline__ void epi_step(const GemmProblem& pr, const EpiRow& r,
   }
 }
 
-template <int CL, bool FULL>
+// SPLIT (fp16x3, CL = 1, K-major operands only): tm_a / tm_b are 3-D maps whose third coordinate selects the hi (0) or lo (1)
+// plane.  A problem walks its taps x kblk_per_tap k-blocks three times - (A hi, B hi), (A lo, B hi), (A hi, B lo) - into the
+// same accumulators; only the producer knows about the planes.
+template <int CL, bool FULL, bool SPLIT = false>
 __global__ void __launch_bounds__(kGemmThreads, 1) gemm_wgmma_kernel(const __grid_constant__ GemmGroup g) {
   using Cfg = GemmCfg<CL>;
   const int BN = g.bn;
@@ -377,13 +400,21 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_wgmma_kernel(const __gri
       int stage = 0;
       uint32_t phase = 0;
       TileInfo ti;
-      for (int t = tile0; decode_tile<CL>(g, BN, t, crank, ti); t += tstep) {
+      for (int t = tile0; decode_tile<CL, SPLIT>(g, BN, t, crank, ti); t += tstep) {
         const GemmProblem& pr = g.p[ti.p];
         const int m0 = ti.m_blk * GEMM_BM;
         const int n0 = ti.n_blk * BN;
         for (int kb = ti.kb0; kb < ti.kb1; ++kb) {
-          const int tap = kb / pr.kblk_per_tap;
-          const int kk = (kb - tap * pr.kblk_per_tap) * GEMM_BK;
+          int kbt = kb, plane_a = 0, plane_b = 0;
+          if constexpr (SPLIT) {
+            const int per_product = pr.taps * pr.kblk_per_tap;
+            const int prod = kb / per_product;  // 0: hi x hi, 1: lo x hi, 2: hi x lo
+            kbt = kb - prod * per_product;
+            plane_a = prod == 1;
+            plane_b = prod == 2;
+          }
+          const int tap = kbt / pr.kblk_per_tap;
+          const int kk = (kbt - tap * pr.kblk_per_tap) * GEMM_BK;
           mbar_wait(&empty_bar[stage], phase ^ 1);
           uint8_t* sa = stage_base + stage * kStageBytes;
           uint8_t* sb = sa + Cfg::kABytes;
@@ -393,13 +424,17 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_wgmma_kernel(const __gri
           const int b1 = pr.cb.base1 + n0 * pr.cb.mn1s + tap * pr.cb.tap1 + kk * pr.cb.k1s;
           if (elect_one()) {
             mbar_arrive_expect_tx(&full_bar[stage], Cfg::kABytes + BN * 128);
-            if (!pr.a_mn) {
+            if constexpr (SPLIT) {
+              tma_load_3d(sa, &pr.tm_a, &full_bar[stage], a0, a1, plane_a);
+              tma_load_3d(sb, &pr.tm_b, &full_bar[stage], b0, b1, plane_b);
+            } else if (!pr.a_mn) {
               tma_load_2d(sa, &pr.tm_a, &full_bar[stage], a0, a1);
             } else {
 #pragma unroll
               for (int j = 0; j < GEMM_BM / 64; ++j) tma_load_2d(sa + j * 8192, &pr.tm_a, &full_bar[stage], a0 + 64 * j, a1);
             }
-            if (CL == 1) {
+            if constexpr (SPLIT) {
+            } else if (CL == 1) {
               if (!pr.b_mn) {
                 tma_load_2d(sb, &pr.tm_b, &full_bar[stage], b0, b1);
               } else if (pr.b_3d) {
@@ -444,7 +479,7 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_wgmma_kernel(const __gri
       }
     };
     bool first_tile = true;
-    for (int t = tile0; decode_tile<CL>(g, BN, t, crank, ti); t += tstep) {
+    for (int t = tile0; decode_tile<CL, SPLIT>(g, BN, t, crank, ti); t += tstep) {
       const GemmProblem& pr = g.p[ti.p];
       const int bf = pr.a_fmt < 0 ? fmt : pr.a_fmt;  // both operands share it (checked on the host)
       // descriptor = constant high part (layout, LBO/SBO) + start address; one k-step of 16 elements advances the address by
@@ -498,7 +533,7 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_wgmma_kernel(const __gri
       r.mask_row = (FULL && pr.mask16) ? pr.mask16 + orow * pr.ld_mask : nullptr;
       r.add_row = pr.addtab ? pr.addtab + (size_t)m * pr.ld_addtab : nullptr;
       r.o32_row = pr.out32 ? pr.out32 + orow * pr.ld32 : nullptr;
-      r.o32i_row = (FULL && pr.out32_id) ? pr.out32_id + (size_t)m * pr.ld32_id : nullptr;
+      r.o32i_row = ((FULL || SPLIT) && pr.out32_id) ? pr.out32_id + (size_t)m * pr.ld32_id : nullptr;
       r.o16_row = pr.out16 ? pr.out16 + orow * pr.ld16 : nullptr;
       r.o16p_row = pr.out16p ? pr.out16p + orow * pr.ld16 : nullptr;
       r.pre_row = (FULL && pr.pre32) ? pr.pre32 + orow * pr.ld_pre : nullptr;
@@ -523,7 +558,7 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_wgmma_kernel(const __gri
 #pragma unroll
               for (int j = 0; j < 16; ++j) v[j] += (n0 + j < pN) ? __ldg(bias + n0 + j) : 0.f;
             }
-            epi_step<FULL>(pr, r, v, n0, fmt, lane);
+            epi_step<FULL, SPLIT>(pr, r, v, n0, fmt, lane, g.lo16);
           }
           named_bar_sync(1 + cw, 128);
         }
@@ -591,8 +626,10 @@ struct TmapKey {
   const void* base;
   uint64_t rows, cols, ld;
   uint32_t box_rows, box_cols, kind;
+  uint64_t plane;  // kind 4 (fp16x3 pair): element offset of the lo plane
   bool operator==(const TmapKey& o) const {
-    return base == o.base && rows == o.rows && cols == o.cols && ld == o.ld && box_rows == o.box_rows && box_cols == o.box_cols && kind == o.kind;
+    return base == o.base && rows == o.rows && cols == o.cols && ld == o.ld && box_rows == o.box_rows && box_cols == o.box_cols && kind == o.kind &&
+           plane == o.plane;
   }
 };
 struct TmapSlot {
@@ -606,13 +643,14 @@ static inline TmapSlot* tmap_slot(const TmapKey& k) {
   if (g_tmap_cache == nullptr) g_tmap_cache = static_cast<TmapSlot*>(calloc(kTmapCacheSlots, sizeof(TmapSlot)));
   uint64_t h = reinterpret_cast<uintptr_t>(k.base) * 0x9E3779B97F4A7C15ull;
   h ^= (k.rows * 0xC2B2AE3D27D4EB4Full) ^ (k.cols << 17) ^ (k.ld << 29) ^ ((uint64_t)k.box_rows << 41) ^ ((uint64_t)k.box_cols << 47) ^ ((uint64_t)k.kind << 55);
+  h ^= k.plane * 0x94D049BB133111EBull;
   h ^= h >> 29;
   return g_tmap_cache ? &g_tmap_cache[h & (kTmapCacheSlots - 1)] : nullptr;
 }
 
 int make_tmap_2d(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols, uint64_t ld_elems, uint32_t box_rows,
                  uint32_t box_cols) {
-  const TmapKey key{base, rows, cols, ld_elems, box_rows, box_cols, 2u};
+  const TmapKey key{base, rows, cols, ld_elems, box_rows, box_cols, 2u, 0};
   TmapSlot* slot = tmap_slot(key);
   if (slot != nullptr && slot->used && slot->key == key) {
     *out = slot->map;
@@ -650,10 +688,46 @@ int make_tmap_2d_uncached(CUtensorMap* out, const void* base, uint64_t rows, uin
   return 0;
 }
 
+int make_tmap_split(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols, uint64_t ld_elems, uint32_t box_rows,
+                    uint32_t box_cols, uint64_t lo_elems) {
+  const TmapKey key{base, rows, cols, ld_elems, box_rows, box_cols, 4u, lo_elems};
+  TmapSlot* slot = tmap_slot(key);
+  if (slot != nullptr && slot->used && slot->key == key) {
+    *out = slot->map;
+    return 0;
+  }
+  EncodeTiledFn fn = get_encode_fn();
+  if (!fn) return 1;
+  if ((reinterpret_cast<uintptr_t>(base) & 15) != 0 || (ld_elems * 2) % 16 != 0 || (lo_elems * 2) % 16 != 0) {
+    set_error("tensor map: base %p / pitch %llu B / lo-plane offset %llu B not 16-byte aligned", base, (unsigned long long)(ld_elems * 2),
+              (unsigned long long)(lo_elems * 2));
+    return 2;
+  }
+  cuuint64_t dims[3] = {cols, rows, 2};
+  cuuint64_t strides[2] = {ld_elems * 2, lo_elems * 2};
+  cuuint32_t box[3] = {box_cols, box_rows, 1};
+  cuuint32_t estr[3] = {1, 1, 1};
+  CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_UINT16, 3, const_cast<void*>(base), dims, strides, box, estr,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) {
+    set_error("cuTensorMapEncodeTiled (fp16x3 pair) failed: CUresult %d (rows %llu cols %llu ld %llu lo %llu box %ux%u)", (int)r,
+              (unsigned long long)rows, (unsigned long long)cols, (unsigned long long)ld_elems, (unsigned long long)lo_elems, box_rows,
+              box_cols);
+    return 3;
+  }
+  if (slot != nullptr) {
+    slot->key = key;
+    slot->map = *out;
+    slot->used = true;
+  }
+  return 0;
+}
+
 int make_tmap_b_mn(GemmProblem& p, const void* base, uint64_t rows, uint64_t cols, uint64_t ld_elems, int bn, bool allow_3d) {
   p.b_3d = 0;
   if (!allow_3d || cols % 64 != 0 || bn % 64 != 0 || bn < 64) return make_tmap_2d(&p.tm_b, base, rows, cols, ld_elems, 64, 64);
-  const TmapKey key{base, rows, cols, ld_elems, (uint32_t)bn, 64u, 3u};
+  const TmapKey key{base, rows, cols, ld_elems, (uint32_t)bn, 64u, 3u, 0};
   TmapSlot* slot = tmap_slot(key);
   if (slot != nullptr && slot->used && slot->key == key) {
     p.tm_b = slot->map;
@@ -708,6 +782,8 @@ int launch_gemm_group(GemmGroup& g, int bn, int num_sms, cudaStream_t stream, in
       e = cudaFuncSetAttribute(gemm_wgmma_kernel<2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes);
     if (e == cudaSuccess)
       e = cudaFuncSetAttribute(gemm_wgmma_kernel<2, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes);
+    if (e == cudaSuccess)
+      e = cudaFuncSetAttribute(gemm_wgmma_kernel<1, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes);
     if (e != cudaSuccess) {
       set_error("cudaFuncSetAttribute(gemm, smem=%d): %s", Cfg::kSmemBytes, cudaGetErrorString(e));
       return (int)e;
@@ -718,10 +794,18 @@ int launch_gemm_group(GemmGroup& g, int bn, int num_sms, cudaStream_t stream, in
     set_error("cluster GEMM needs BN %% 32 == 0 (got %d)", bn);
     return (int)cudaErrorInvalidValue;
   }
+  if (g.split && (cl != 1 || g.fmt != 0)) {
+    set_error("fp16x3 gemm group: needs cluster 1 and group format 0 (got cluster %d, fmt %d)", cl, g.fmt);
+    return (int)cudaErrorInvalidValue;
+  }
   int total = 0;
   for (int p = 0; p < g.num; ++p) {
     const GemmProblem& pr = g.p[p];
-    if (pr.ksplit < 1 || pr.taps < 1 || pr.kblk_per_tap < 1 || pr.ksplit > pr.taps * pr.kblk_per_tap) {
+    if (g.split && (pr.a_mn || pr.b_mn || pr.a_fmt > 0 || pr.b_fmt > 0 || pr.out_fmt > 0)) {
+      set_error("gemm problem %d: fp16x3 problems need K-major fp16 operands and output", p);
+      return (int)cudaErrorInvalidValue;
+    }
+    if (pr.ksplit < 1 || pr.taps < 1 || pr.kblk_per_tap < 1 || pr.ksplit > pr.taps * pr.kblk_per_tap * (g.split ? 3 : 1)) {
       set_error("gemm problem %d: bad k configuration (taps %d kblk %d ksplit %d)", p, pr.taps, pr.kblk_per_tap, pr.ksplit);
       return (int)cudaErrorInvalidValue;
     }
@@ -757,7 +841,7 @@ int launch_gemm_group(GemmGroup& g, int bn, int num_sms, cudaStream_t stream, in
       set_error("gemm problem %d: A and B must share one 16-bit format (wgmma), got %d and %d", p, fa, fb);
       return (int)cudaErrorInvalidValue;
     }
-    const int total_kb = pr.taps * pr.kblk_per_tap;
+    const int total_kb = pr.taps * pr.kblk_per_tap * (g.split ? 3 : 1);
     const int per = (total_kb + pr.ksplit - 1) / pr.ksplit;
     if ((pr.ksplit - 1) * per >= total_kb) {
       set_error("gemm problem %d: ksplit %d leaves an empty split for %d k-blocks", p, pr.ksplit, total_kb);
@@ -771,19 +855,24 @@ int launch_gemm_group(GemmGroup& g, int bn, int num_sms, cudaStream_t stream, in
                (!pr.pre32 || (al16(pr.pre32) && pr.ld_pre % 4 == 0)) && (!pr.dact16 || (al16(pr.dact16) && pr.ld_dact % 8 == 0)) && (!pr.mask16 || (al16(pr.mask16) && pr.ld_mask % 8 == 0)) &&
                (!pr.resid || (al16(pr.resid) && pr.ld_resid % 4 == 0)) && (!pr.addtab || (al16(pr.addtab) && pr.ld_addtab % 4 == 0)) &&
                (!pr.out32 || (al16(pr.out32) && pr.ld32 % 4 == 0)) && (!pr.out32_id || (al16(pr.out32_id) && pr.ld32_id % 4 == 0)) &&
-               ((!pr.out16 && !pr.out16p) || (pr.ld16 % 8 == 0 && al16(pr.out16) && al16(pr.out16p)));
+               ((!pr.out16 && !pr.out16p) || (pr.ld16 % 8 == 0 && al16(pr.out16) && al16(pr.out16p) && g.lo16 % 8 == 0));
     auto al32 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 31) == 0; };
     // 256-bit accesses (one whole 32-byte sector per thread and instruction) when every leading dimension keeps rows 32-byte aligned
     if (w.vec_ok && (!pr.pre32 || (al32(pr.pre32) && pr.ld_pre % 8 == 0)) && (!pr.dact16 || (al32(pr.dact16) && pr.ld_dact % 16 == 0)) && (!pr.aux32 || (al32(pr.aux32) && pr.ld_aux % 8 == 0)) && (!pr.addtab || (al32(pr.addtab) && pr.ld_addtab % 8 == 0)) && (!pr.resid || (al32(pr.resid) && pr.ld_resid % 8 == 0)) &&
         (!pr.out32 || (al32(pr.out32) && pr.ld32 % 8 == 0)) && (!pr.out32_id || (al32(pr.out32_id) && pr.ld32_id % 8 == 0)) &&
-        ((!pr.out16 && !pr.out16p) || (pr.ld16 % 16 == 0 && al32(pr.out16) && al32(pr.out16p))))
+        ((!pr.out16 && !pr.out16p) || (pr.ld16 % 16 == 0 && al32(pr.out16) && al32(pr.out16p) && g.lo16 % 16 == 0)))
       w.vec_ok = 2;
   }
   if (total == 0) return 0;
   bool full = false;  // does any problem of the group need an epilogue option only the FULL variant compiles in?
   for (int p = 0; p < g.num; ++p) {
     const GemmProblem& pr = g.p[p];
-    full = full || pr.vec_ok != 2 || pr.pre32 || pr.dact16 || pr.aux32 || pr.mask16 || pr.accumulate || pr.ksplit > 1 || pr.out32_id || pr.colsum || pr.cs32 > 1;
+    full = full || pr.vec_ok != 2 || pr.pre32 || pr.dact16 || pr.aux32 || pr.mask16 || pr.accumulate || pr.ksplit > 1 ||
+           (pr.out32_id && !g.split) || pr.colsum || pr.cs32 > 1;  // the split lean variant also stores out32_id
+  }
+  if (g.split && full) {  // inference products only: the lean epilogue (the FULL one would spill with the split producer)
+    set_error("fp16x3 gemm group: needs the lean epilogue (N %% 16 == 0, 32-byte aligned outputs and lo planes, no training options or split-K)");
+    return (int)cudaErrorInvalidValue;
   }
   if (used_full) *used_full = full ? 1 : 0;
   g.bn = bn;
@@ -791,8 +880,13 @@ int launch_gemm_group(GemmGroup& g, int bn, int num_sms, cudaStream_t stream, in
   cudaError_t e;
   if (cl == 1) {
     const int grid = total < num_sms ? total : num_sms;
-    if (full) launch_k(gemm_wgmma_kernel<1, true>, dim3(grid), dim3(kGemmThreads), Cfg::kSmemBytes, stream, g);
-    else launch_k(gemm_wgmma_kernel<1, false>, dim3(grid), dim3(kGemmThreads), Cfg::kSmemBytes, stream, g);
+    if (g.split) {
+      launch_k(gemm_wgmma_kernel<1, false, true>, dim3(grid), dim3(kGemmThreads), Cfg::kSmemBytes, stream, g);
+    } else if (full) {
+      launch_k(gemm_wgmma_kernel<1, true>, dim3(grid), dim3(kGemmThreads), Cfg::kSmemBytes, stream, g);
+    } else {
+      launch_k(gemm_wgmma_kernel<1, false>, dim3(grid), dim3(kGemmThreads), Cfg::kSmemBytes, stream, g);
+    }
     e = cudaGetLastError();
   } else {
     const int max_clusters = num_sms / 2;

@@ -86,6 +86,9 @@ struct GemmGroup {
   int fmt;  // 0 fp16, 1 bf16
   int bn;   // tile width of this launch (set by launch_gemm_group)
   int cluster;  // 2: CTA pairs share the B tile through TMA multicast (K-major B maps must then use box rows = bn/2)
+  int split;    // 1: fp16x3 (fmt 0, cluster 1, K-major operands): tm_a / tm_b are make_tmap_split pairs, every product is
+                //    A_hi B_hi + A_lo B_hi + A_hi B_lo, and out16 / out16p are stored as hi / lo pairs
+  long long lo16;  // split: elements from out16 / out16p to their lo planes
   unsigned long long* dbg;  // optional [gridDim.x][8] %globaltimer stamps per CTA (profiling aid), normally null
   GemmProblem p[GEMM_MAX_GROUP];
 };
@@ -106,6 +109,10 @@ int make_tmap_b_mn(GemmProblem& p, const void* base, uint64_t rows, uint64_t col
 // box {box_cols, box_rows}, 128-byte swizzle, zero fill out of bounds.  Returns 0 on success.
 int make_tmap_2d(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols, uint64_t ld_elems, uint32_t box_rows,
                  uint32_t box_cols);
+
+// fp16x3 pair: a 3-D map {cols, rows, 2} over a hi plane and the lo plane `lo_elems` elements after it (same rows, cols, pitch).
+int make_tmap_split(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols, uint64_t ld_elems, uint32_t box_rows,
+                    uint32_t box_cols, uint64_t lo_elems);
 
 void set_gemm_timeline_buffer(unsigned long long* buf);  // debugging: stamps for every following GEMM launch
 const char* last_error();

@@ -85,10 +85,28 @@ bool check_cfg(const univtg_config* c) {
     set_error("feature dims must be positive");
     return false;
   }
-  if (c->operand_format != 0 && c->operand_format != 1) {
-    set_error("operand_format %d must be 0 (fp16) or 1 (bf16)", c->operand_format);
+  if (c->operand_format < 0 || c->operand_format > 2) {
+    set_error("operand_format %d must be 0 (fp16), 1 (bf16) or 2 (fp16x3)", c->operand_format);
     return false;
   }
+  return true;
+}
+
+// fp16x3 (operand_format 2) stores every 16-bit buffer as a hi plane (fp16) and a lo plane; the kernels then run with 16-bit
+// format 0 and their split flag.  The lo planes of a buffer set (the packed weights, the inference workspace) form a second copy
+// of that set's layout, placed right after it: the lo plane of a 16-bit buffer lies `total` bytes after its hi plane.
+inline bool is_split(const univtg_config& c) { return c.operand_format == 2; }
+inline int kernel_fmt(const univtg_config& c) { return is_split(c) ? 0 : c.operand_format; }
+inline size_t planes(const univtg_config& c) { return is_split(c) ? 2 : 1; }
+// Training keeps one 16-bit format per plan (gradients, AdamW repack); fp16x3 is an inference mode.
+inline bool refuse_split(const univtg_config& c, const char* fn) {
+  if (!is_split(c)) return false;
+  set_error("%s: operand_format 2 (fp16x3) is an inference mode; training needs fp16 or bf16", fn);
+  return true;
+}
+inline bool refuse_fmt2(int fmt, const char* fn) {
+  if (fmt != 2) return false;
+  set_error("%s: format 2 (fp16x3) is an inference mode; the backward operators take fp16 (0) or bf16 (1)", fn);
   return true;
 }
 
@@ -157,6 +175,7 @@ constexpr int kPackTasksPerLaunch = 64;
 constexpr int kPackItemsPerBlock = 256 * 8;  // work items per block (an item = 4 output elements, or one conv (n, c) pair)
 struct PackTable {
   int n, fmt;
+  long long lo;  // fp16x3: bytes from a 16-bit destination to its lo plane (0: one plane)
   PackTask t[kPackTasksPerLaunch];
 };
 
@@ -166,6 +185,7 @@ inline size_t pack_task_items(const PackTask& k) {
   return ((size_t)k.rows + 3) / 4;
 }
 
+template <bool SPLIT = false>  // SPLIT: fp16x3, the 16-bit kinds also write their lo planes (tab.lo)
 __global__ void __launch_bounds__(256) pack_multi_kernel(const __grid_constant__ PackTable tab) {
   pdl_prologue();
   int ti = 0;
@@ -193,6 +213,7 @@ __global__ void __launch_bounds__(256) pack_multi_kernel(const __grid_constant__
         v.w = c + 3 < k.cols ? __ldg(row + c + 3) : 0.f;
       }
       dst2[it] = make_uint2(cvt16x2(v.x, v.y, fmt), cvt16x2(v.z, v.w, fmt));
+      if constexpr (SPLIT) reinterpret_cast<uint2*>(reinterpret_cast<uint8_t*>(k.dst) + tab.lo)[it] = make_uint2(cvt16x2_lo(v.x, v.y), cvt16x2_lo(v.z, v.w));
     }
   } else if (k.kind == 1 || k.kind == 2) {
     // item = one (n, c) pair: three consecutive source floats (taps), scattered to the three tap planes of row n
@@ -211,6 +232,12 @@ __global__ void __launch_bounds__(256) pack_multi_kernel(const __grid_constant__
         d16[o] = cvt16(v0, fmt);
         d16[o + C] = cvt16(v1, fmt);
         d16[o + 2 * C] = cvt16(v2, fmt);
+        if constexpr (SPLIT) {
+          uint16_t* l16 = reinterpret_cast<uint16_t*>(reinterpret_cast<uint8_t*>(k.dst) + tab.lo);
+          l16[o] = cvt16_lo(v0);
+          l16[o + C] = cvt16_lo(v1);
+          l16[o + 2 * C] = cvt16_lo(v2);
+        }
       } else {
         float* d32 = reinterpret_cast<float*>(k.dst);
         d32[o] = v0;
@@ -231,6 +258,7 @@ __global__ void __launch_bounds__(256) pack_multi_kernel(const __grid_constant__
 struct Packer {
   uint8_t* base;
   int fmt;
+  long long lo;  // fp16x3: bytes to the lo planes
   cudaStream_t st;
   PackTable tab;
   bool skip_matrices = false;  // only the fp32 vectors / small tensors (kinds 2, 3)
@@ -242,12 +270,16 @@ struct Packer {
   void flush() {
     if (tab.n == 0) return;
     tab.fmt = fmt;
+    tab.lo = lo;
     int blocks = 0;
     for (int i = 0; i < tab.n; ++i) {
       tab.t[i].blk0 = blocks;
       blocks += (int)((pack_task_items(tab.t[i]) + kPackItemsPerBlock - 1) / kPackItemsPerBlock);
     }
-    if (blocks > 0) launch_k(pack_multi_kernel, dim3(blocks), dim3(256), 0, st, tab);
+    if (blocks > 0) {
+      if (lo) launch_k(pack_multi_kernel<true>, dim3(blocks), dim3(256), 0, st, tab);
+      else launch_k(pack_multi_kernel<false>, dim3(blocks), dim3(256), 0, st, tab);
+    }
     tab.n = 0;
   }
   void rows(const float* src, size_t off, int rows_, int cols, int ld) { push(PackTask{src, nullptr, base + off, 0, rows_, cols, ld, 0}); }
@@ -298,6 +330,7 @@ struct univtg_plan {
   int num_sms_bwd;  // SM budget of the backward's GEMM launches (0: num_sms); see univtg_plan_set_backward_sm_budget
   float attn_dropout;  // p of the attention dropout of univtg_forward_train / univtg_backward (0: off); univtg_forward ignores it
   int txt_pos_on;           // learned text positions (univtg_plan_set_txt_pos); 0: off
+  long long pk_lo, ws_lo;   // fp16x3: elements from a 16-bit weight / workspace buffer to its lo plane (0: one plane)
   univtg_txt_pos txt_pos;
   int B, Lv, Lt, L, d, ff, H, dh, M, Mv, Mt, Mh;
   int bn_proj[3];  // tile widths of the forward's GEMM launches (tile_for)
@@ -360,9 +393,21 @@ struct Mat16 {  // row-major 16-bit matrix view
   int rows, cols, ld;
 };
 
+// Operand map of a K-major 16-bit matrix: a plain 2-D map, or with lo > 0 (fp16x3) a hi / lo pair `lo` elements apart.
+inline int make_tmap_op(CUtensorMap* m, const void* base, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_rows, uint32_t box_cols,
+                        long long lo) {
+  return lo ? make_tmap_split(m, base, rows, cols, ld, box_rows, box_cols, (uint64_t)lo) : make_tmap_2d(m, base, rows, cols, ld, box_rows, box_cols);
+}
+
 // C[M,N] = sum_k A(m,k) B(n,k).  a_mn: A is stored [K rows, M cols] (else [M rows, K cols]); same for B.
-int setup_gemm(GemmProblem& p, Mat16 A, int a_mn, Mat16 B, int b_mn, int M, int N, int K, int bn) {
+// lo_a / lo_b > 0: fp16x3 operands (K-major only) whose lo planes lie that many elements after A / B.
+int setup_gemm(GemmProblem& p, Mat16 A, int a_mn, Mat16 B, int b_mn, int M, int N, int K, int bn, long long lo_a = 0,
+               long long lo_b = 0) {
   init_problem(p);
+  if ((lo_a || lo_b) && (a_mn || b_mn || !lo_a || !lo_b)) {
+    set_error("fp16x3 GEMM operands must both be split and K-major");
+    return 1;
+  }
   p.M = M;
   p.N = N;
   p.a_mn = a_mn;
@@ -370,13 +415,13 @@ int setup_gemm(GemmProblem& p, Mat16 A, int a_mn, Mat16 B, int b_mn, int M, int 
   p.kblk_per_tap = (K + 63) / 64;
   int rc = 0;
   if (!a_mn) {
-    rc |= make_tmap_2d(&p.tm_a, A.p, (uint64_t)A.rows, (uint64_t)A.cols, (uint64_t)A.ld, GEMM_BM, 64);
+    rc |= make_tmap_op(&p.tm_a, A.p, (uint64_t)A.rows, (uint64_t)A.cols, (uint64_t)A.ld, GEMM_BM, 64, lo_a);
   } else {
     rc |= make_tmap_2d(&p.tm_a, A.p, (uint64_t)A.rows, (uint64_t)A.cols, (uint64_t)A.ld, 64, 64);
     p.ca = OperandCoord{0, 1, 0, 0, 0, 0, 0, 1};
   }
   if (!b_mn) {
-    rc |= make_tmap_2d(&p.tm_b, B.p, (uint64_t)B.rows, (uint64_t)B.cols, (uint64_t)B.ld, (uint32_t)bn, 64);
+    rc |= make_tmap_op(&p.tm_b, B.p, (uint64_t)B.rows, (uint64_t)B.cols, (uint64_t)B.ld, (uint32_t)bn, 64, lo_b);
     p.b_box_rows = bn;
   } else {
     rc |= make_tmap_b_mn(p, B.p, (uint64_t)B.rows, (uint64_t)B.cols, (uint64_t)B.ld, bn);
@@ -425,8 +470,9 @@ int conv_wgrad_problem(GemmProblem& p, int Mh, const uint16_t* dY, int ldy, int 
 }
 
 // K-major linear problem: A [M, K] (pitch lda), W [N, K] (pitch ldw).
-inline int setup_linear(GemmProblem& p, const uint16_t* A, int M, int K, int lda, const uint16_t* W, int N, int ldw, int bn) {
-  return setup_gemm(p, Mat16{A, M, K, lda}, 0, Mat16{W, N, K, ldw}, 0, M, N, K, bn);
+inline int setup_linear(GemmProblem& p, const uint16_t* A, int M, int K, int lda, const uint16_t* W, int N, int ldw, int bn,
+                        long long lo_a = 0, long long lo_w = 0) {
+  return setup_gemm(p, Mat16{A, M, K, lda}, 0, Mat16{W, N, K, ldw}, 0, M, N, K, bn, lo_a, lo_w);
 }
 
 // Tile width + split-K factor for one grouped launch (cost model: choose_tile, gemm.cu).  K in elements; step 16 when every B

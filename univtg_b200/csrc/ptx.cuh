@@ -274,5 +274,10 @@ UV_DEVINL uint32_t cvt16x2(float lo, float hi, int fmt) {
 UV_DEVINL float ld16(uint16_t v, int fmt) {
   return fmt ? __bfloat162float(__ushort_as_bfloat16(v)) : __half2float(__ushort_as_half(v));
 }
+// Split fp16 ("fp16x3", operand_format 2): a value v is stored as two fp16 planes, hi = fp16(v) (cvt16 with fmt 0) and
+// lo = fp16(v - hi).  v - hi is exact in fp32, and hi + lo is exact in fp32 again.
+UV_DEVINL uint16_t cvt16_lo(float v) { return cvt16(v - ld16(cvt16(v, 0), 0), 0); }
+UV_DEVINL uint32_t cvt16x2_lo(float a, float b) { return (uint32_t)cvt16_lo(a) | ((uint32_t)cvt16_lo(b) << 16); }
+UV_DEVINL float ld16x3(uint16_t hi, uint16_t lo) { return ld16(hi, 0) + ld16(lo, 0); }
 
 }  // namespace uv

@@ -17,8 +17,10 @@ namespace uv {
 // LayerNorm over rows.  One warp per row.
 // TXT: the text rows of out16p also get a.pos_txt (learned text positions); a separate instantiation, so the kernels without
 // text positions are compiled exactly as before.
+// SPLIT: fp16x3 (LnArgs.split) - add16 is read and out16 / out16p / outc are written as hi / lo pairs, the lo plane `a.lo`
+// elements after the hi plane; again a separate instantiation.
 // ------------------------------------------------------------------------------------------------
-template <bool TXT = false>
+template <bool TXT = false, bool SPLIT = false>
 struct LnStore {
   const LnArgs& a;
   int row, b, l;
@@ -45,32 +47,61 @@ struct LnStore {
       const float4 m = drop_mul4(a.drop, (unsigned int)row, (unsigned int)j);
       v.x *= m.x; v.y *= m.y; v.z *= m.z; v.w *= m.w;
     }
-    uint2 pk;
+    uint2 pk, pkl = make_uint2(0u, 0u);
     pk.x = cvt16x2(v.x, v.y, a.fmt);
     pk.y = cvt16x2(v.z, v.w, a.fmt);
-    if (a.out16) *reinterpret_cast<uint2*>(a.out16 + (size_t)row * a.ld16 + j) = pk;
+    if constexpr (SPLIT) pkl = make_uint2(cvt16x2_lo(v.x, v.y), cvt16x2_lo(v.z, v.w));
+    if (a.out16) {
+      *reinterpret_cast<uint2*>(a.out16 + (size_t)row * a.ld16 + j) = pk;
+      if constexpr (SPLIT) *reinterpret_cast<uint2*>(a.out16 + a.lo + (size_t)row * a.ld16 + j) = pkl;
+    }
     if (a.out16p) {
-      uint2 pp = pk;
+      uint2 pp = pk, ppl = pkl;
       if (has_pos) {
         const float4 p = *reinterpret_cast<const float4*>(a.pos + prow * a.d + j);
         pp.x = cvt16x2(v.x + p.x, v.y + p.y, a.fmt);
         pp.y = cvt16x2(v.z + p.z, v.w + p.w, a.fmt);
+        if constexpr (SPLIT) ppl = make_uint2(cvt16x2_lo(v.x + p.x, v.y + p.y), cvt16x2_lo(v.z + p.z, v.w + p.w));
       }
       if constexpr (TXT) {
         if (a.L > 0 && l >= a.Lv) {
           const float4 p = *reinterpret_cast<const float4*>(a.pos_txt + trow * a.d + j);
           pp.x = cvt16x2(v.x + p.x, v.y + p.y, a.fmt);
           pp.y = cvt16x2(v.z + p.z, v.w + p.w, a.fmt);
+          if constexpr (SPLIT) ppl = make_uint2(cvt16x2_lo(v.x + p.x, v.y + p.y), cvt16x2_lo(v.z + p.z, v.w + p.w));
         }
       }
       *reinterpret_cast<uint2*>(a.out16p + (size_t)row * a.ld16 + j) = pp;
+      if constexpr (SPLIT) *reinterpret_cast<uint2*>(a.out16p + a.lo + (size_t)row * a.ld16 + j) = ppl;
     }
-    if (a.outc && a.L > 0 && l < a.Lv) *reinterpret_cast<uint2*>(a.outc + crow * a.d + j) = pk;
+    if (a.outc && a.L > 0 && l < a.Lv) {
+      *reinterpret_cast<uint2*>(a.outc + crow * a.d + j) = pk;
+      if constexpr (SPLIT) *reinterpret_cast<uint2*>(a.outc + a.lo + crow * a.d + j) = pkl;
+    }
   }
   __device__ __forceinline__ void store1(int j, float v) const {
     if (a.out32) a.out32[(size_t)row * a.d + j] = v;
     if (a.mul32) v *= a.mul32[(size_t)row * a.d + j];
     else if (a.drop.on) v *= drop_mul1(a.drop, (unsigned int)row, (unsigned int)j);
+    if constexpr (SPLIT) {
+      const uint16_t h = cvt16(v, a.fmt), hl = cvt16_lo(v);
+      if (a.out16) {
+        a.out16[(size_t)row * a.ld16 + j] = h;
+        a.out16[a.lo + (size_t)row * a.ld16 + j] = hl;
+      }
+      if (a.out16p) {
+        float vp = v;
+        if (has_pos) vp = v + a.pos[prow * a.d + j];
+        if (TXT && a.L > 0 && l >= a.Lv) vp = v + a.pos_txt[trow * a.d + j];
+        a.out16p[(size_t)row * a.ld16 + j] = cvt16(vp, a.fmt);
+        a.out16p[a.lo + (size_t)row * a.ld16 + j] = cvt16_lo(vp);
+      }
+      if (a.outc && a.L > 0 && l < a.Lv) {
+        a.outc[crow * a.d + j] = h;
+        a.outc[a.lo + crow * a.d + j] = hl;
+      }
+      return;
+    }
     const uint16_t h = cvt16(v, a.fmt);
     if (a.out16) a.out16[(size_t)row * a.ld16 + j] = h;
     if (a.out16p) {
@@ -85,7 +116,7 @@ struct LnStore {
 };
 
 // d == NV * 128: the row lives in registers (NV float4 per lane), one global read.
-template <int NV, bool TXT>
+template <int NV, bool TXT, bool SPLIT = false>
 __global__ void __launch_bounds__(256) layernorm_rows_vec_kernel(const LnArgs a) {
   pdl_prologue();
   const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
@@ -105,10 +136,18 @@ __global__ void __launch_bounds__(256) layernorm_rows_vec_kernel(const LnArgs a)
     v[i] = *reinterpret_cast<const float4*>(x + j);
     if (a.add16) {
       const uint2 h = *reinterpret_cast<const uint2*>(a.add16 + (size_t)warp * a.ld_add16 + j);
-      v[i].x += ld16((uint16_t)(h.x & 0xffff), a.fmt);
-      v[i].y += ld16((uint16_t)(h.x >> 16), a.fmt);
-      v[i].z += ld16((uint16_t)(h.y & 0xffff), a.fmt);
-      v[i].w += ld16((uint16_t)(h.y >> 16), a.fmt);
+      if constexpr (SPLIT) {
+        const uint2 hl = *reinterpret_cast<const uint2*>(a.add16 + a.lo + (size_t)warp * a.ld_add16 + j);
+        v[i].x += ld16x3((uint16_t)(h.x & 0xffff), (uint16_t)(hl.x & 0xffff));
+        v[i].y += ld16x3((uint16_t)(h.x >> 16), (uint16_t)(hl.x >> 16));
+        v[i].z += ld16x3((uint16_t)(h.y & 0xffff), (uint16_t)(hl.y & 0xffff));
+        v[i].w += ld16x3((uint16_t)(h.y >> 16), (uint16_t)(hl.y >> 16));
+      } else {
+        v[i].x += ld16((uint16_t)(h.x & 0xffff), a.fmt);
+        v[i].y += ld16((uint16_t)(h.x >> 16), a.fmt);
+        v[i].z += ld16((uint16_t)(h.y & 0xffff), a.fmt);
+        v[i].w += ld16((uint16_t)(h.y >> 16), a.fmt);
+      }
       if (a.sum_out) *reinterpret_cast<float4*>(a.sum_out + (size_t)warp * a.d + j) = v[i];
     }
     s += (v[i].x + v[i].y) + (v[i].z + v[i].w);
@@ -126,7 +165,7 @@ __global__ void __launch_bounds__(256) layernorm_rows_vec_kernel(const LnArgs a)
     if (a.mean_out) a.mean_out[warp] = mean;
     if (a.rstd_out) a.rstd_out[warp] = rstd;
   }
-  const LnStore<TXT> st(a, warp);
+  const LnStore<TXT, SPLIT> st(a, warp);
 #pragma unroll
   for (int i = 0; i < NV; ++i) {
     const int j = (i * 32 + lane) * 4;
@@ -142,6 +181,7 @@ __global__ void __launch_bounds__(256) layernorm_rows_vec_kernel(const LnArgs a)
 }
 
 // arbitrary d (e.g. 2818 = SlowFast+CLIP+TEF): three passes over the row, later passes hit L1/L2.
+template <bool SPLIT = false>
 __global__ void __launch_bounds__(256) layernorm_rows_generic_kernel(const LnArgs a) {
   pdl_prologue();
   const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
@@ -164,15 +204,18 @@ __global__ void __launch_bounds__(256) layernorm_rows_generic_kernel(const LnArg
     if (a.mean_out) a.mean_out[warp] = mean;
     if (a.rstd_out) a.rstd_out[warp] = rstd;
   }
-  const LnStore<> st(a, warp);
+  const LnStore<false, SPLIT> st(a, warp);
   for (int j = lane; j < a.d; j += 32) st.store1(j, (X(j) - mean) * rstd * a.gamma[j] + a.beta[j]);
   // zero the K padding of the 16-bit operand row (columns d .. ld16)
   if (a.out16)
-    for (int j = a.d + lane; j < a.ld16; j += 32) a.out16[(size_t)warp * a.ld16 + j] = 0;
+    for (int j = a.d + lane; j < a.ld16; j += 32) {
+      a.out16[(size_t)warp * a.ld16 + j] = 0;
+      if constexpr (SPLIT) a.out16[a.lo + (size_t)warp * a.ld16 + j] = 0;
+    }
 }
 
 // arbitrary d <= 128*EPT: one 128-thread block per row, the row lives in registers (single HBM read).
-template <int EPT, bool TXT>
+template <int EPT, bool TXT, bool SPLIT = false>
 __global__ void __launch_bounds__(128) layernorm_rows_block_kernel(const LnArgs a) {
   pdl_prologue();
   __shared__ float s_red[4];
@@ -188,7 +231,10 @@ __global__ void __launch_bounds__(128) layernorm_rows_block_kernel(const LnArgs 
     const int j = tid + 128 * i;
     v[i] = j < a.d ? (x16 ? ld16(x16[j], a.in_fmt) : x[j]) : 0.f;
     if (a.add16 && j < a.d) {
-      v[i] += ld16(a.add16[(size_t)row * a.ld_add16 + j], a.fmt);
+      if constexpr (SPLIT)
+        v[i] += ld16x3(a.add16[(size_t)row * a.ld_add16 + j], a.add16[a.lo + (size_t)row * a.ld_add16 + j]);
+      else
+        v[i] += ld16(a.add16[(size_t)row * a.ld_add16 + j], a.fmt);
       if (a.sum_out) a.sum_out[(size_t)row * a.d + j] = v[i];
     }
     s += v[i];
@@ -218,19 +264,22 @@ __global__ void __launch_bounds__(128) layernorm_rows_block_kernel(const LnArgs 
   }
   __syncthreads();
   const float rstd = s_stat[1];
-  const LnStore<TXT> st(a, row);
+  const LnStore<TXT, SPLIT> st(a, row);
 #pragma unroll
   for (int i = 0; i < EPT; ++i) {
     const int j = tid + 128 * i;
     if (j < a.d) st.store1(j, (v[i] - mean) * rstd * a.gamma[j] + a.beta[j]);
   }
   if (a.out16)
-    for (int j = a.d + tid; j < a.ld16; j += 128) a.out16[(size_t)row * a.ld16 + j] = 0;
+    for (int j = a.d + tid; j < a.ld16; j += 128) {
+      a.out16[(size_t)row * a.ld16 + j] = 0;
+      if constexpr (SPLIT) a.out16[a.lo + (size_t)row * a.ld16 + j] = 0;
+    }
 }
 
 // even d <= 256*EPT2 with 8-byte aligned rows: same as the block kernel with 64-bit loads / 32-bit 16-bit-pair stores
 // (the 2818-wide video features: 27 MB read once, 14 MB written).
-template <int EPT2>
+template <int EPT2, bool SPLIT = false>
 __global__ void __launch_bounds__(128) layernorm_rows_block2_kernel(const LnArgs a) {
   pdl_prologue();
   __shared__ float s_red[4];
@@ -304,14 +353,18 @@ __global__ void __launch_bounds__(128) layernorm_rows_block2_kernel(const LnArgs
           oy *= m8[2 * k + 1];
         }
         *reinterpret_cast<uint32_t*>(a.out16 + (size_t)row * a.ld16 + j) = cvt16x2(ox, oy, a.fmt);
+        if constexpr (SPLIT) *reinterpret_cast<uint32_t*>(a.out16 + a.lo + (size_t)row * a.ld16 + j) = cvt16x2_lo(ox, oy);
       }
     }
   }
-  for (int j = a.d + 2 * tid; j < a.ld16; j += 256) *reinterpret_cast<uint32_t*>(a.out16 + (size_t)row * a.ld16 + j) = 0u;
+  for (int j = a.d + 2 * tid; j < a.ld16; j += 256) {
+    *reinterpret_cast<uint32_t*>(a.out16 + (size_t)row * a.ld16 + j) = 0u;
+    if constexpr (SPLIT) *reinterpret_cast<uint32_t*>(a.out16 + a.lo + (size_t)row * a.ld16 + j) = 0u;
+  }
 }
 
-int launch_layernorm(const LnArgs& a, cudaStream_t stream) {
-  if (a.rows <= 0) return 0;
+template <bool SPLIT>
+static int launch_layernorm_impl(const LnArgs& a, cudaStream_t stream) {
   const int threads = 256;
   const int blocks = (a.rows * 32 + threads - 1) / threads;
   const bool vec_ok = (a.ld_in % 4 == 0) && (a.ld16 == a.d) &&
@@ -321,37 +374,50 @@ int launch_layernorm(const LnArgs& a, cudaStream_t stream) {
       set_error("layernorm: text positions need the structured q/k operand and d <= 3072");
       return (int)cudaErrorInvalidValue;
     }
-    if (vec_ok && a.d == 1024) launch_k(layernorm_rows_vec_kernel<8, true>, dim3(blocks), dim3(threads), 0, stream, a);
-    else if (vec_ok && a.d == 512) launch_k(layernorm_rows_vec_kernel<4, true>, dim3(blocks), dim3(threads), 0, stream, a);
-    else if (vec_ok && a.d == 256) launch_k(layernorm_rows_vec_kernel<2, true>, dim3(blocks), dim3(threads), 0, stream, a);
-    else if (a.d <= 128 * 8) launch_k(layernorm_rows_block_kernel<8, true>, dim3(a.rows), dim3(128), 0, stream, a);
-    else launch_k(layernorm_rows_block_kernel<24, true>, dim3(a.rows), dim3(128), 0, stream, a);
-  } else if (vec_ok && a.d == 1024) launch_k(layernorm_rows_vec_kernel<8, false>, dim3(blocks), dim3(threads), 0, stream, a);
-  else if (vec_ok && a.d == 512) launch_k(layernorm_rows_vec_kernel<4, false>, dim3(blocks), dim3(threads), 0, stream, a);
-  else if (vec_ok && a.d == 256) launch_k(layernorm_rows_vec_kernel<2, false>, dim3(blocks), dim3(threads), 0, stream, a);
+    if (vec_ok && a.d == 1024) launch_k(layernorm_rows_vec_kernel<8, true, SPLIT>, dim3(blocks), dim3(threads), 0, stream, a);
+    else if (vec_ok && a.d == 512) launch_k(layernorm_rows_vec_kernel<4, true, SPLIT>, dim3(blocks), dim3(threads), 0, stream, a);
+    else if (vec_ok && a.d == 256) launch_k(layernorm_rows_vec_kernel<2, true, SPLIT>, dim3(blocks), dim3(threads), 0, stream, a);
+    else if (a.d <= 128 * 8) launch_k(layernorm_rows_block_kernel<8, true, SPLIT>, dim3(a.rows), dim3(128), 0, stream, a);
+    else launch_k(layernorm_rows_block_kernel<24, true, SPLIT>, dim3(a.rows), dim3(128), 0, stream, a);
+  } else if (vec_ok && a.d == 1024) launch_k(layernorm_rows_vec_kernel<8, false, SPLIT>, dim3(blocks), dim3(threads), 0, stream, a);
+  else if (vec_ok && a.d == 512) launch_k(layernorm_rows_vec_kernel<4, false, SPLIT>, dim3(blocks), dim3(threads), 0, stream, a);
+  else if (vec_ok && a.d == 256) launch_k(layernorm_rows_vec_kernel<2, false, SPLIT>, dim3(blocks), dim3(threads), 0, stream, a);
   else if (a.d > 1024 && a.d <= 1024 * 3 && a.d % 2 == 0 && a.ld_in % 2 == 0 && a.ld16 % 2 == 0 && a.out16 && !a.out32 &&
            !a.out16p && !a.outc && !a.add16 && (a.in16 ? (reinterpret_cast<uintptr_t>(a.in16) & 3) == 0 : (reinterpret_cast<uintptr_t>(a.in) & 7) == 0) &&
            (reinterpret_cast<uintptr_t>(a.gamma) & 7) == 0 && (reinterpret_cast<uintptr_t>(a.beta) & 7) == 0 &&
            (!a.mul32 || (reinterpret_cast<uintptr_t>(a.mul32) & 7) == 0))
-    launch_k(layernorm_rows_block2_kernel<12>, dim3(a.rows), dim3(128), 0, stream, a);
-  else if (a.d <= 128 * 8) launch_k(layernorm_rows_block_kernel<8, false>, dim3(a.rows), dim3(128), 0, stream, a);
-  else if (a.d <= 128 * 24) launch_k(layernorm_rows_block_kernel<24, false>, dim3(a.rows), dim3(128), 0, stream, a);
+    launch_k(layernorm_rows_block2_kernel<12, SPLIT>, dim3(a.rows), dim3(128), 0, stream, a);
+  else if (a.d <= 128 * 8) launch_k(layernorm_rows_block_kernel<8, false, SPLIT>, dim3(a.rows), dim3(128), 0, stream, a);
+  else if (a.d <= 128 * 24) launch_k(layernorm_rows_block_kernel<24, false, SPLIT>, dim3(a.rows), dim3(128), 0, stream, a);
   else {
     if (a.add16) {
       set_error("layernorm: fused branch add needs d <= 3072");
       return (int)cudaErrorInvalidValue;
     }
-    launch_k(layernorm_rows_generic_kernel, dim3(blocks), dim3(threads), 0, stream, a);
+    launch_k(layernorm_rows_generic_kernel<SPLIT>, dim3(blocks), dim3(threads), 0, stream, a);
   }
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) set_error("layernorm launch failed: %s", cudaGetErrorString(e));
   return (int)e;
 }
 
+int launch_layernorm(const LnArgs& a, cudaStream_t stream) {
+  if (a.rows <= 0) return 0;
+  if (a.split) {
+    if (a.fmt != 0 || a.mul32 != nullptr || a.drop.on) {
+      set_error("layernorm: fp16x3 output needs fmt 0 and no dropout");
+      return (int)cudaErrorInvalidValue;
+    }
+    return launch_layernorm_impl<true>(a, stream);
+  }
+  return launch_layernorm_impl<false>(a, stream);
+}
+
 // ------------------------------------------------------------------------------------------------
 // Learned text positions (TxtPosArgs, rowops.h).  One warp per text row; lane owns columns 2 (lane + 32 i), i < d / 64.
 // ------------------------------------------------------------------------------------------------
 constexpr int kTxtPosMaxPairs = 16;  // d <= 64 * 16
+template <bool SPLIT = false>
 __global__ void __launch_bounds__(256) txt_pos_rows_kernel(const TxtPosArgs a) {
   pdl_prologue();
   const int row = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
@@ -407,6 +473,7 @@ __global__ void __launch_bounds__(256) txt_pos_rows_kernel(const TxtPosArgs a) {
       *reinterpret_cast<float2*>(a.pos + (size_t)row * a.d + j) = make_float2(ox, oy);
       const float2 xv = *reinterpret_cast<const float2*>(x + j);
       *reinterpret_cast<uint32_t*>(xp + j) = cvt16x2(xv.x + ox, xv.y + oy, a.fmt);
+      if constexpr (SPLIT) *reinterpret_cast<uint32_t*>(xp + a.lo + j) = cvt16x2_lo(xv.x + ox, xv.y + oy);
     }
   }
 }
@@ -417,7 +484,8 @@ int launch_txt_pos(const TxtPosArgs& a, cudaStream_t stream) {
     return (int)cudaErrorInvalidValue;
   }
   const int rows = a.B * a.Lt;
-  launch_k(txt_pos_rows_kernel, dim3((rows * 32 + 255) / 256), dim3(256), 0, stream, a);
+  if (a.split) launch_k(txt_pos_rows_kernel<true>, dim3((rows * 32 + 255) / 256), dim3(256), 0, stream, a);
+  else launch_k(txt_pos_rows_kernel<false>, dim3((rows * 32 + 255) / 256), dim3(256), 0, stream, a);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) set_error("txt_pos launch failed: %s", cudaGetErrorString(e));
   return (int)e;
@@ -623,6 +691,8 @@ int launch_pool_saliency(const PoolSalArgs& a, cudaStream_t stream) {
 // Final conv layer of both heads (out channels 1 and 2) + sigmoid + sign.  One warp per (b, l).
 // Hidden activations are 16-bit in the separated conv layout: row 1 + b*(Lv+1) + l, zero separator rows.
 // ------------------------------------------------------------------------------------------------
+// SPLIT: the hidden activations are fp16x3 pairs (lo plane a.lo elements after the hi plane).
+template <bool SPLIT = false>
 __global__ void __launch_bounds__(256) conv_head_final_kernel(const HeadFinalArgs a) {
   pdl_prologue();
   const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
@@ -640,8 +710,16 @@ __global__ void __launch_bounds__(256) conv_head_final_kernel(const HeadFinalArg
     for (int j = lane * 2; j < a.d; j += 64) {
       const uint32_t c2 = *reinterpret_cast<const uint32_t*>(hc + j);
       const uint32_t s2 = *reinterpret_cast<const uint32_t*>(hs + j);
-      const float c0 = ld16((uint16_t)(c2 & 0xffff), a.fmt), c1 = ld16((uint16_t)(c2 >> 16), a.fmt);
-      const float s0 = ld16((uint16_t)(s2 & 0xffff), a.fmt), s1 = ld16((uint16_t)(s2 >> 16), a.fmt);
+      float c0 = ld16((uint16_t)(c2 & 0xffff), a.fmt), c1 = ld16((uint16_t)(c2 >> 16), a.fmt);
+      float s0 = ld16((uint16_t)(s2 & 0xffff), a.fmt), s1 = ld16((uint16_t)(s2 >> 16), a.fmt);
+      if constexpr (SPLIT) {
+        const uint32_t c2l = *reinterpret_cast<const uint32_t*>(hc + a.lo + j);
+        const uint32_t s2l = *reinterpret_cast<const uint32_t*>(hs + a.lo + j);
+        c0 = ld16x3((uint16_t)(c2 & 0xffff), (uint16_t)(c2l & 0xffff));
+        c1 = ld16x3((uint16_t)(c2 >> 16), (uint16_t)(c2l >> 16));
+        s0 = ld16x3((uint16_t)(s2 & 0xffff), (uint16_t)(s2l & 0xffff));
+        s1 = ld16x3((uint16_t)(s2 >> 16), (uint16_t)(s2l >> 16));
+      }
       acc_c += c0 * wc[j] + c1 * wc[j + 1];
       acc_s0 += s0 * ws0[j] + s1 * ws0[j + 1];
       acc_s1 += s0 * ws1[j] + s1 * ws1[j + 1];
@@ -664,7 +742,8 @@ int launch_conv_head_final(const HeadFinalArgs& a, cudaStream_t stream) {
   const int rows = a.B * a.Lv;
   const int threads = 256;
   const int blocks = (rows * 32 + threads - 1) / threads;
-  launch_k(conv_head_final_kernel, dim3(blocks), dim3(threads), 0, stream, a);
+  if (a.split) launch_k(conv_head_final_kernel<true>, dim3(blocks), dim3(threads), 0, stream, a);
+  else launch_k(conv_head_final_kernel<false>, dim3(blocks), dim3(threads), 0, stream, a);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) set_error("conv_head_final launch failed: %s", cudaGetErrorString(e));
   return (int)e;

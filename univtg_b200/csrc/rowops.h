@@ -34,6 +34,8 @@ struct LnArgs {
   DropSpec drop;       // in-kernel input dropout (drop.on; ignored when mul32 is given): same multiplier semantics
   float* mean_out;     // [rows] (training)
   float* rstd_out;     // [rows]
+  int split;           // 1: fp16x3 (fmt 0, inference): add16 is read and out16 / out16p / outc are written as hi / lo pairs
+  long long lo;        // split: elements from each of those buffers to its lo plane
 };
 int launch_layernorm(const LnArgs& a, cudaStream_t stream);
 
@@ -51,6 +53,8 @@ struct TxtPosArgs {
   float* rstd_out;
   uint16_t* xpos16;     // [B*L, d] q/k operand of encoder layer 0
   int B, Lt, L, Lv, d, fmt;
+  int split;            // 1: fp16x3 - xpos16 gets its lo plane too, `lo` elements after the hi plane
+  long long lo;
 };
 int launch_txt_pos(const TxtPosArgs& a, cudaStream_t stream);
 
@@ -87,6 +91,8 @@ struct HeadFinalArgs {
   float* pred_logits;      // [B, Lv, 1]
   float* pred_spans;       // [B, Lv, 2]
   int B, Lv, d, fmt;
+  int split;               // 1: fp16x3 - h_cls / h_span are hi / lo pairs, the lo planes `lo` elements after the hi planes
+  long long lo;
 };
 int launch_conv_head_final(const HeadFinalArgs& a, cudaStream_t stream);
 
@@ -99,6 +105,8 @@ struct AttnArgs {
   float* lse;             // [B, H, L] log-sum-exp per query row (training) or null
   int B, L, H, dh, d, fmt;
   DropSpec drop;          // attention dropout (drop.on; stream = encoder layer): P o M feeds P V, the row sum and lse stay un-dropped
+  int split;              // 1: fp16x3 (fmt 0, no dropout): qkv and out are hi / lo pairs; tm_qkv is then a make_tmap_split pair
+  long long lo_qkv, lo_out;  // split: elements from qkv / out to their lo planes
 };
 int launch_attention(const AttnArgs& a, cudaStream_t stream);
 // SIMT variant for head sizes outside {64,128}; reads qkv through a plain pointer.

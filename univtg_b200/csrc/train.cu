@@ -131,13 +131,16 @@ int univtg_prepare_workspace(const univtg_config* cfg, const univtg_shape* shape
     zero(w.hs2, (Mh + 2) * d * 2);
   };
   if (training_ws) {
+    if (refuse_split(*cfg, "univtg_prepare_workspace (training workspace)")) return 1;
     const TrainWs T = make_train_ws(*cfg, *shape, L, base);
     zero_heads(T);
     zero(T.dhc2, (Mh + 2) * d * 2);
     zero(T.dhs2, (Mh + 2) * d * 2);
     zero(T.dh1, (Mh + 2) * 2 * d * 2);
   } else {
-    zero_heads(make_infer_ws(*cfg, *shape, L, base));
+    const FwdBufs w = make_infer_ws(*cfg, *shape, L, base);
+    zero_heads(w);
+    if (is_split(*cfg)) zero_heads(make_infer_ws(*cfg, *shape, L, base + w.total));  // the lo planes
   }
   if (e != cudaSuccess) {
     set_error("univtg_prepare_workspace: %s", cudaGetErrorString(e));
@@ -147,7 +150,7 @@ int univtg_prepare_workspace(const univtg_config* cfg, const univtg_shape* shape
 }
 
 size_t univtg_train_workspace_bytes(const univtg_config* cfg, const univtg_shape* shape) {
-  if (!check_cfg(cfg) || !check_shape(shape)) return 0;
+  if (!check_cfg(cfg) || !check_shape(shape) || refuse_split(*cfg, "univtg_train_workspace_bytes")) return 0;
   return make_train_ws(*cfg, *shape, make_layout(*cfg), nullptr).total;
 }
 
@@ -163,6 +166,7 @@ int univtg_forward_train(univtg_plan* P, void* ws, const float* src_txt, const f
     set_error("univtg_forward_train: null argument");
     return 1;
   }
+  if (refuse_split(P->cfg, "univtg_forward_train")) return 1;
   if (P->attn_dropout > 0.f && !rng) {
     set_error("univtg_forward_train: attention dropout p = %g needs an rng (its masks are drawn in-kernel)", (double)P->attn_dropout);
     return 1;
@@ -191,6 +195,7 @@ int univtg_backward(univtg_plan* P, void* ws, const float* src_txt, const float*
     set_error("univtg_backward: null argument");
     return 1;
   }
+  if (refuse_split(P->cfg, "univtg_backward")) return 1;
   const univtg_config& c = P->cfg;
   const int n_params = univtg_num_params(&c) + (P->txt_pos_on ? 3 : 0);  // + txt_position_embed.* with learned text positions
   if (n_grads != n_params) {
@@ -859,6 +864,7 @@ int univtg_op_attention_bwd(const void* qkv, const void* dO, const void* O, cons
     set_error("univtg_op_attention_bwd: null argument");
     return 1;
   }
+  if (refuse_fmt2(fmt_act, "univtg_op_attention_bwd")) return 1;
   cudaStream_t st = (cudaStream_t)stream;
   const int d = H * dh, M = B * L;
   int rc = launch_attn_delta(reinterpret_cast<const uint16_t*>(dO), fmt_act, reinterpret_cast<const uint16_t*>(O), fmt_act,
@@ -904,6 +910,7 @@ int univtg_op_gemm_group(univtg_gemm_problem* problems, int32_t num, int32_t fmt
                          void* stream) {
   const char* fn = "univtg_op_gemm_group";
   UV_REQ(problems != nullptr && num >= 1 && num <= GEMM_MAX_GROUP, "%s: problems must hold 1..%d entries", fn, GEMM_MAX_GROUP);
+  if (refuse_fmt2(fmt, fn)) return 1;
   UV_REQ(fmt == 0 || fmt == 1, "%s: fmt %d (0 fp16, 1 bf16)", fn, fmt);
   UV_REQ(bn >= 32 && bn <= 256 && bn % 16 == 0, "%s: bn %d (multiple of 16 in [32, 256])", fn, bn);
   UV_REQ(cluster == 1 || cluster == 2, "%s: cluster %d (1 or 2)", fn, cluster);
@@ -1011,6 +1018,7 @@ int univtg_op_layernorm_bwd(const univtg_ln_bwd* q, const univtg_rng* rng, int32
   UV_REQ(!q->dbr16 || q->ld16 >= q->d, "%s: ld16 %d smaller than d %d", fn, q->ld16, q->d);
   UV_REQ(!q->y16 || (!q->dy32 && !q->dbr16), "%s: a 16-bit y (y16) is only supported for parameter gradients (dy32 = dbr16 = NULL)", fn);
   UV_REQ(!q->row_scale || q->L >= 1, "%s: row_scale needs L >= 1", fn);
+  if (refuse_fmt2(q->fmt16, fn) || refuse_fmt2(q->y_fmt, fn)) return 1;
   UV_REQ(q->fmt16 == 0 || q->fmt16 == 1, "%s: fmt16 %d", fn, q->fmt16);
   UV_REQ(q->y_fmt == 0 || q->y_fmt == 1, "%s: y_fmt %d", fn, q->y_fmt);
   UV_REQ(al_(q->dout, 4) && al_(q->y, 4) && al_(q->y16, 2) && al_(q->dbr16, 2) && al_(q->dy32, 4) && al_(q->dgamma, 4) &&
@@ -1058,6 +1066,7 @@ int univtg_op_head_final_bwd(const univtg_head_final_bwd* q, void* stream) {
   UV_REQ((q->cs_cls == nullptr) == (q->cs_span == nullptr), "%s: cs_cls and cs_span must both be given or both be NULL", fn);
   UV_REQ(q->B >= 1 && q->Lv >= 1, "%s: B %d / Lv %d", fn, q->B, q->Lv);
   UV_REQ(q->d >= 8 && q->d % 8 == 0, "%s: d %d must be a positive multiple of 8 (128-bit loads)", fn, q->d);
+  if (refuse_fmt2(q->fmt_act, fn) || refuse_fmt2(q->fmt_grad, fn)) return 1;
   UV_REQ((q->fmt_act == 0 || q->fmt_act == 1) && (q->fmt_grad == 0 || q->fmt_grad == 1), "%s: fmt_act / fmt_grad", fn);
   UV_REQ(al_(q->h_cls, 16) && al_(q->h_span, 16) && al_(q->dh_cls, 16) && al_(q->dh_span, 16) && al_(q->dz, 16) && al_(q->gw_cls, 16) &&
              al_(q->gw_span, 16) && al_(q->cs_cls, 16) && al_(q->cs_span, 16),
@@ -1114,6 +1123,7 @@ int univtg_op_colsum16(const void* in16, int32_t ld, int32_t rows, int32_t cols,
   UV_REQ(rows >= 1 && cols >= 8 && cols % 8 == 0 && ld >= cols && ld % 8 == 0, "%s: rows %d / cols %d / ld %d (multiples of 8, ld >= cols)", fn,
          rows, cols, ld);
   UV_REQ(al_(in16, 16) && al_(colsum, 16), "%s: in16 and colsum must be 16-byte aligned", fn);
+  if (refuse_fmt2(fmt, fn)) return 1;
   UV_REQ(fmt == 0 || fmt == 1, "%s: fmt %d", fn, fmt);
   TxtRows t;
   if (txt_rows_arg(fn, txt16, L, Lv, txt_cols, rows, cols, 8, t)) return 1;
@@ -1127,6 +1137,7 @@ int univtg_op_cvt16_colsum(const float* in32, int32_t ld_in, void* out16, int32_
   UV_REQ(rows >= 1 && cols >= 4 && cols % 4 == 0 && ld_in >= cols && ld_in % 4 == 0 && ld_out >= cols && ld_out % 4 == 0,
          "%s: rows %d / cols %d / ld_in %d / ld_out %d (multiples of 4, pitches >= cols)", fn, rows, cols, ld_in, ld_out);
   UV_REQ(al_(in32, 16) && al_(out16, 8) && al_(colsum, 4), "%s: in32 must be 16-byte, out16 8-byte aligned", fn);
+  if (refuse_fmt2(fmt, fn)) return 1;
   UV_REQ(fmt == 0 || fmt == 1, "%s: fmt %d", fn, fmt);
   TxtRows t;
   if (txt_rows_arg(fn, txt16, L, Lv, txt_cols, rows, cols, 4, t)) return 1;
@@ -1141,6 +1152,7 @@ int univtg_op_stream_gather(const float* dx, int32_t L, int32_t off, const float
   UV_REQ(B >= 1 && Ls >= 1 && off >= 0 && off + Ls <= L, "%s: B %d / Ls %d / off %d / L %d (off + Ls <= L)", fn, B, Ls, off, L);
   UV_REQ(d >= 4 && d % 4 == 0, "%s: d %d must be a positive multiple of 4", fn, d);
   UV_REQ(al_(dx, 16) && al_(extra, 16) && al_(out16, 8) && al_(colsum, 4), "%s: dx / extra must be 16-byte, out16 8-byte aligned", fn);
+  if (refuse_fmt2(fmt, fn)) return 1;
   UV_REQ(fmt == 0 || fmt == 1, "%s: fmt %d", fn, fmt);
   return launch_stream_gather(dx, L, off, extra, extra_scale, reinterpret_cast<uint16_t*>(out16), colsum, colsum_scale, B, Ls, d, fmt,
                               (cudaStream_t)stream);

@@ -26,6 +26,10 @@ class FlatAdamW(torch.optim.Optimizer):
     def __init__(self, model, lr=1e-4, betas=(0.9, 0.999), eps=1e-8, weight_decay=1e-4, max_grad_norm=0.1,
                  write_clipped_grads=False, dynamic_loss_scale=True, growth_interval=2000, max_loss_scale=65536.0,
                  zero_grad_after_step=False):
+        if getattr(model, "operand_format", 0) == 2:
+            from .plugin import STRICT_TRAINING_REFUSAL
+
+            raise NotImplementedError(STRICT_TRAINING_REFUSAL)
         self.model = model
         # zero_grad_after_step: step() ends by zero-filling the flat gradient buffer on a side stream (as if zero_grad() were called
         # right after it - the reference loop calls it before the next backward anyway, train_vlp_ddp.py:63); the fill then runs

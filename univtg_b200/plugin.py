@@ -122,6 +122,10 @@ class _WorkspaceLease:
             pass
 
 
+STRICT_TRAINING_REFUSAL = ("operand_format='fp16x3' is an inference mode: run the forward under model.eval() or torch.no_grad(), "
+                           "and train with operand_format='fp16' or 'bf16'")
+
+
 class Model(nn.Module):
     """H100-native UniVTG model: the reference `Model` (model/univtg.py:51-155) behind the same interface."""
 
@@ -141,7 +145,7 @@ class Model(nn.Module):
         self.span_loss_type = args.span_loss_type
         self.use_txt_pos = bool(args.use_txt_pos)
         self.max_v_l = int(getattr(args, "max_v_l", 75))
-        self.operand_format = {"fp16": 0, "bf16": 1}[getattr(args, "operand_format", "fp16")]
+        self.operand_format = {"fp16": 0, "bf16": 1, "fp16x3": 2}[getattr(args, "operand_format", "fp16")]
         self.grad_scale = float(getattr(args, "grad_scale", 1024.0 if self.operand_format == 0 else 1.0))
         if bool(getattr(args, "pre_norm", False)):
             # the reference raises AttributeError here (forward_pre is not defined, transformer_encoder_droppath.py:128-134)
@@ -167,14 +171,15 @@ class Model(nn.Module):
 
         # One 16-bit operand format per model (a wgmma takes A and B in ONE format): fp16 by default - its 11-bit
         # significand keeps the north-star tolerance - with gradients carried under a power-of-two loss scale in backward
-        # (fp16 would underflow otherwise); "bf16" needs no scaling but is 8x coarser.
+        # (fp16 would underflow otherwise); "bf16" needs no scaling but is 8x coarser.  "fp16x3" (inference only) stores every
+        # operand as fp16 hi + lo planes and multiplies A_hi B_hi + A_lo B_hi + A_hi B_lo: it tracks an fp32 forward to ~1e-6.
         self._packed = {}
         self._packed_key = {}
         self._plans = {}
         self._dim_t = None
         self._cfgs = {
             fmt: _lib.Config(d, self.nheads, self.dim_feedforward, self.enc_layers, self.n_input_proj, self.vid_dim, self.txt_dim, fmt)
-            for fmt in (0, 1)}
+            for fmt in (0, 1, 2)}
         self._cfg = self._cfgs[self.operand_format]
 
     # ---- initialisation with the reference's distributions --------------------------------------------------------
@@ -493,6 +498,8 @@ class Model(nn.Module):
         if tuple(src_vid_mask.shape) != (B, Lv) or tuple(src_txt_mask.shape) != (B, Lt):
             raise ValueError("mask shapes do not match the features")
         training = self.training and torch.is_grad_enabled()
+        if training and self.operand_format == 2:
+            raise NotImplementedError(STRICT_TRAINING_REFUSAL)
         if training:
             from .autograd import forward_train  # backward kernels live in the same library
 
