@@ -26,8 +26,10 @@
 
 namespace uv {
 
-// The tile width BN is a RUN-TIME value (multiple of 16, 16..256; multiple of 64 when B is MN-major, of 128 for MN-major B in
-// clusters): the host picks it per launch so that the tile count fills the SMs with as little wave quantisation as possible.
+// The tile width BN is a launch argument, checked by launch_gemm_group: a multiple of 16 in [32, 256]; a multiple of 32 for 2-CTA
+// clusters, which need a K-major B; a multiple of 64 when B is MN-major (CL = 1 only).  The host picks it per launch so that the
+// tile count fills the SMs with as little wave quantisation as possible; the consumers dispatch on it once (consumer_tiles<BN>),
+// and only the widths above are compiled.
 // Operand ring: kRingBytes of shared memory cut into as many stages as the tile width allows (a stage = the 16 KB A tile + BN x
 // 128 B of B), at most kMaxStages.
 template <int CL>
@@ -98,43 +100,89 @@ __device__ __forceinline__ void mma_cols(float* acc, uint64_t da, uint64_t db, u
     mma_cols<N - W, OFF + W, BF, TA, TB>(acc, da, db + adv, scale_d);
   }
 }
-template <int N, int BF, int TA, int TB>
-__device__ __forceinline__ void mma_kblock(float* acc, uint64_t da, uint64_t db, uint32_t a_step, uint32_t b_step, bool acc_in) {
-#pragma unroll
-  for (int k = 0; k < GEMM_BK / 16; ++k) mma_cols<N, 0, BF, TA, TB>(acc, da + k * a_step, db + k * b_step, (acc_in || k > 0) ? 1u : 0u);
+
+// The consumer's view of the operand ring: where the stages are and which stage / phase it waits on next.
+struct Ring {
+  uint8_t* base;
+  uint64_t* full;
+  uint64_t* empty;
+  int stage_bytes, stages;
+  int stage;
+  uint32_t phase;
+};
+
+template <int CL>
+__device__ __forceinline__ void release_stage(const Ring& ring, int s, int tid, int crank) {
+  // this warpgroup is done with stage s (in every CTA the stage was multicast from)
+  if (tid == 0) {
+    mbar_arrive(&ring.empty[s]);
+    if (CL > 1) mbar_arrive_cluster(mapa_shared(smem_u32(&ring.empty[s]), (uint32_t)(crank ^ 1)));
+  }
 }
-template <int N>
-__device__ __forceinline__ void mma_kblock_n(float* acc, int bf, int a_mn, int b_mn, uint64_t da, uint64_t db, uint32_t a_step,
-                                             uint32_t b_step, bool acc_in) {
-  if constexpr (N % 64 == 0) {
-    if (b_mn) {
-      if (bf) {
-        if (a_mn) mma_kblock<N, 1, 1, 1>(acc, da, db, a_step, b_step, acc_in);
-        else mma_kblock<N, 1, 0, 1>(acc, da, db, a_step, b_step, acc_in);
-      } else {
-        if (a_mn) mma_kblock<N, 0, 1, 1>(acc, da, db, a_step, b_step, acc_in);
-        else mma_kblock<N, 0, 0, 1>(acc, da, db, a_step, b_step, acc_in);
-      }
-      return;
+
+// k-blocks [kb0, kb1) of one tile into acc (BN / 2 floats: one m64nBN accumulator).  Width, operand format and both layouts are
+// template parameters, so each combination gets a k-loop of its own; with a run-time choice inside the k-loop ptxas cannot keep
+// more than one wgmma in flight.
+template <int CL, int BN, int BF, int TA, int TB>
+__device__ __forceinline__ void tile_mainloop(float* acc, Ring& ring, int kb0, int kb1, int cw, int tid, int crank) {
+  // descriptor = constant high part (layout, LBO/SBO) + start address; one k-step of 16 elements advances the address by 32 B
+  // inside the 128 B swizzle span (K-major) or by two 1024 B swizzle atoms (MN-major), in 16-byte units
+  const uint64_t da_hi = TA ? make_smem_desc_sw128(0, 8192, 1024) : make_smem_desc_sw128(0, 16, 1024);
+  const uint64_t db_hi = TB ? make_smem_desc_sw128(0, 8192, 1024) : make_smem_desc_sw128(0, 16, 1024);
+  constexpr uint32_t a_step = TA ? 128u : 2u, b_step = TB ? 128u : 2u;
+  int prev = -1;
+  for (int kb = kb0; kb < kb1; ++kb) {
+    mbar_wait(&ring.full[ring.stage], ring.phase);
+    const uint32_t sa = smem_u32(ring.base + ring.stage * ring.stage_bytes);
+    // this warpgroup's 64 rows of A: K-major rows 64 cw.. (64 x 128 B); MN-major the cw-th 64-wide M block (8 KB each)
+    const uint64_t da = da_hi + (uint64_t)((sa + cw * 8192) >> 4);
+    const uint64_t db = db_hi + (uint64_t)((sa + GemmCfg<CL>::kABytes) >> 4);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < GEMM_BK / 16; ++k)
+      mma_cols<BN, 0, BF, TA, TB>(acc, da + k * a_step, db + k * b_step, (kb > kb0 || k > 0) ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<1>();  // the previous k-block's MMAs have retired: its stage can be refilled
+    if (prev >= 0) release_stage<CL>(ring, prev, tid, crank);
+    prev = ring.stage;
+    if (++ring.stage == ring.stages) {
+      ring.stage = 0;
+      ring.phase ^= 1;
     }
   }
-  if (bf) {
-    if (a_mn) mma_kblock<N, 1, 1, 0>(acc, da, db, a_step, b_step, acc_in);
-    else mma_kblock<N, 1, 0, 0>(acc, da, db, a_step, b_step, acc_in);
-  } else {
-    if (a_mn) mma_kblock<N, 0, 1, 0>(acc, da, db, a_step, b_step, acc_in);
-    else mma_kblock<N, 0, 0, 0>(acc, da, db, a_step, b_step, acc_in);
-  }
+  wgmma_wait<0>();
+#pragma unroll
+  for (int i = 0; i < BN / 2; ++i) reg_fence(acc[i]);
+  if (prev >= 0) release_stage<CL>(ring, prev, tid, crank);
 }
-__device__ __forceinline__ void mma_kblock_bn(int bn, float* acc, int bf, int a_mn, int b_mn, uint64_t da, uint64_t db,
-                                              uint32_t a_step, uint32_t b_step, bool acc_in) {
-  switch (bn >> 4) {
-#define UV_BN_CASE(k) \
-  case k: mma_kblock_n<16 * k>(acc, bf, a_mn, b_mn, da, db, a_step, b_step, acc_in); break;
-    UV_BN_CASE(1) UV_BN_CASE(2) UV_BN_CASE(3) UV_BN_CASE(4) UV_BN_CASE(5) UV_BN_CASE(6) UV_BN_CASE(7) UV_BN_CASE(8)
-    UV_BN_CASE(9) UV_BN_CASE(10) UV_BN_CASE(11) UV_BN_CASE(12) UV_BN_CASE(13) UV_BN_CASE(14) UV_BN_CASE(15) UV_BN_CASE(16)
-#undef UV_BN_CASE
-    default: break;
+
+// Operand format and layouts are per problem: pick the k-loop once per tile.  fp16x3 groups are K-major fp16 only, clusters
+// need a K-major B and MN-major B needs BN % 64 == 0 (all checked on the host), so only those k-loops are compiled.
+template <int CL, bool SPLIT, int BN>
+__device__ __forceinline__ void tile_mainloop_any(float* acc, Ring& ring, int bf, int a_mn, int b_mn, int kb0, int kb1, int cw, int tid,
+                                                  int crank) {
+  if constexpr (SPLIT) {
+    tile_mainloop<CL, BN, 0, 0, 0>(acc, ring, kb0, kb1, cw, tid, crank);
+  } else {
+    if constexpr (CL == 1 && BN % 64 == 0) {
+      if (b_mn) {
+        if (bf) {
+          if (a_mn) tile_mainloop<CL, BN, 1, 1, 1>(acc, ring, kb0, kb1, cw, tid, crank);
+          else tile_mainloop<CL, BN, 1, 0, 1>(acc, ring, kb0, kb1, cw, tid, crank);
+        } else {
+          if (a_mn) tile_mainloop<CL, BN, 0, 1, 1>(acc, ring, kb0, kb1, cw, tid, crank);
+          else tile_mainloop<CL, BN, 0, 0, 1>(acc, ring, kb0, kb1, cw, tid, crank);
+        }
+        return;
+      }
+    }
+    if (bf) {
+      if (a_mn) tile_mainloop<CL, BN, 1, 1, 0>(acc, ring, kb0, kb1, cw, tid, crank);
+      else tile_mainloop<CL, BN, 1, 0, 0>(acc, ring, kb0, kb1, cw, tid, crank);
+    } else {
+      if (a_mn) tile_mainloop<CL, BN, 0, 1, 0>(acc, ring, kb0, kb1, cw, tid, crank);
+      else tile_mainloop<CL, BN, 0, 0, 0>(acc, ring, kb0, kb1, cw, tid, crank);
+    }
   }
 }
 
@@ -344,6 +392,96 @@ __device__ __forceinline__ void epi_step(const GemmProblem& pr, const EpiRow& r,
   }
 }
 
+// ---- one consumer warpgroup: every tile of its schedule at tile width BN ----
+// Each width has its own accumulator array, k-loops and epilogue read-out; the kernel picks the width once, before the first tile.
+template <int CL, bool FULL, bool SPLIT, int BN>
+__device__ __forceinline__ void consumer_tiles(const GemmGroup& g, Ring& ring, float* epi_buf, int tile0, int tstep, int crank, int cw,
+                                               int lane) {
+  using Cfg = GemmCfg<CL>;
+  const int tid = threadIdx.x & 127;
+  const int fr = 16 * (tid >> 5) + (lane >> 2);  // accumulator fragment: rows fr, fr + 8; columns 8 i + fc, + 1
+  const int fc = 2 * (lane & 3);
+  const int erow = tid & 63, ehalf = tid >> 6;  // epilogue: thread = row erow, columns [16 ehalf, +16) of each 32-column chunk
+  float* ebuf = epi_buf + cw * 64 * Cfg::kEpiStride;
+  const int fmt = g.fmt;
+  float acc[BN / 2];
+#pragma unroll
+  for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+  TileInfo ti;
+  bool first_tile = true;
+  for (int t = tile0; decode_tile<CL, SPLIT>(g, BN, t, crank, ti); t += tstep) {
+    const GemmProblem& pr = g.p[ti.p];
+    const int bf = pr.a_fmt < 0 ? fmt : pr.a_fmt;  // both operands share it (checked on the host)
+    if (first_tile && g.dbg != nullptr && ti.kb0 < ti.kb1) {
+      mbar_wait(&ring.full[ring.stage], ring.phase);
+      if (tid == 0 && cw == 0) stamp(g.dbg, 3);  // first operand stage landed
+    }
+    tile_mainloop_any<CL, SPLIT, BN>(acc, ring, bf, pr.a_mn, pr.b_mn, ti.kb0, ti.kb1, cw, tid, crank);
+    if (tid == 0 && cw == 0) stamp(g.dbg, 4);  // last MMA of the tile retired
+    first_tile = false;
+
+    // ========================================= epilogue =========================================
+    const int pM = pr.M, pN = pr.N, rps_in = pr.rps_in;
+    const int m = ti.m_blk * GEMM_BM + cw * 64 + erow;
+    int b = 0, l = m;
+    if (rps_in > 0) {
+      b = m / rps_in;
+      l = m - b * rps_in;
+    }
+    const bool is_sep = (rps_in > 0) && (l == rps_in - 1);
+    EpiRow r;
+    r.valid = (m < pM) && !(pr.skip_sep && is_sep);
+    r.rsc = pr.alpha;
+    if (pr.row_scale != nullptr && m < pM) r.rsc *= pr.row_scale[b];
+    if (pr.zero_sep && is_sep) r.rsc = 0.f;
+    const size_t orow = (size_t)((rps_in > 0 ? b * pr.rps_out + l : m) + pr.row_off);
+    r.resid_row = pr.resid ? pr.resid + orow * pr.ld_resid : nullptr;
+    r.aux_row = (FULL && pr.aux32) ? pr.aux32 + orow * pr.ld_aux : nullptr;
+    r.mask_row = (FULL && pr.mask16) ? pr.mask16 + orow * pr.ld_mask : nullptr;
+    r.add_row = pr.addtab ? pr.addtab + (size_t)m * pr.ld_addtab : nullptr;
+    r.o32_row = pr.out32 ? pr.out32 + orow * pr.ld32 : nullptr;
+    r.o32i_row = ((FULL || SPLIT) && pr.out32_id) ? pr.out32_id + (size_t)m * pr.ld32_id : nullptr;
+    r.o16_row = pr.out16 ? pr.out16 + orow * pr.ld16 : nullptr;
+    r.o16p_row = pr.out16p ? pr.out16p + orow * pr.ld16 : nullptr;
+    r.pre_row = (FULL && pr.pre32) ? pr.pre32 + orow * pr.ld_pre : nullptr;
+    r.dact_row = (FULL && pr.dact16) ? pr.dact16 + orow * pr.ld_dact : nullptr;
+    const float* __restrict__ bias = (ti.split == 0) ? pr.bias : nullptr;
+    const int nt0 = ti.n_blk * BN;
+    // 32-column chunks; when BN % 32 == 16 the last chunk holds 16 columns (its ehalf = 1 half is neither staged nor read).
+    // The chunk loop stays rolled so that each width carries one copy of the epilogue; only the staging of a chunk's
+    // accumulators (registers named at compile time) is unrolled.
+#pragma unroll 1
+    for (int cc = 0; cc < (BN + 31) / 32 && nt0 + cc * 32 < pN; ++cc) {  // warpgroup-uniform
+#pragma unroll
+      for (int c = 0; c < (BN + 31) / 32; ++c) {
+        if (c == cc) {
+#pragma unroll
+          for (int ii = 0; ii < 4; ++ii) {
+            const int i = 4 * c + ii;
+            if (8 * i < BN) {
+              *reinterpret_cast<float2*>(ebuf + fr * Cfg::kEpiStride + 8 * ii + fc) = make_float2(acc[4 * i], acc[4 * i + 1]);
+              *reinterpret_cast<float2*>(ebuf + (fr + 8) * Cfg::kEpiStride + 8 * ii + fc) = make_float2(acc[4 * i + 2], acc[4 * i + 3]);
+            }
+          }
+        }
+      }
+      named_bar_sync(1 + cw, 128);
+      const int n0 = nt0 + cc * 32 + ehalf * 16;
+      if (cc * 32 + ehalf * 16 < BN && n0 < pN) {  // warp-uniform (a warp's rows share ehalf)
+        float v[16];
+        ld16f(ebuf + erow * Cfg::kEpiStride + ehalf * 16, v);
+        if (bias != nullptr) {
+#pragma unroll
+          for (int j = 0; j < 16; ++j) v[j] += (n0 + j < pN) ? __ldg(bias + n0 + j) : 0.f;
+        }
+        epi_step<FULL, SPLIT>(pr, r, v, n0, fmt, lane, g.lo16);
+      }
+      named_bar_sync(1 + cw, 128);
+    }
+    if (tid == 0 && cw == 1) stamp(g.dbg, 6);  // epilogue of the tile done (second warpgroup)
+  }
+}
+
 // SPLIT (fp16x3, CL = 1, K-major operands only): tm_a / tm_b are 3-D maps whose third coordinate selects the hi (0) or lo (1)
 // plane.  A problem walks its taps x kblk_per_tap k-blocks three times - (A hi, B hi), (A lo, B hi), (A hi, B lo) - into the
 // same accumulators; only the producer knows about the planes.
@@ -459,111 +597,20 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_wgmma_kernel(const __gri
   } else {
     setmaxnreg_inc<232>();
     // ======================================= consumers =======================================
-    const int cw = wg;                       // rows [64 cw, 64 cw + 64) of the tile
-    const int tid = threadIdx.x & 127;
-    const int fr = 16 * (tid >> 5) + (lane >> 2);  // accumulator fragment: rows fr, fr + 8; columns 8 i + fc, + 1
-    const int fc = 2 * (lane & 3);
-    const int erow = tid & 63, ehalf = tid >> 6;  // epilogue: thread = row erow, columns [16 ehalf, +16) of each 32-column chunk
-    float* ebuf = epi_buf + cw * 64 * Cfg::kEpiStride;
-    const int fmt = g.fmt;
-    float acc[128];
-#pragma unroll
-    for (int i = 0; i < 128; ++i) acc[i] = 0.f;
-    int stage = 0;
-    uint32_t phase = 0;
-    TileInfo ti;
-    auto release = [&](int s) {  // this warpgroup is done with stage s (in every CTA the stage was multicast from)
-      if (tid == 0) {
-        mbar_arrive(&empty_bar[s]);
-        if (CL > 1) mbar_arrive_cluster(mapa_shared(smem_u32(&empty_bar[s]), (uint32_t)(crank ^ 1)));
-      }
-    };
-    bool first_tile = true;
-    for (int t = tile0; decode_tile<CL, SPLIT>(g, BN, t, crank, ti); t += tstep) {
-      const GemmProblem& pr = g.p[ti.p];
-      const int bf = pr.a_fmt < 0 ? fmt : pr.a_fmt;  // both operands share it (checked on the host)
-      // descriptor = constant high part (layout, LBO/SBO) + start address; one k-step of 16 elements advances the address by
-      // 32 B inside the 128 B swizzle span (K-major) or by two 1024 B swizzle atoms (MN-major), in 16-byte units
-      const uint64_t da_hi = pr.a_mn ? make_smem_desc_sw128(0, 8192, 1024) : make_smem_desc_sw128(0, 16, 1024);
-      const uint64_t db_hi = pr.b_mn ? make_smem_desc_sw128(0, 8192, 1024) : make_smem_desc_sw128(0, 16, 1024);
-      const uint32_t a_step = pr.a_mn ? 128u : 2u, b_step = pr.b_mn ? 128u : 2u;
-      int prev = -1;
-      for (int kb = ti.kb0; kb < ti.kb1; ++kb) {
-        mbar_wait(&full_bar[stage], phase);
-        if (tid == 0 && cw == 0 && kb == ti.kb0 && first_tile) stamp(g.dbg, 3);  // first operand stage landed
-        const uint32_t sa = smem_u32(stage_base + stage * kStageBytes);
-        // this warpgroup's 64 rows of A: K-major rows 64 cw.. (64 x 128 B); MN-major the cw-th 64-wide M block (8 KB each)
-        const uint64_t da = da_hi + (uint64_t)((sa + cw * 8192) >> 4);
-        const uint64_t db = db_hi + (uint64_t)((sa + Cfg::kABytes) >> 4);
-        wgmma_fence();
-        mma_kblock_bn(BN, acc, bf, pr.a_mn, pr.b_mn, da, db, a_step, b_step, kb > ti.kb0);
-        wgmma_commit();
-        wgmma_wait<1>();  // the previous k-block's MMAs have retired: its stage can be refilled
-        if (prev >= 0) release(prev);
-        prev = stage;
-        if (++stage == kStages) {
-          stage = 0;
-          phase ^= 1;
-        }
-      }
-      wgmma_wait<0>();
-#pragma unroll
-      for (int i = 0; i < 128; ++i) reg_fence(acc[i]);
-      if (prev >= 0) release(prev);
-      if (tid == 0 && cw == 0) stamp(g.dbg, 4);  // last MMA of the tile retired
-      first_tile = false;
-
-      // ========================================= epilogue =========================================
-      const int pM = pr.M, pN = pr.N, rps_in = pr.rps_in;
-      const int m = ti.m_blk * GEMM_BM + cw * 64 + erow;
-      int b = 0, l = m;
-      if (rps_in > 0) {
-        b = m / rps_in;
-        l = m - b * rps_in;
-      }
-      const bool is_sep = (rps_in > 0) && (l == rps_in - 1);
-      EpiRow r;
-      r.valid = (m < pM) && !(pr.skip_sep && is_sep);
-      r.rsc = pr.alpha;
-      if (pr.row_scale != nullptr && m < pM) r.rsc *= pr.row_scale[b];
-      if (pr.zero_sep && is_sep) r.rsc = 0.f;
-      const size_t orow = (size_t)((rps_in > 0 ? b * pr.rps_out + l : m) + pr.row_off);
-      r.resid_row = pr.resid ? pr.resid + orow * pr.ld_resid : nullptr;
-      r.aux_row = (FULL && pr.aux32) ? pr.aux32 + orow * pr.ld_aux : nullptr;
-      r.mask_row = (FULL && pr.mask16) ? pr.mask16 + orow * pr.ld_mask : nullptr;
-      r.add_row = pr.addtab ? pr.addtab + (size_t)m * pr.ld_addtab : nullptr;
-      r.o32_row = pr.out32 ? pr.out32 + orow * pr.ld32 : nullptr;
-      r.o32i_row = ((FULL || SPLIT) && pr.out32_id) ? pr.out32_id + (size_t)m * pr.ld32_id : nullptr;
-      r.o16_row = pr.out16 ? pr.out16 + orow * pr.ld16 : nullptr;
-      r.o16p_row = pr.out16p ? pr.out16p + orow * pr.ld16 : nullptr;
-      r.pre_row = (FULL && pr.pre32) ? pr.pre32 + orow * pr.ld_pre : nullptr;
-      r.dact_row = (FULL && pr.dact16) ? pr.dact16 + orow * pr.ld_dact : nullptr;
-      const float* __restrict__ bias = (ti.split == 0) ? pr.bias : nullptr;
-      const int nt0 = ti.n_blk * BN;
-#pragma unroll
-      for (int cc = 0; cc < 8; ++cc) {
-        if (cc * 32 < BN && nt0 + cc * 32 < pN) {  // warpgroup-uniform
-#pragma unroll
-          for (int ii = 0; ii < 4; ++ii) {
-            const int i = 4 * cc + ii;
-            *reinterpret_cast<float2*>(ebuf + fr * Cfg::kEpiStride + 8 * ii + fc) = make_float2(acc[4 * i], acc[4 * i + 1]);
-            *reinterpret_cast<float2*>(ebuf + (fr + 8) * Cfg::kEpiStride + 8 * ii + fc) = make_float2(acc[4 * i + 2], acc[4 * i + 3]);
-          }
-          named_bar_sync(1 + cw, 128);
-          const int n0 = nt0 + cc * 32 + ehalf * 16;
-          if (cc * 32 + ehalf * 16 < BN && n0 < pN) {  // warp-uniform (a warp's rows share ehalf)
-            float v[16];
-            ld16f(ebuf + erow * Cfg::kEpiStride + ehalf * 16, v);
-            if (bias != nullptr) {
-#pragma unroll
-              for (int j = 0; j < 16; ++j) v[j] += (n0 + j < pN) ? __ldg(bias + n0 + j) : 0.f;
-            }
-            epi_step<FULL, SPLIT>(pr, r, v, n0, fmt, lane, g.lo16);
-          }
-          named_bar_sync(1 + cw, 128);
-        }
-      }
-      if (tid == 0 && cw == 1) stamp(g.dbg, 6);  // epilogue of the tile done (second warpgroup)
+    // warpgroup wg computes rows [64 wg, 64 wg + 64) of each tile.  The host accepts multiples of 16 in [32, 256] (of 32 in
+    // clusters), so only those widths are compiled.
+    Ring ring{stage_base, full_bar, empty_bar, kStageBytes, kStages, 0, 0u};
+    switch (BN >> 4) {
+#define UV_BN_CASE(k) \
+  case k: consumer_tiles<CL, FULL, SPLIT, 16 * k>(g, ring, epi_buf, tile0, tstep, crank, wg, lane); break;
+#define UV_BN_CASE_ODD(k) \
+  case k: if constexpr (CL == 1) consumer_tiles<CL, FULL, SPLIT, 16 * k>(g, ring, epi_buf, tile0, tstep, crank, wg, lane); break;
+      UV_BN_CASE(2) UV_BN_CASE_ODD(3) UV_BN_CASE(4) UV_BN_CASE_ODD(5) UV_BN_CASE(6) UV_BN_CASE_ODD(7) UV_BN_CASE(8)
+      UV_BN_CASE_ODD(9) UV_BN_CASE(10) UV_BN_CASE_ODD(11) UV_BN_CASE(12) UV_BN_CASE_ODD(13) UV_BN_CASE(14) UV_BN_CASE_ODD(15)
+      UV_BN_CASE(16)
+#undef UV_BN_CASE_ODD
+#undef UV_BN_CASE
+      default: __trap();  // launch_gemm_group rejects every other width; without consumers the producer would wait forever
     }
   }
 
