@@ -453,6 +453,58 @@ int univtg_op_attention_bwd(const void* qkv, const void* dO, const void* O, cons
                             float* delta_ws, float* dqkv32, int32_t B, int32_t L, int32_t H, int32_t dh, int32_t fmt_act,
                             int32_t impl, void* stream);
 
+/* ---- CLIP feature extraction (inference only): the ViT image tower and the text tower of OpenAI CLIP
+ * (reference run_on_video/clip/model.py: VisualTransformer 202-236, encode_text 339-352), which produce the video and query
+ * features the grounding model consumes.  Every head is 64 wide (heads = width / 64, model.py:268); LayerNorm eps 1e-5. ---- */
+typedef struct univtg_clip_config {
+  int32_t embed_dim;         /* text_projection.shape[1] = visual.proj.shape[1]; multiple of 16 */
+  int32_t vision_width;      /* visual.conv1.weight.shape[0]; multiple of 64, <= 1024 */
+  int32_t vision_layers;     /* visual.transformer.resblocks.* count, 1..64 */
+  int32_t patch_size;        /* visual.conv1.weight.shape[-1] (P) */
+  int32_t image_resolution;  /* R = P * grid; frames are R x R */
+  int32_t text_width;        /* ln_final.weight.shape[0]; multiple of 64, <= 1024 */
+  int32_t text_layers;       /* transformer.resblocks.* count, 1..64 */
+  int32_t context_length;    /* positional_embedding.shape[0]; tokens are [n, context_length] */
+  int32_t vocab_size;        /* token_embedding.weight.shape[0] */
+  int32_t operand_format;    /* 0 fp16, 1 bf16 GEMM / attention operands (fp32 accumulation, LayerNorm and residual stream);
+                              * 2 (fp16x3) is refused */
+} univtg_clip_config;
+/* Number of parameter tensors univtg_clip_pack_weights expects, in this order (reference state_dict names):
+ *   visual.{conv1.weight, class_embedding, positional_embedding, ln_pre.weight, ln_pre.bias},
+ *   for l < vision_layers: visual.transformer.resblocks.l.{attn.in_proj_weight, attn.in_proj_bias, attn.out_proj.weight,
+ *        attn.out_proj.bias, ln_1.weight, ln_1.bias, mlp.c_fc.weight, mlp.c_fc.bias, mlp.c_proj.weight, mlp.c_proj.bias,
+ *        ln_2.weight, ln_2.bias},
+ *   visual.{ln_post.weight, ln_post.bias, proj},
+ *   token_embedding.weight, positional_embedding, for l < text_layers: transformer.resblocks.l.{same twelve},
+ *   ln_final.weight, ln_final.bias, text_projection */
+int univtg_clip_num_params(const univtg_clip_config* cfg);
+size_t univtg_clip_packed_bytes(const univtg_clip_config* cfg);
+/* params: HOST array of device pointers, contiguous tensors of element type src_dtype (0 f32, 1 fp16: released CLIP checkpoints
+ * are mostly fp16).  Matrices become 16-bit GEMM operands; visual.proj and text_projection are stored transposed. */
+int univtg_clip_pack_weights(const univtg_clip_config* cfg, const void* const* params, int32_t n_params, int32_t src_dtype,
+                             void* packed, void* stream);
+/* Workspace bytes for encoding up to n_images frames and up to n_texts token rows of text_len positions (either count may be 0).
+ * The two towers share one workspace: calls on one stream may reuse it. */
+size_t univtg_clip_workspace_bytes(const univtg_clip_config* cfg, int32_t n_images, int32_t n_texts, int32_t text_len);
+/* encode_image of n frames -> out [n, embed_dim] f32.
+ *   pixel_kind 0: uint8 [n, R, R, 3] RGB (ffmpeg rgb24); normalised in-kernel as run_on_video/preprocessing.py does:
+ *                 (x / 255 - mean[c]) / (std[c] + 1e-8) with CLIP's mean and std.
+ *   pixel_kind 1: f32 [n, 3, R, R], already normalised (encode_image's own input).
+ * n (frames here, token rows in univtg_clip_encode_text) is at most 65535 per call. */
+int univtg_clip_encode_image(const univtg_clip_config* cfg, const void* packed, const void* pixels, int32_t pixel_kind, int32_t n,
+                             void* ws, size_t ws_bytes, float* out, void* stream);
+/* encode_text of n token rows: tokens [n, context_length] int64 (clip.tokenize ids).  Only positions < ctx_used are computed:
+ * the causal mask makes them independent of later tokens, so ctx_used = context_length is the reference's encode_text and a
+ * smaller ctx_used that still covers every row's argmax (EOT) gives the same rows.  last_hidden (nullable): [n, ctx_used, text_width]
+ * f32 = ln_final(x); pooled (nullable): [n, embed_dim] f32 = ln_final(x)[argmax(tokens)] @ text_projection.  The tokens are read
+ * back to the host and checked before anything launches (ids in [0, vocab_size), argmax < ctx_used): the call synchronises
+ * `stream` once. */
+int univtg_clip_encode_text(const univtg_clip_config* cfg, const void* packed, const int64_t* tokens, int32_t n, int32_t ctx_used,
+                            void* ws, size_t ws_bytes, float* last_hidden, float* pooled, void* stream);
+/* Kernels one call launches: tower 0 = univtg_clip_encode_image, 1 = univtg_clip_encode_text with text_outputs bit 0 = last_hidden,
+ * bit 1 = pooled. */
+int univtg_clip_num_launches(const univtg_clip_config* cfg, int32_t tower, int32_t text_outputs);
+
 #ifdef __cplusplus
 }
 #endif

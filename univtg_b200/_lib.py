@@ -87,6 +87,13 @@ class TxtPosBwd(ctypes.Structure):
         [("pgrad_scale", c_float), ("B", c_int), ("Lt", c_int), ("L", c_int), ("Lv", c_int), ("d", c_int)]
 
 
+class ClipConfig(ctypes.Structure):
+    """univtg_clip_config."""
+
+    _fields_ = [(n, c_int) for n in ("embed_dim", "vision_width", "vision_layers", "patch_size", "image_resolution", "text_width",
+                                     "text_layers", "context_length", "vocab_size", "operand_format")]
+
+
 # symbol -> (restype, argtypes); every symbol declared in include/univtg_b200.h must be listed here
 SIGNATURES = {
     "univtg_last_error": (ctypes.c_char_p, []),
@@ -155,6 +162,15 @@ SIGNATURES = {
     "univtg_op_attention": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int,
                                     c_void_p]),
     "univtg_op_attention_bwd": (c_int, [c_void_p] * 7 + [c_int, c_int, c_int, c_int, c_int, c_int, c_void_p]),
+    "univtg_clip_num_params": (c_int, [ctypes.POINTER(ClipConfig)]),
+    "univtg_clip_packed_bytes": (c_size_t, [ctypes.POINTER(ClipConfig)]),
+    "univtg_clip_pack_weights": (c_int, [ctypes.POINTER(ClipConfig), ctypes.POINTER(c_void_p), c_int, c_int, c_void_p, c_void_p]),
+    "univtg_clip_workspace_bytes": (c_size_t, [ctypes.POINTER(ClipConfig), c_int, c_int, c_int]),
+    "univtg_clip_encode_image": (c_int, [ctypes.POINTER(ClipConfig), c_void_p, c_void_p, c_int, c_int, c_void_p, c_size_t, c_void_p,
+                                         c_void_p]),
+    "univtg_clip_encode_text": (c_int, [ctypes.POINTER(ClipConfig), c_void_p, c_void_p, c_int, c_int, c_void_p, c_size_t, c_void_p,
+                                        c_void_p, c_void_p]),
+    "univtg_clip_num_launches": (c_int, [ctypes.POINTER(ClipConfig), c_int, c_int]),
 }
 
 

@@ -42,8 +42,10 @@ __device__ __forceinline__ float quad_sum(float v) {
 
 // DROP = 1: attention dropout.  The multipliers of the tile are generated while the S product runs (one Philox call per 8
 // elements) and kept as keep-bits; P o M is what feeds P V, while the row sum, the running max and lse stay un-dropped.
-template <int DH, int BF, int DROP>
-__global__ void __launch_bounds__(256, 1) attention_wgmma_kernel(const __grid_constant__ AttnArgs a) {
+// CAUSAL = 1: query row i sees keys j <= i only (the additive triu(-inf) mask of CLIP's text transformer).  Key tiles that lie
+// wholly above the diagonal are not loaded, and masked scores enter the softmax as -inf, so they contribute exactly 0.
+template <int DH, int BF, int DROP, int CAUSAL>
+__device__ __forceinline__ void attention_tile(const AttnArgs& a) {
   using Cfg = AttnCfg<DH>;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw_addr = smem_u32(smem_raw);
@@ -65,7 +67,7 @@ __global__ void __launch_bounds__(256, 1) attention_wgmma_kernel(const __grid_co
   const int h = blockIdx.y;
   const int b = blockIdx.z;
   const int L = a.L;
-  const int num_kv = (L + 127) / 128;
+  const int num_kv = CAUSAL ? min((L + 127) / 128, q0 / 128 + 1) : (L + 127) / 128;
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&a.tm_qkv);
@@ -150,7 +152,10 @@ __global__ void __launch_bounds__(256, 1) attention_wgmma_kernel(const __grid_co
     for (int i = 0; i < 16; ++i) {
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
-        const float x = sacc[4 * i + e] * kLog2e + bias[8 * i + fc + (e & 1)];
+        float x = sacc[4 * i + e] * kLog2e + bias[8 * i + fc + (e & 1)];
+        if constexpr (CAUSAL != 0) {
+          if (j * 128 + 8 * i + fc + (e & 1) > q0 + wg * 64 + fr + 8 * (e >> 1)) x = -INFINITY;
+        }
         sacc[4 * i + e] = x;
         mx[e >> 1] = fmaxf(mx[e >> 1], x);
       }
@@ -216,6 +221,17 @@ __global__ void __launch_bounds__(256, 1) attention_wgmma_kernel(const __grid_co
       if (a.lse && (lane & 3) == 0) a.lse[((size_t)b * a.H + h) * L + qi] = m_run[r] * 0.6931471805599453f + logf(l);
     }
   }
+}
+
+template <int DH, int BF, int DROP>
+__global__ void __launch_bounds__(256, 1) attention_wgmma_kernel(const __grid_constant__ AttnArgs a) {
+  attention_tile<DH, BF, DROP, 0>(a);
+}
+
+// dh = 64 with the causal mask (inference, no dropout): CLIP's text transformer.
+template <int BF>
+__global__ void __launch_bounds__(256, 1) attention_wgmma_causal_kernel(const __grid_constant__ AttnArgs a) {
+  attention_tile<64, BF, 0, 1>(a);
 }
 
 // fp16x3 attention (inference, no dropout).  tm_qkv is a plane pair; S takes Q_hi K_hi + Q_lo K_hi + Q_hi K_lo, P is split in registers
@@ -495,6 +511,25 @@ static int launch_tc(const AttnArgs& a, cudaStream_t stream) {
   return (int)e;
 }
 
+template <int BF>
+static int launch_tc_causal(const AttnArgs& a, cudaStream_t stream) {
+  using Cfg = AttnCfg<64>;
+  static bool attr_set = false;
+  if (!attr_set) {
+    cudaError_t e = cudaFuncSetAttribute(attention_wgmma_causal_kernel<BF>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes);
+    if (e != cudaSuccess) {
+      set_error("cudaFuncSetAttribute(attention, causal): %s", cudaGetErrorString(e));
+      return (int)e;
+    }
+    attr_set = true;
+  }
+  dim3 grid((a.L + 127) / 128, a.H, a.B);
+  launch_k(attention_wgmma_causal_kernel<BF>, dim3(grid), dim3(256), Cfg::kSmemBytes, stream, a);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) set_error("attention launch failed: %s", cudaGetErrorString(e));
+  return (int)e;
+}
+
 template <int DH>
 static int launch_tc_split(const AttnArgs& a, cudaStream_t stream) {
   using Cfg = AttnCfg<DH, true>;
@@ -542,6 +577,13 @@ int launch_attention_simt(const AttnArgs& a, const uint16_t* qkv, cudaStream_t s
 }
 
 int launch_attention(const AttnArgs& a, cudaStream_t stream) {
+  if (a.causal) {
+    if (a.dh != 64 || a.split || a.drop.on) {
+      set_error("launch_attention: the causal mask needs dh = 64, fp16 or bf16 operands and no dropout");
+      return (int)cudaErrorInvalidValue;
+    }
+    return a.fmt ? launch_tc_causal<1>(a, stream) : launch_tc_causal<0>(a, stream);
+  }
   if (a.split) {
     if (a.fmt != 0 || a.drop.on) {
       set_error("launch_attention: fp16x3 needs fmt 0 and no dropout");

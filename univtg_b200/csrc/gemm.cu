@@ -262,6 +262,9 @@ __device__ __forceinline__ void epi_step(const GemmProblem& pr, const EpiRow& r,
   } else if (act == ACT_RELU) {
 #pragma unroll
     for (int j = 0; j < 16; ++j) v[j] = fmaxf(v[j], 0.f) * rsc;
+  } else if (act == ACT_QUICKGELU) {
+#pragma unroll
+    for (int j = 0; j < 16; ++j) v[j] = v[j] / (1.f + expf(-1.702f * v[j])) * rsc;
   } else {
 #pragma unroll
     for (int j = 0; j < 16; ++j) v[j] *= rsc;

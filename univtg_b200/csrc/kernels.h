@@ -11,7 +11,7 @@ constexpr int GEMM_BM = 128;  // tile rows: two consumer warpgroups of wgmma M =
 constexpr int GEMM_BK = 64;   // one 128-byte swizzle span of 16-bit elements
 constexpr int GEMM_MAX_GROUP = 4;
 
-enum Act { ACT_NONE = 0, ACT_RELU = 1, ACT_GELU = 2 };
+enum Act { ACT_NONE = 0, ACT_RELU = 1, ACT_GELU = 2, ACT_QUICKGELU = 3 };  // QuickGELU: x * sigmoid(1.702 x) (CLIP MLP)
 
 // TMA coordinate rule of one operand for the k-block (tap, kk) of the output tile whose first
 // row (A) / first column (B) is `mn0`:

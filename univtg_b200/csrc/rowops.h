@@ -107,6 +107,7 @@ struct AttnArgs {
   DropSpec drop;          // attention dropout (drop.on; stream = encoder layer): P o M feeds P V, the row sum and lse stay un-dropped
   int split;              // 1: fp16x3 (fmt 0, no dropout): qkv and out are hi / lo pairs; tm_qkv is then a make_tmap_split pair
   long long lo_qkv, lo_out;  // split: elements from qkv / out to their lo planes
+  int causal;             // 1: query i attends to keys j <= i only (dh = 64, tensor cores, no dropout, no split)
 };
 int launch_attention(const AttnArgs& a, cudaStream_t stream);
 // SIMT variant for head sizes outside {64,128}; reads qkv through a plain pointer.

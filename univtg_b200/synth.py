@@ -197,3 +197,98 @@ def flops_forward(cfg, batch=None, l_vid=None, l_txt=None):
     proj = 2 * Lv * (cfg["v_feat_dim"] * d + d * d) + 2 * Lt * (cfg["t_feat_dim"] * d + d * d)
     heads = 8 * Lv * 3 * d * d + 18 * Lv * d
     return B * (enc + proj + heads), B * enc
+
+
+# CLIP (run_on_video/clip/model.py) shapes: ViT-B/32 as the reference's feature extractor loads it, and two small ones for goldens
+CLIP_CONFIGS = {
+    "vit_b32": dict(embed_dim=512, vision_width=768, vision_layers=12, patch_size=32, image_resolution=224, text_width=512,
+                    text_layers=12, context_length=77, vocab_size=49408),
+    "small224": dict(embed_dim=64, vision_width=128, vision_layers=2, patch_size=32, image_resolution=224, text_width=128,
+                     text_layers=2, context_length=77, vocab_size=49408),
+    "small64": dict(embed_dim=64, vision_width=64, vision_layers=2, patch_size=16, image_resolution=64, text_width=64,
+                    text_layers=2, context_length=77, vocab_size=49408),
+}
+CLIP_SOT, CLIP_EOT = 49406, 49407  # <|startoftext|>, <|endoftext|> of clip.tokenize (the largest ids: argmax finds EOT)
+
+
+def clip_state_dict_shapes(cfg):
+    """Key -> shape of a ViT CLIP state dict (model.py:202-291), in the reference module's registration order."""
+    Wv, Wt, E, P = cfg["vision_width"], cfg["text_width"], cfg["embed_dim"], cfg["patch_size"]
+    grid = cfg["image_resolution"] // P
+
+    def blocks(pre, W, n):
+        out = {}
+        for l in range(n):
+            p = f"{pre}resblocks.{l}."
+            out.update({p + "attn.in_proj_weight": (3 * W, W), p + "attn.in_proj_bias": (3 * W,), p + "attn.out_proj.weight": (W, W),
+                        p + "attn.out_proj.bias": (W,), p + "ln_1.weight": (W,), p + "ln_1.bias": (W,), p + "mlp.c_fc.weight": (4 * W, W),
+                        p + "mlp.c_fc.bias": (4 * W,), p + "mlp.c_proj.weight": (W, 4 * W), p + "mlp.c_proj.bias": (W,),
+                        p + "ln_2.weight": (W,), p + "ln_2.bias": (W,)})
+        return out
+
+    s = {"positional_embedding": (cfg["context_length"], Wt), "text_projection": (Wt, E), "logit_scale": (),
+         "visual.class_embedding": (Wv,), "visual.positional_embedding": (grid * grid + 1, Wv), "visual.proj": (Wv, E),
+         "visual.conv1.weight": (Wv, 3, P, P), "visual.ln_pre.weight": (Wv,), "visual.ln_pre.bias": (Wv,)}
+    s.update(blocks("visual.transformer.", Wv, cfg["vision_layers"]))
+    s.update({"visual.ln_post.weight": (Wv,), "visual.ln_post.bias": (Wv,)})
+    s.update(blocks("transformer.", Wt, cfg["text_layers"]))
+    s.update({"token_embedding.weight": (cfg["vocab_size"], Wt), "ln_final.weight": (Wt,), "ln_final.bias": (Wt,)})
+    return s
+
+
+def make_clip_state_dict(cfg, seed=0, dtype=torch.float32):
+    """Seeded ViT CLIP weights with the reference's keys and shapes and CLIP's init scales (model.py:209-217, 295-322), plus
+    non-trivial LayerNorm affine terms and biases.  Like released checkpoints it carries the integer entries input_resolution,
+    context_length and vocab_size."""
+    g = torch.Generator(device="cpu").manual_seed(seed)
+    sd = {}
+    for k, shp in clip_state_dict_shapes(cfg).items():
+        if k == "logit_scale":
+            t = torch.tensor(math.log(1 / 0.07))
+        elif len(shp) == 1 and k.endswith(".weight"):  # LayerNorm scales
+            t = 1.0 + 0.1 * torch.randn(shp, generator=g)
+        elif len(shp) == 1 and k != "visual.class_embedding":
+            t = 0.05 * torch.randn(shp, generator=g)
+        elif k == "token_embedding.weight":
+            t = 0.02 * torch.randn(shp, generator=g)
+        elif k == "positional_embedding":
+            t = 0.01 * torch.randn(shp, generator=g)
+        elif k in ("visual.class_embedding", "visual.positional_embedding", "visual.proj"):
+            t = cfg["vision_width"] ** -0.5 * torch.randn(shp, generator=g)
+        elif k == "text_projection":
+            t = cfg["text_width"] ** -0.5 * torch.randn(shp, generator=g)
+        elif k == "visual.conv1.weight":
+            t = (3 * cfg["patch_size"] ** 2) ** -0.5 * torch.randn(shp, generator=g)
+        else:  # block matrices: in_proj / c_fc std width^-0.5, out_proj / c_proj scaled down with depth
+            Wd = shp[1] if "c_proj" not in k else shp[0]
+            n = cfg["vision_layers"] if k.startswith("visual.") else cfg["text_layers"]
+            std = Wd ** -0.5 * ((2 * n) ** -0.5 if ("out_proj" in k or "c_proj" in k) else 1.0)
+            t = std * torch.randn(shp, generator=g)
+        sd[k] = t.to(dtype)
+    sd["input_resolution"] = torch.tensor(cfg["image_resolution"])
+    sd["context_length"] = torch.tensor(cfg["context_length"])
+    sd["vocab_size"] = torch.tensor(cfg["vocab_size"])
+    return sd
+
+
+def make_clip_frames(cfg, n, seed=1):
+    """uint8 [n, R, R, 3] RGB frames (smooth gradients plus noise, like decoded video rather than white noise)."""
+    g = torch.Generator(device="cpu").manual_seed(seed)
+    R = cfg["image_resolution"]
+    yy, xx = torch.meshgrid(torch.linspace(0, 1, R), torch.linspace(0, 1, R), indexing="ij")
+    ph = torch.rand(n, 3, generator=g)
+    base = 0.5 + 0.35 * torch.sin(6.0 * (yy[None, None] * ph[:, :, None, None] + xx[None, None] * (1 - ph[:, :, None, None])) + 6.0 * ph[:, :, None, None])
+    x = base + 0.1 * torch.randn(n, 3, R, R, generator=g)
+    return (x.clamp(0, 1) * 255).round().to(torch.uint8).permute(0, 2, 3, 1).contiguous()
+
+
+def make_clip_tokens(cfg, lengths, seed=2):
+    """int64 [len(lengths), context_length] clip.tokenize-shaped rows: SOT, lengths[i] - 2 word ids, EOT, zero padding."""
+    g = torch.Generator(device="cpu").manual_seed(seed)
+    out = torch.zeros(len(lengths), cfg["context_length"], dtype=torch.int64)
+    for i, n in enumerate(lengths):
+        assert 2 <= n <= cfg["context_length"]
+        out[i, 0] = CLIP_SOT
+        out[i, 1:n - 1] = torch.randint(1, CLIP_SOT, (n - 2,), generator=g)
+        out[i, n - 1] = CLIP_EOT
+    return out
