@@ -200,6 +200,23 @@ int univtg_loss_backward(const float* w5, const float* vid_mem_proj, const float
                          int32_t B, int32_t Lv, int32_t d, const void* scratch, float* d_logits, float* d_spans,
                          float* d_vid_mem_proj, float* d_txt_mem_proj, void* stream);
 
+/* SetCriterion for model_id=univtg_qfvs (reference model/univtg_qfvs.py:215-261, 358-377), query-focused video summarisation.
+ * The outputs of one forward over B = max_segment_num segments of Lv = max_frame_num frames are read as N = B * Lv flat positions.
+ * Position i is kept iff mask_gt[i] (bool bytes, [N]); the k-th kept position pairs with saliency_scores[k] (row 0 of the
+ * targets, at least N entries; entries at or beyond the kept count are ignored).  losses5 as univtg_loss_forward:
+ *   loss_f       = sum over kept of BCE(pred_logits, t) (logs clamped at -100) / sum(t)
+ *   loss_s_intra = -mean over kept t > 0 of log softmax(z), over all kept positions; z = (cos(vid_mem_proj, txt_mem_proj)
+ *                  + log(src_vid_mask + 1e-45)) / temperature, i.e. the model's saliency_scores / temperature
+ *   loss_b = loss_g = loss_s_inter = 0.  loss_f and loss_s_intra are 0 when sum(t) == 0, loss_s_intra also when
+ *   has_pos_labels == 0; their gradients are then 0.  No host synchronisation.  `scratch`: univtg_loss_scratch_bytes(B, Lv). */
+int univtg_qfvs_loss_forward(const float* pred_logits, const float* vid_mem_proj, const float* txt_mem_proj, const float* src_vid_mask,
+                             const uint8_t* mask_gt, const float* saliency_scores, int32_t has_pos_labels, int32_t B, int32_t Lv,
+                             int32_t d, float temperature, float* losses5, void* scratch, void* stream);
+/* w5: device fp32 [5] = dL/d(loss_k).  Writes d pred_logits [N], d vid_mem_proj [B, Lv, d] and d txt_mem_proj [B, d];
+ * pred_spans gets no gradient.  Overwrites the span-gradient part of `scratch`. */
+int univtg_qfvs_loss_backward(const float* w5, const float* vid_mem_proj, const float* txt_mem_proj, int32_t B, int32_t Lv,
+                              int32_t d, void* scratch, float* d_logits, float* d_vid_mem_proj, float* d_txt_mem_proj, void* stream);
+
 /* Number of kernels one univtg_forward launches (for bench accounting). */
 int univtg_forward_num_launches(const univtg_plan* plan);
 /* Kernels this library has launched since it was loaded (every launch of every entry point; memsets / memcpys not counted). */

@@ -129,7 +129,10 @@ SIGNATURES = {
     "univtg_loss_forward": (c_int, [c_void_p] * 10 + [c_int, c_int, c_int, c_float, c_float, c_void_p, c_void_p, c_void_p]),
     "univtg_loss_backward": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
                                      c_void_p, c_void_p, c_void_p]),
-    "univtg_backward_stages": (c_int, [ctypes.POINTER(Config), c_void_p, c_int]),
+    "univtg_qfvs_loss_forward": (c_int, [c_void_p] * 6 + [c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p, c_void_p]),
+    "univtg_qfvs_loss_backward": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
+                                          c_void_p]),
+    "univtg_backward_stages":(c_int, [ctypes.POINTER(Config), c_void_p, c_int]),
     "univtg_plan_set_grad_events": (c_int, [c_void_p, ctypes.POINTER(c_void_p), c_int]),
     "univtg_plan_set_backward_sm_budget": (c_int, [c_void_p, c_int]),
     "univtg_decode_mr": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,

@@ -260,6 +260,130 @@ int launch_loss_forward(const LossArgs& a, cudaStream_t stream) {
 }
 
 // ------------------------------------------------------------------------------------------------
+// QFVS criterion (reference model/univtg_qfvs.py:215-261, 358-377), one block, any N = B * Lv.
+//   kept positions: i with mask_gt[i]; the k-th kept position (k = exclusive prefix count of mask_gt) pairs with t = sal[k]
+//   loss_f        sum over kept of BCE(pred_logits, t) (log clamped at -100) / sum(t)
+//   loss_s_intra  -mean over kept positions with t > 0 of log softmax(z), the softmax over all kept positions
+//   z[i] = (cos_in[i] + log(vmask[i] + 1e-45)) / tau: the model's saliency_scores / tau
+// Both are 0 when sum(t) == 0, loss_s_intra also without saliency_pos_labels; their gradients are then exactly 0.
+// ------------------------------------------------------------------------------------------------
+__device__ __forceinline__ float block_max(float v, float* s_red) {
+  v = warp_max(v);
+  __syncthreads();
+  if ((threadIdx.x & 31) == 0) s_red[threadIdx.x >> 5] = v;
+  __syncthreads();
+  float t = -INFINITY;
+  const int nw = blockDim.x >> 5;
+  for (int i = 0; i < nw; ++i) t = fmaxf(t, s_red[i]);
+  return t;
+}
+
+__global__ void __launch_bounds__(1024) qfvs_loss_kernel(const QfvsLossArgs a) {
+  pdl_prologue();
+  __shared__ float s_red[32];
+  __shared__ int s_cnt[32];
+  const int tid = threadIdx.x, nt = blockDim.x, lane = tid & 31, warp = tid >> 5, nw = nt >> 5;
+  const int n = a.B * a.Lv;
+  const float inv_tau = 1.0f / a.temperature;
+  // pass 1, in chunks of nt positions: ranks, target sum, positive count, BCE sum, sum of z over positives and a running
+  // (max, sum of exp) of z per thread.  Each thread parks t (0 when not kept) in g_logits_f[i] and the keep flag in g_cos_in[i]
+  // for pass 2, which visits the same i with the same thread.
+  int ranked = 0;  // kept positions in earlier chunks
+  float c_t = 0.f, c_pos = 0.f, c_bce = 0.f, c_zpos = 0.f, mx = -INFINITY, se = 0.f;
+  for (int base = 0; base < n; base += nt) {
+    const int i = base + tid;
+    const bool keep = i < n && a.mask_gt[i] != 0;
+    const unsigned bal = __ballot_sync(0xffffffffu, keep);
+    if (lane == 0) s_cnt[warp] = __popc(bal);
+    __syncthreads();
+    int before = 0, total = 0;
+    for (int w = 0; w < nw; ++w) {
+      const int c = s_cnt[w];
+      before += w < warp ? c : 0;
+      total += c;
+    }
+    __syncthreads();  // s_cnt is rewritten by the next chunk
+    if (i < n) {
+      float t = 0.f;
+      if (keep) {
+        t = a.sal[ranked + before + __popc(bal & ((1u << lane) - 1u))];
+        const float p = a.pred_logits[i];
+        const float lp = fmaxf(logf(p), -100.f), l1p = fmaxf(logf(1.f - p), -100.f);
+        c_t += t;
+        c_bce += -(t * lp + (1.f - t) * l1p);
+        const float z = (a.cos_in[i] + logf(a.vmask[i] + 1e-45f)) * inv_tau;
+        if (t > 0.f) {
+          c_pos += 1.f;
+          c_zpos += z;
+        }
+        if (z > mx) {
+          se = se * expf(mx - z) + 1.f;
+          mx = z;
+        } else {
+          se += expf(z - mx);
+        }
+      }
+      a.g_logits_f[i] = t;
+      a.g_cos_in[i] = keep ? 1.f : 0.f;
+    }
+    ranked += total;
+  }
+  const float sum_t = block_sum(c_t, s_red);
+  const float n_pos = block_sum(c_pos, s_red);
+  const float bce = block_sum(c_bce, s_red);
+  const float zpos = block_sum(c_zpos, s_red);
+  const float zmax = block_max(mx, s_red);
+  const float lse = zmax + logf(block_sum(mx == -INFINITY ? 0.f : se * expf(mx - zmax), s_red));
+  const bool on = sum_t != 0.f;          // reference: `if saliency_scores.sum() == 0: return 0.`
+  const bool sal_on = on && a.has_pos != 0;
+  // pass 2: unit gradients d loss_f / d pred_logits (torch's BCE backward) and d loss_s_intra / d cos_in
+  for (int i = tid; i < n; i += nt) {
+    const float t = a.g_logits_f[i];
+    const bool keep = a.g_cos_in[i] != 0.f;
+    float gf = 0.f, gc = 0.f;
+    if (keep && on) {
+      const float p = a.pred_logits[i];
+      gf = (p - t) / fmaxf(p * (1.f - p), 1e-12f) / sum_t;
+    }
+    if (keep && sal_on) {
+      const float z = (a.cos_in[i] + logf(a.vmask[i] + 1e-45f)) * inv_tau;
+      gc = (expf(z - lse) - (t > 0.f ? 1.f / n_pos : 0.f)) * inv_tau;
+    }
+    a.g_logits_f[i] = gf;
+    a.g_cos_in[i] = gc;
+    a.g_spans_b[2 * i] = 0.f;
+    a.g_spans_b[2 * i + 1] = 0.f;
+    a.g_spans_g[2 * i] = 0.f;
+    a.g_spans_g[2 * i + 1] = 0.f;
+  }
+  if (tid == 0) {
+    a.losses[0] = 0.f;
+    a.losses[1] = 0.f;
+    a.losses[2] = on ? bce / sum_t : 0.f;
+    a.losses[3] = 0.f;
+    a.losses[4] = sal_on ? lse - zpos / n_pos : 0.f;
+  }
+}
+
+int launch_qfvs_loss_forward(const QfvsLossArgs& q, cudaStream_t stream) {
+  // cosines through loss_cos_kernel with one warp per block: every warp index is below B * Lv, so its B x B part never runs
+  LossArgs c = {};
+  c.xv = q.xv;
+  c.xt = q.xt;
+  c.B = q.B;
+  c.Lv = q.Lv;
+  c.d = q.d;
+  c.cos_in = q.cos_in;
+  c.vnorm = q.vnorm;
+  c.tnorm = q.tnorm;
+  launch_k(loss_cos_kernel, dim3(q.B * q.Lv), dim3(32), 0, stream, c);
+  launch_k(qfvs_loss_kernel, dim3(1), dim3(1024), 0, stream, q);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) set_error("qfvs loss forward launch failed: %s", cudaGetErrorString(e));
+  return (int)e;
+}
+
+// ------------------------------------------------------------------------------------------------
 // backward: weights w[5] (dL/d loss_k) -> gradients of the model outputs.
 //   d cos(u, v)/du = v / (|u||v|) - cos * u / |u|^2
 // ------------------------------------------------------------------------------------------------
@@ -382,6 +506,16 @@ int launch_loss_backward(const LossBwdArgs& a, cudaStream_t stream) {
   launch_k(loss_bwd_txt_kernel, dim3(a.B, (a.d + 127) / 128), dim3(128), (size_t)(a.Lv + 2 * a.B) * sizeof(float), stream, a);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) set_error("loss backward launch failed: %s", cudaGetErrorString(e));
+  return (int)e;
+}
+
+int launch_qfvs_loss_backward(const LossBwdArgs& a, cudaStream_t stream) {
+  const int n = a.B * a.Lv;
+  launch_k(loss_bwd_small_kernel, dim3((n + 255) / 256), dim3(256), 0, stream, a);
+  launch_k(loss_bwd_vid_kernel, dim3((n * 32 + 255) / 256), dim3(256), (size_t)8 * a.B * sizeof(float), stream, a);
+  launch_k(loss_bwd_txt_kernel, dim3(a.B, (a.d + 127) / 128), dim3(128), (size_t)(a.Lv + 2 * a.B) * sizeof(float), stream, a);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) set_error("qfvs loss backward launch failed: %s", cudaGetErrorString(e));
   return (int)e;
 }
 

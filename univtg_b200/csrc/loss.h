@@ -56,4 +56,31 @@ struct LossBwdArgs {
 };
 int launch_loss_backward(const LossBwdArgs& a, cudaStream_t stream);
 
+// QFVS criterion (reference model/univtg_qfvs.py): outputs [B, Lv] flattened row-major to N = B * Lv positions.
+struct QfvsLossArgs {
+  const float* pred_logits;  // [N]
+  const float* xv;           // [B, Lv, d] vid_mem_proj
+  const float* xt;           // [B, d]     txt_mem_proj
+  const float* vmask;        // [N] src_vid_mask of the outputs
+  const uint8_t* mask_gt;    // [N] bool: position i is kept iff mask_gt[i]
+  const float* sal;          // row 0 of targets saliency_scores; entry k pairs with the k-th kept position (k < count <= N)
+  int has_pos;               // "saliency_pos_labels" in targets
+  float temperature;
+  int B, Lv, d;
+  // outputs: losses [5] as LossArgs; the rest is the LossArgs scratch (g_spans_* zeroed, g_logits_f, cos_in, vnorm, tnorm,
+  // g_cos_in written) so that the MR/HL backward kernels apply unchanged
+  float* losses;
+  float* g_spans_b;
+  float* g_spans_g;
+  float* g_logits_f;
+  float* cos_in;
+  float* vnorm;
+  float* tnorm;
+  float* g_cos_in;
+};
+int launch_qfvs_loss_forward(const QfvsLossArgs& a, cudaStream_t stream);
+// loss_bwd_small + loss_bwd_vid + loss_bwd_txt with pos_idx = null; unlike launch_loss_backward, the saliency term is never
+// skipped (the QFVS saliency loss needs no positive index)
+int launch_qfvs_loss_backward(const LossBwdArgs& a, cudaStream_t stream);
+
 }  // namespace uv

@@ -1314,4 +1314,82 @@ int univtg_loss_backward(const float* w5, const float* vid_mem_proj, const float
   return launch_loss_backward(a, (cudaStream_t)stream);
 }
 
+namespace {
+bool qfvs_loss_shape_ok(const char* fn, int32_t B, int32_t Lv, int32_t d) {
+  if (B < 1 || Lv < 1 || d < 4 || d % 4 != 0 || (int64_t)B * Lv > INT32_MAX / 32) {
+    set_error("%s: bad shape B %d, Lv %d, d %d (d must be a positive multiple of 4)", fn, B, Lv, d);
+    return false;
+  }
+  if ((size_t)(Lv + 2 * B) * sizeof(float) > 48 * 1024 || B > 1536) {  // dynamic shared memory of loss_bwd_txt / loss_bwd_vid
+    set_error("%s: B %d, Lv %d exceed the backward kernels' shared memory", fn, B, Lv);
+    return false;
+  }
+  return true;
+}
+}  // namespace
+
+int univtg_qfvs_loss_forward(const float* pred_logits, const float* vid_mem_proj, const float* txt_mem_proj, const float* src_vid_mask,
+                             const uint8_t* mask_gt, const float* saliency_scores, int32_t has_pos_labels, int32_t B, int32_t Lv,
+                             int32_t d, float temperature, float* losses5, void* scratch, void* stream) {
+  if (!pred_logits || !vid_mem_proj || !txt_mem_proj || !src_vid_mask || !mask_gt || !saliency_scores || !losses5 || !scratch) {
+    set_error("univtg_qfvs_loss_forward: null argument");
+    return 1;
+  }
+  if (!qfvs_loss_shape_ok("univtg_qfvs_loss_forward", B, Lv, d)) return 1;
+  const LossScratch s = make_loss_scratch(B, Lv, reinterpret_cast<uint8_t*>(scratch));
+  QfvsLossArgs a;
+  a.pred_logits = pred_logits;
+  a.xv = vid_mem_proj;
+  a.xt = txt_mem_proj;
+  a.vmask = src_vid_mask;
+  a.mask_gt = mask_gt;
+  a.sal = saliency_scores;
+  a.has_pos = has_pos_labels != 0;
+  a.temperature = temperature;
+  a.B = B;
+  a.Lv = Lv;
+  a.d = d;
+  a.losses = losses5;
+  a.g_spans_b = s.g_spans_b;
+  a.g_spans_g = s.g_spans_g;
+  a.g_logits_f = s.g_logits_f;
+  a.cos_in = s.cos_in;
+  a.vnorm = s.vnorm;
+  a.tnorm = s.tnorm;
+  a.g_cos_in = s.g_cos_in;
+  return launch_qfvs_loss_forward(a, (cudaStream_t)stream);
+}
+
+int univtg_qfvs_loss_backward(const float* w5, const float* vid_mem_proj, const float* txt_mem_proj, int32_t B, int32_t Lv,
+                              int32_t d, void* scratch, float* d_logits, float* d_vid_mem_proj, float* d_txt_mem_proj, void* stream) {
+  if (!w5 || !vid_mem_proj || !txt_mem_proj || !scratch || !d_logits || !d_vid_mem_proj || !d_txt_mem_proj) {
+    set_error("univtg_qfvs_loss_backward: null argument");
+    return 1;
+  }
+  if (!qfvs_loss_shape_ok("univtg_qfvs_loss_backward", B, Lv, d)) return 1;
+  const LossScratch s = make_loss_scratch(B, Lv, reinterpret_cast<uint8_t*>(scratch));
+  LossBwdArgs a;
+  a.w = w5;
+  a.g_spans_b = s.g_spans_b;
+  a.g_spans_g = s.g_spans_g;
+  a.g_logits_f = s.g_logits_f;
+  a.cos_in = s.cos_in;
+  a.vnorm = s.vnorm;
+  a.tnorm = s.tnorm;
+  a.sim = s.sim;
+  a.g_cos_in = s.g_cos_in;
+  a.g_sim = s.g_sim;
+  a.xv = vid_mem_proj;
+  a.xt = txt_mem_proj;
+  a.pos_idx = nullptr;
+  a.B = B;
+  a.Lv = Lv;
+  a.d = d;
+  a.d_logits = d_logits;
+  a.d_spans = s.g_spans_b;  // pred_spans takes no part in the QFVS losses: loss_bwd_small's (zero) span gradient lands in scratch
+  a.d_xv = d_vid_mem_proj;
+  a.d_xt = d_txt_mem_proj;
+  return launch_qfvs_loss_backward(a, (cudaStream_t)stream);
+}
+
 }  // extern "C"

@@ -55,11 +55,29 @@ def _f32(t, dev):
     return t.detach().to(device=dev, dtype=torch.float32).contiguous()
 
 
+def _check_target_shapes(crit, outputs, targets):
+    """The loss kernels index the dense targets as [B, Lv] (and [B, Lv, 2]) and saliency_pos_labels by sample: a target of
+    another shape would be read out of bounds, so it is refused here (shape metadata only, no device access)."""
+    B, Lv = outputs["pred_logits"].shape[:2]
+    dense = {"timestamp_mask": (B, Lv), "timestamp_window": (B, Lv)}
+    if "spans" in crit.losses:
+        dense.update(timestamp=(B, Lv, 2), span_labels_nn=(B, Lv, 2))
+    if "saliency" in crit.losses and "saliency_pos_labels" in targets and "saliency_scores" in targets:
+        dense["saliency_scores"] = (B, Lv)
+        pos = targets["saliency_pos_labels"]
+        if pos.dim() != 2 or pos.shape[0] != B or pos.shape[1] < 1:
+            raise ValueError(f"saliency_pos_labels must be [B, k >= 1] with B = {B} rows, got {list(pos.shape)}")
+    for k, shp in dense.items():
+        if tuple(targets[k].shape) != shp:
+            raise ValueError(f"target {k} must be {list(shp)} (B, Lv of pred_logits), got {list(targets[k].shape)}")
+
+
 def criterion_forward(crit, outputs, targets):
     """Returns the reference's loss dict (model/univtg.py:338-351).  Supported loss lists: the ones build_model produces for
     dset_type in {mr, vlp} without 'tal' (spans, labels, saliency) and {hl, vs} (labels, saliency)."""
     if "saliency_cls" in crit.losses:
         raise NotImplementedError("loss 'saliency_cls' ('tal' train_path) is outside the accelerated path")
+    _check_target_shapes(crit, outputs, targets)
     dev = outputs["pred_logits"].device
     if dev.type != "cuda":
         raise RuntimeError("univtg_b200: the criterion runs on CUDA tensors only (no CPU path)")

@@ -292,3 +292,57 @@ def make_clip_tokens(cfg, lengths, seed=2):
         out[i, 1:n - 1] = torch.randint(1, CLIP_SOT, (n - 2,), generator=g)
         out[i, n - 1] = CLIP_EOT
     return out
+
+
+# ---- query-focused video summarisation (main/dataset_qfvs.py) -------------------------------------------------------------
+def make_qfvs_item(cfg, seed, S, Lf, seg_len, L1, L2):
+    """One DatasetQFVS item (main/dataset_qfvs.py:125-208) with seeded contents: features [S, Lf, Dv - 2] zero beyond each
+    segment's seg_len (segments past len(seg_len) are empty), the [S, Lf] bool mask_GT, per-shot 0/1 targets over the first
+    sum(seg_len) shots of S * Lf entries (concept 1, concept 2 and the oracle summary), one positive shot index per target as
+    a [1] float tensor ([0] when there is none), and two L2-normalised concept embeddings [L1, Dt] / [L2, Dt]."""
+    g = torch.Generator(device="cpu").manual_seed(seed)
+    Dv, Dt = cfg["v_feat_dim"] - 2, cfg["t_feat_dim"]
+    seg_len = torch.tensor(list(seg_len), dtype=torch.int64)
+    mask = torch.zeros(S, Lf, dtype=torch.bool)
+    for j, n in enumerate(seg_len.tolist()):
+        mask[j, :n] = True
+    feats = torch.randn(S, Lf, Dv, generator=g)
+    feats = feats / (feats.norm(dim=-1, keepdim=True) + 1e-5) * mask[..., None]
+    count = int(seg_len.sum())
+    item = {"features": feats, "seg_len": seg_len, "mask_GT": mask}
+    for name, key in (("concept1_GT", "saliency_pos_labels_1"), ("concept2_GT", "saliency_pos_labels_2"),
+                      ("oracle_summary", "saliency_pos_labels_oracle")):
+        t = torch.zeros(S * Lf)
+        t[:count] = (torch.rand(count, generator=g) < 0.3).float()
+        pos = torch.nonzero(t > 0).flatten()
+        item[name] = t
+        item[key] = torch.Tensor([float(pos[int(torch.randint(0, len(pos), (1,), generator=g))])]) if len(pos) else torch.Tensor(0)
+    for key, L in (("tokens_pad1", L1), ("tokens_pad2", L2)):
+        e = torch.randn(L, Dt, generator=g)
+        item[key] = e / (e.norm(dim=-1, keepdim=True) + 1e-5)
+    return item
+
+
+def make_qfvs_batch(cfg, seed, S, Lf, seg_len, L1, L2):
+    """start_end_collate_qfvs + prepare_batch_inputs_qfvs (main/dataset_qfvs.py:211-284) of make_qfvs_item(...), on the CPU:
+    (inputs_1, inputs_2, inputs_oracle, targets_1, targets_2, targets_oracle, mask_GT).  The three inputs share the video
+    src_vid [S, Lf, Dv] (features + the TEF columns of one Lf-frame segment, padded frames included) and src_vid_mask [S, Lf];
+    the texts are concept 1 [S, L1, Dt], concept 2 [S, L2, Dt] and their concatenation [S, L1 + L2, Dt], each segment getting
+    the same query.  Targets: saliency_scores [1, S * Lf], saliency_pos_labels [1, 1] (or [1, 0]), timestamp_mask = the video
+    mask and timestamp_window = saliency_scores.  mask_GT: bool [1, S * Lf]."""
+    it = make_qfvs_item(cfg, seed, S, Lf, seg_len, L1, L2)
+    vmask = it["mask_GT"].float()
+    tef_st = torch.arange(0, Lf, 1.0) / Lf
+    tef = torch.stack([tef_st, tef_st + 1.0 / Lf], dim=1).repeat(S, 1, 1)
+    src_vid = torch.cat([it["features"], tef], dim=-1)
+    t1 = it["tokens_pad1"].float().repeat(S, 1, 1)
+    t2 = it["tokens_pad2"].float().repeat(S, 1, 1)
+    m1, m2 = torch.ones(S, L1), torch.ones(S, L2)
+    inputs = [dict(src_vid=src_vid, src_vid_mask=vmask, src_txt=t, src_txt_mask=m)
+              for t, m in ((t1, m1), (t2, m2), (torch.cat((t1, t2), dim=1), torch.cat((m1, m2), dim=1)))]
+    targets = []
+    for name, key in (("concept1_GT", "saliency_pos_labels_1"), ("concept2_GT", "saliency_pos_labels_2"),
+                      ("oracle_summary", "saliency_pos_labels_oracle")):
+        sal = it[name][None]
+        targets.append(dict(saliency_scores=sal, saliency_pos_labels=it[key][None], timestamp_mask=vmask, timestamp_window=sal))
+    return (*inputs, *targets, it["mask_GT"].reshape(1, -1))
