@@ -454,6 +454,22 @@ int univtg_decode_mr(const float* pred_logits, const float* pred_spans, const fl
 int univtg_temporal_nms(const double* windows, int32_t B, int32_t n, int32_t max_before_nms, double nms_thd, int32_t max_after_nms,
                         double* out, int32_t* counts, void* stream);
 
+/* Per-query metrics of the reference's eval_submission (eval/eval.py:20-289, eval/utils.py:17-211), IEEE double, equal to numpy's
+ * values bit for bit; univtg_b200/metrics.py does the packing and the means over queries.
+ * univtg_eval_mr: pred [Q,10,3] f64 = the first n_pred[q] (1..10) rows [st, ed, score] of each query in submission order;
+ *   gt [Q,G,2] f64 = the n_gt[q] (1..G) gt windows, G <= 64.  For the ranges r = 0 (0,10], 1 (10,30], 2 (30,inf), 3 full
+ *   (get_data_by_range's length filter): kept [4,Q] = 1 when the query has a gt window in the range; then ap [4,Q,10] =
+ *   compute_average_precision_detection at IoU 0.50:0.05:0.95 (gt windows visited NaN first, then decreasing IoU, ties to the
+ *   higher index), iou_r1 [4,Q] and iou_r5 [4,Q] = the paired IoUs of compute_mr_r1 / compute_mr_r5.  Rows not kept are 0.
+ * univtg_eval_hl: sal [Q,S] f64 = the n_sal[q] (>= 1) predicted saliency scores, zero padded; labels [Q,C] bit (3*l + a) =
+ *   (score of annotator a >= 2 + l) over the n_clips[q] = int(duration / 2) clips (1..C, C <= 4096); scratch [Q,9,C] f64.
+ *   ap [3,Q,3] = get_ap(labels, sal cut / zero-padded to n_clips) (scikit-learn precision_recall_curve); hit [3,Q,3] = the label
+ *   at np.argmax of the whole predicted list (0 when that index is >= n_clips). */
+int univtg_eval_mr(const double* pred, const int32_t* n_pred, const double* gt, const int32_t* n_gt, int32_t Q, int32_t G, double* ap,
+                   double* iou_r1, double* iou_r5, uint8_t* kept, void* stream);
+int univtg_eval_hl(const double* sal, const int32_t* n_sal, const uint16_t* labels, const int32_t* n_clips, int32_t Q, int32_t S,
+                   int32_t C, double* scratch, double* ap, double* hit, void* stream);
+
 /* LayerNorm rows: in [rows,d] f32 -> out32 [rows,d] f32 and/or out16 [rows,ld16] 16-bit (zero padded). */
 int univtg_op_layernorm(const float* in, int32_t rows, int32_t d, const float* gamma, const float* beta, float eps,
                         int32_t fmt, float* out32, void* out16, int32_t ld16, void* stream);

@@ -5,6 +5,8 @@ Input conventions follow the reference data pipeline: row-L2-normalised features
 targets (main/dataset.py:501, 525-556, 1078-1098).  Seeds: weights torch.Generator(seed), data Generator(seed+1).
 """
 import math
+import random
+import struct
 from argparse import Namespace
 
 import torch
@@ -346,3 +348,127 @@ def make_qfvs_batch(cfg, seed, S, Lf, seg_len, L1, L2):
         sal = it[name][None]
         targets.append(dict(saliency_scores=sal, saliency_pos_labels=it[key][None], timestamp_mask=vmask, timestamp_window=sal))
     return (*inputs, *targets, it["mask_GT"].reshape(1, -1))
+
+
+# ---- evaluation submissions (eval/eval.py) --------------------------------------------------------------------------------
+def _half(x):
+    return struct.unpack("e", struct.pack("e", x))[0]
+
+
+def _cross_iou(p, g):
+    """eval/utils.py compute_temporal_iou_batch_cross for one pair, in the same double operations (0/0 -> NaN)."""
+    inter = max(min(p[1], g[1]) - max(p[0], g[0]), 0.0)
+    union = (p[1] - p[0]) + (g[1] - g[0]) - inter
+    if union == 0:
+        return math.nan
+    return inter / union
+
+
+def _ambiguous_gt_tie(rows, windows):
+    """True when one of the first 10 predicted windows has equal IoU >= 0.5 (or NaN) with two different gt windows: the
+    reference's gt visit order (numpy's default argsort) then depends on the machine."""
+    for p in rows[:10]:
+        seen = {}
+        for g in windows:
+            v = _cross_iou(p, g)
+            key = "nan" if math.isnan(v) else v
+            if key != "nan" and v < 0.5:
+                continue
+            if key in seen and seen[key] != tuple(g):
+                return True
+            seen[key] = tuple(g)
+    return False
+
+
+def make_eval_case(seed, n_queries=40, n_windows=10, durations=(150, 149, 148, 60), gt_lengths=(0, 2, 4, 10, 10, 14, 30, 30, 44, 90),
+                   max_gt=4, sort_windows=True, match_number=True, tasks="mr+hl"):
+    """A deterministic (Python `random`) submission / ground-truth pair in the format eval/eval.py:eval_submission reads.
+
+    Ground truth per query: duration from `durations`; 1..max_gt windows [st, ed] on the 2 s clip grid with lengths from
+    `gt_lengths` (0 = zero-length; 10 and 30 sit on the range edges), clipped to the duration; relevant_clip_ids (sometimes
+    unsorted) covering the windows, with 3 annotator scores in 0..4 (some annotators all below 2 -> all-0 label columns; some
+    queries cover every clip with one annotator at 4 -> all-1 columns).
+    Submission per query: n_windows rows [st, ed, score] (some queries fewer than 5) rounded to 4 decimals like the decode, scores
+    often multiples of 1/16 (ties), some rows copying or jittering a gt window, zero-length rows including one on a zero-length
+    gt window (0/0 IoU); sorted by score (descending, stable) or, with sort_windows=False, in start order like --no_sort_results.
+    pred_saliency_scores are fp16-rounded (or multiples of 1/16), sometimes longer or shorter than int(duration / 2).
+    Queries whose first 10 rows tie two different gt windows at IoU >= 0.5 (or NaN) are redrawn.
+    match_number=False: the two lists share only part of their qids.  tasks "mr" / "hl" leaves out pred_saliency_scores /
+    pred_relevant_windows (the metrics of the other task are then skipped).
+    Returns {"submission", "ground_truth", "match_number"}."""
+    rng = random.Random(seed)
+    sub, gt = [], []
+    for qid in range(n_queries):
+        while True:
+            dur = rng.choice(durations)
+            n_clips = int(dur / 2)
+            windows = []
+            for _ in range(rng.randint(1, max_gt) if rng.random() < 0.5 else 1):
+                ln = min(rng.choice(gt_lengths), 2 * n_clips)
+                st = 2 * rng.randint(0, (2 * n_clips - ln) // 2)
+                windows.append([st, st + ln])
+            if rng.random() < 0.1:
+                windows.append(list(windows[0]))  # identical duplicate: harmless for the tie rule
+            if rng.random() < 0.2:
+                windows = [[float(s), float(e)] for s, e in windows]
+            every = rng.random() < 0.06
+            if every:
+                clips = list(range(n_clips))
+            else:
+                clips = sorted({c for s, e in windows for c in range(int(s) // 2, min(int(e) // 2, n_clips))})
+                if not clips:
+                    clips = [rng.randrange(n_clips)]
+            if rng.random() < 0.3:
+                rng.shuffle(clips)
+            low = rng.randrange(3) if rng.random() < 0.3 else -1
+            scores = []
+            for _ in clips:
+                row = [rng.randint(0, 4) for _ in range(3)]
+                if low >= 0:
+                    row[low] = rng.randint(0, 1)
+                if every:
+                    row[(low + 1) % 3] = 4
+                scores.append(row)
+            n = rng.randint(1, 4) if rng.random() < 0.1 else n_windows
+            rows = []
+            for _ in range(n):
+                u = rng.random()
+                if u < 0.25:
+                    s, e = rng.choice(windows)
+                    if rng.random() < 0.5:
+                        s, e = s + rng.uniform(-3, 3), e + rng.uniform(-3, 3)
+                    s, e = min(max(s, 0.0), dur), min(max(e, 0.0), dur)
+                    s, e = min(s, e), max(s, e)
+                elif u < 0.3:
+                    s = e = rng.uniform(0, dur)
+                else:
+                    s = rng.uniform(0, dur)
+                    e = min(dur, s + rng.choice([2.0, 10.0, 30.0, rng.uniform(0, dur)]))
+                sc = rng.randrange(17) / 16 if rng.random() < 0.5 else rng.random()
+                rows.append([float(f"{s:.4f}"), float(f"{e:.4f}"), float(f"{sc:.4f}")])
+            zero = [w for w in windows if w[0] == w[1]]
+            if zero and rng.random() < 0.5:
+                rows[rng.randrange(len(rows))][:2] = [float(zero[0][0]), float(zero[0][1])]  # 0/0 IoU
+            if not _ambiguous_gt_tie(rows, windows):
+                break
+        if sort_windows:
+            rows.sort(key=lambda r: -r[2])
+        else:
+            rows.sort(key=lambda r: r[0])
+        n_sal = n_clips + (rng.choice([-3, -1, 1, 4]) if rng.random() < 0.2 else 0)
+        if rng.random() < 0.3:
+            sal = [rng.randrange(-16, 17) / 16 for _ in range(max(n_sal, 1))]
+        else:
+            sal = [_half(rng.uniform(-1, 1)) for _ in range(max(n_sal, 1))]
+        gt.append(dict(qid=qid, query=f"query {qid}", duration=dur, vid=f"vid{qid}", relevant_windows=windows,
+                       relevant_clip_ids=clips, saliency_scores=scores))
+        pred = dict(qid=qid, query=f"query {qid}", vid=f"vid{qid}", pred_relevant_windows=rows, pred_saliency_scores=sal)
+        if tasks == "mr":
+            del pred["pred_saliency_scores"]
+        elif tasks == "hl":
+            del pred["pred_relevant_windows"]
+        sub.append(pred)
+    if not match_number:
+        k = max(1, n_queries // 5)
+        sub, gt = sub[k:], gt[:-k]
+    return {"submission": sub, "ground_truth": gt, "match_number": match_number}
