@@ -254,6 +254,9 @@ int univtg_op_gemm_cluster(const void* a, const void* b, int32_t M, int32_t N, i
  *             row m of the result is sum_t dY[m - t + 1] W[:, :, t].  a_mn = 0, b_mn = 1.
  *   conv = 2: weight gradient of tap `tap`: a = dY [K+2, M], b = X [K+2, N] (same layout); C[n, c] = sum_m dY[m, n] X[m + tap - 1, c]
  *             over the K logical rows.  a_mn = b_mn = 1.
+ *   conv = 3: k=3 Conv1d forward of the heads over the same layout: a = X [M+2, K/3] (pitch lda; rows 0, M+1 and the separator rows
+ *             zero), b = packed weight [N, K] with b[o, t*K/3 + c] = W[o, c, t] (ldb = K); row m of the result is
+ *             sum_t X[m + t - 1] W[:, :, t] (logical rows).  a_mn = b_mn = 0, K/3 % 64 == 0, cluster 1.
  * Epilogue: v = act(acc + bias[n]) * alpha * row_scale[m / rps_in]; out row = (m / rps_in) * rps_out + m % rps_in + row_off
  * (identity when rps_in = 0); zero_sep stores v = 0 and skip_sep stores nothing on rows with m % rps_in == rps_in - 1;
  * v += resid[out row]; mask16 (indexed like out16, group fmt) zeroes v where mask16 <= 0, or multiplies v by it (mask_mul = 1);
@@ -478,6 +481,98 @@ int univtg_op_layernorm(const float* in, int32_t rows, int32_t d, const float* g
  * impl: 0 = tensor cores (wgmma, dh in {64,128}), 1 = SIMT (any dh). */
 int univtg_op_attention(const void* qkv, const float* key_mask, void* out, float* lse, int32_t B, int32_t L, int32_t H,
                         int32_t dh, int32_t fmt, int32_t impl, void* stream);
+
+/* LayerNorm forward with the fused store epilogue of univtg_forward (one entry per LnArgs field of csrc/rowops.h):
+ *   v = (in or in16) + add16 (sum_out = v, fp32 [rows, d]);  y = (v - mean) * rstd * gamma + beta, rstd = 1/sqrt(var + eps);
+ *   out32 = y;  y' = y * (mul32 or the in-kernel dropout of (rng, mask_index), as univtg_dropout_mask reads it back);
+ *   out16 = 16-bit(y') [rows, ld16] (columns [d, ld16) zeroed);  out16p = 16-bit(y' + pos[b*Lv + l]) on video rows l < Lv,
+ *   16-bit(y' + pos_txt[b*(L-Lv) + l - Lv]) on text rows when pos_txt is given, else 16-bit(y');  outc = 16-bit(y') at row
+ *   1 + b*(Lv+1) + l of the conv-head layout for video rows;  mean_out / rstd_out [rows].  Row r = b*L + l (L = 0: unstructured).
+ * fmt 0 fp16, 1 bf16, 2 fp16x3 (no dropout): add16, out16, out16p and outc are hi planes whose lo planes lie `lo` elements after
+ * them.  fp32 pointers must be 16-byte and 16-bit pointers 8-byte aligned. */
+typedef struct univtg_ln_fwd {
+  const float* in;
+  const void* in16;
+  int32_t in_fmt, ld_in;
+  const void* add16;
+  int32_t ld_add16;
+  float* sum_out;
+  int32_t rows, d;
+  const float* gamma;
+  const float* beta;
+  float eps;
+  int32_t fmt;
+  int64_t lo;
+  int32_t L, Lv;
+  float* out32;
+  void* out16;
+  void* out16p;
+  int32_t ld16;
+  const float* pos;
+  const float* pos_txt;
+  void* outc;
+  const float* mul32;
+  float* mean_out;
+  float* rstd_out;
+} univtg_ln_fwd;
+/* kernel_used (optional) receives the instantiation that ran: 0/1/2 warp-per-row d = 1024/512/256, 3/4/5 the same with pos_txt,
+ * 6/7 row-per-block d <= 1024 / <= 3072, 8/9 the same with pos_txt, 10 the 64-bit-load projector kernel (even d in (1024, 3072],
+ * out16 only), 11 any d; + 12 for fp16x3. */
+int univtg_op_layernorm_fwd(const univtg_ln_fwd* args, const univtg_rng* rng, int32_t mask_index, int32_t* kernel_used, void* stream);
+
+/* Learned text positions of univtg_plan_set_txt_pos, one text row r = b*Lt + l at a time: pos[r] = drop(LayerNorm(xt[r] + table[l]))
+ * (eps 1e-5; mul32, else the dropout of (rng, mask_index)); row b*L + Lv + l of xpos16 [B*L, d] = 16-bit(xt[r] + pos[r]), no other
+ * row is written; mean_out / rstd_out [B*Lt] (both or neither).  d % 64 == 0, d <= 1024.  fmt 2: fp16x3, xpos16's lo plane `lo`
+ * elements after it. */
+typedef struct univtg_txt_pos_fwd {
+  const float* xt;
+  const float* table;
+  const float* gamma;
+  const float* beta;
+  const float* mul32;
+  float* pos;
+  float* mean_out;
+  float* rstd_out;
+  void* xpos16;
+  int32_t B, Lt, L, Lv, d, fmt;
+  int64_t lo;
+} univtg_txt_pos_fwd;
+int univtg_op_txt_pos(const univtg_txt_pos_fwd* args, const univtg_rng* rng, int32_t mask_index, void* stream);
+
+/* Sine position table of univtg_forward: c = cumsum_l(vid_mask[b]); pos[b*Lv + l, 2k + {0,1}] = {sin, cos}(c_l / (c_last + 1e-6)
+ * * 2pi / dim_t[2k]) (fp32 [B*Lv, d], d even, 8-byte aligned); key_mask (optional) [B, Lv+Lt] = cat(vid_mask, txt_mask);
+ * dp_out (optional) [n_sites, B] = the DropPath scales of rng (univtg_droppath_scales).  Lv <= 12288. */
+int univtg_op_sine_pos(const float* vid_mask, const float* txt_mask, const float* dim_t, float* pos, float* key_mask, int32_t B, int32_t Lv,
+                       int32_t Lt, int32_t d, const univtg_rng* rng, int32_t n_sites, float* dp_out, void* stream);
+
+/* WeightedPool + cosine saliency of univtg_forward: logits [B, Lt] = x_txt . w + (1 - txt_mask) * -1e30 (scratch, written);
+ * alpha = softmax_l(logits) (alpha_out optional); pooled [B, d] = sum_l alpha_l x_txt[b, l];
+ * saliency [B, Lv] = x_vid . pooled / (max(|x_vid|, 1e-8) max(|pooled|, 1e-8)) + log(vid_mask + 1e-45).
+ * d % 4 == 0, fp32 arrays 16-byte aligned, Lt <= 12288. */
+int univtg_op_pool_saliency(const float* x_txt, const float* x_vid, const float* txt_mask, const float* vid_mask, const float* w,
+                            float* pooled, float* saliency, float* alpha_out, float* logits, int32_t B, int32_t Lt, int32_t Lv, int32_t d,
+                            void* stream);
+
+/* Last conv layer of both heads: h_cls / h_span 16-bit [B*(Lv+1)+2, d] in the conv-head layout (rows 0, B*(Lv+1)+1 and the separator
+ * rows zero); w_cls [3][d], w_span [2][3][d] fp32 (w[o][t][c] = W[o, c, t]); pred_logits [B*Lv] = sigmoid(z_cls), pred_spans [B*Lv, 2]
+ * = (-sigmoid(z_0), sigmoid(z_1)) with z = sum_t h[row + t - 1] . w[t] + bias.  d even; fmt 2 (fp16x3): lo planes directly after the
+ * hi planes ((B*(Lv+1)+2) * d elements later). */
+int univtg_op_conv_head_final(const void* h_cls, const void* h_span, const float* w_cls, const float* w_span, const float* b_cls,
+                              const float* b_span, float* pred_logits, float* pred_spans, int32_t B, int32_t Lv, int32_t d, int32_t fmt,
+                              void* stream);
+
+/* Attention forward with every option of the kernels: qkv, key_mask, out, lse as univtg_op_attention; causal = 1: query i sees keys
+ * j <= i only (dh 64, fmt 0/1, tensor cores, no dropout); impl 0 tensor cores (dh 64 / 128), 1 SIMT (any dh); p > 0: attention
+ * dropout of encoder layer `layer` of rng (univtg_attention_dropout_mask reads it back; fmt 0/1).  kernel_used (optional):
+ * 0..7 tensor cores = 4 (dh 128) + 2 (bf16) + dropout, 8/9 causal fp16/bf16, 10/11 fp16x3 dh 64/128, 12/13/14 SIMT plain/dropout/fp16x3. */
+typedef struct univtg_attn_fwd {
+  const void* qkv;
+  const float* key_mask;
+  void* out;
+  float* lse;
+  int32_t B, L, H, dh, fmt, impl, causal;
+} univtg_attn_fwd;
+int univtg_op_attention_fwd(const univtg_attn_fwd* args, const univtg_rng* rng, float p, int32_t layer, int32_t* kernel_used, void* stream);
 
 /* Attention core backward.  qkv as above; dO [B*L,d] 16-bit gradient of `out`; O = forward output (16-bit, fmt_act);
  * (same 16-bit format as qkv); lse from the forward; delta_ws [B,H,L] f32 scratch; dqkv32 [B*L,3d] f32 receives

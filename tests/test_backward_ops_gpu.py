@@ -5,12 +5,9 @@ Method: the 16-bit inputs are drawn once and the reference is computed in fp64 f
 fp32 statistics where a kernel consumes the forward's mean / rstd / alpha).  Outputs are filled with NaN before the call and
 accumulated outputs with known non-zero values, so "overwritten", "added to" and "left alone" are each checked.
 
-Tolerances come from the arithmetic: an fp32 result must satisfy |got - ref| <= c * 2^-24 * S elementwise, with S the same
-operation applied to absolute values (for composite formulas every term replaced by its absolute value) and
-c = 4 * (ceil(log2 K) + 1): the depth of a K-term reduction plus one level for the few roundings of each term.  A 16-bit result
-may additionally differ by half an ulp of its format.  Masked entries, separator rows, padding columns and ReLU zeros have
-S = 0 and must be exactly zero; rows and columns a kernel must not write must still hold NaN.  The worst |got - ref| / bound
-of every case is printed (pytest -s) and summarised per kernel family at the end of the module.
+Tolerances come from the arithmetic (tests/bounds.py): c(K) * 2^-24 * S with S the same formula over absolute values, plus half
+an ulp for 16-bit results; zero-bound entries must be exact and regions the kernel must not write must still hold NaN.  The
+worst |got - ref| / bound of every case is printed (pytest -s) and summarised per kernel family at the end of the module.
 """
 import ctypes
 import math
@@ -18,23 +15,14 @@ import math
 import pytest
 import torch
 
+from tests.bounds import all_nan, check, offset_view, report_fixture
 from univtg_b200 import _lib
 
 pytestmark = pytest.mark.gpu
 
-U = 2.0 ** -24
 DT = {0: torch.float16, 1: torch.bfloat16}
-_WORST = {}
 _SEEN = {"lnb_kernel": set(), "vec_ok": set(), "full": set()}
-
-
-@pytest.fixture(scope="module", autouse=True)
-def _report():
-    yield
-    print("\nworst |got - ref| / bound per kernel family:")
-    for fam, (r, case) in sorted(_WORST.items()):
-        print(f"  {fam:26s} {r:.3f}  ({case})")
-    print("coverage:", {k: sorted(v) for k, v in _SEEN.items()})
+_report = report_fixture(_SEEN)
 
 
 def lib():
@@ -59,56 +47,6 @@ def nan(shape, dtype=torch.float32):
 
 def rnd16(shape, fmt, g, scale=1.0):
     return (torch.randn(shape, generator=g) * scale).to(DT[fmt]).cuda()
-
-
-def offset_view(rows, ld, dtype, byte_off, fill=float("nan")):
-    """[rows, ld] view that starts byte_off bytes into a fresh allocation (16- but not 32-byte aligned for byte_off = 16)."""
-    es = torch.tensor([], dtype=dtype).element_size()
-    k = byte_off // es
-    flat = torch.full((rows * ld + k + 64,), fill, dtype=dtype, device="cuda")
-    v = flat[k:k + rows * ld].view(rows, ld)
-    assert v.data_ptr() % 32 == byte_off % 32
-    return v
-
-
-def ulp16(x, fmt):
-    """ulp of |x| in fp16 (fmt 0) / bf16 (fmt 1), x fp64 >= 0."""
-    p, emin = (10, -14) if fmt == 0 else (7, -126)
-    _, e = torch.frexp(x)
-    ex = torch.clamp(e.to(torch.float64) - 1, min=emin)
-    return torch.pow(2.0, ex - p)
-
-
-def cfac(K):
-    return 4 * (math.ceil(math.log2(max(int(K), 1))) + 1)
-
-
-def check(family, name, got, ref, S, K, fmt=None):
-    """|got - ref| <= c(K) 2^-24 S (+ half an ulp of `fmt` for 16-bit results); S == 0 means exact."""
-    got = got.double()
-    ref = ref.double()
-    S = S.double()
-    assert got.shape == ref.shape == S.shape, (name, got.shape, ref.shape, S.shape)
-    assert torch.isfinite(got).all(), f"{family}/{name}: {int((~torch.isfinite(got)).sum())} non-finite values (not written?)"
-    b = cfac(K) * U * S
-    if fmt is not None:
-        b = b + 0.5 * ulp16(ref.abs() + b, fmt) * (S > 0)
-    err = (got - ref).abs()
-    ratio = float((err / torch.where(b > 0, b, torch.full_like(b, float("inf")))).max()) if err.numel() else 0.0
-    bad = err > b
-    if bad.any():
-        i = int(bad.flatten().nonzero()[0])
-        raise AssertionError(f"{family}/{name}: {int(bad.sum())} of {bad.numel()} entries out of bound; first flat index {i}: "
-                             f"got {got.flatten()[i].item()!r} ref {ref.flatten()[i].item()!r} bound {b.flatten()[i].item()!r}; "
-                             f"worst ratio {ratio:.3g}")
-    print(f"  {family}/{name}: worst |got-ref|/bound = {ratio:.3f}")
-    fam = family + (" (16-bit)" if fmt is not None else " (fp32)")  # a 16-bit result's ratio is dominated by its half ulp
-    if ratio >= _WORST.get(fam, (-1.0, ""))[0]:
-        _WORST[fam] = (ratio, name)
-
-
-def all_nan(t, what):
-    assert torch.isnan(t.float()).all(), f"{what}: a region the kernel must not write was written"
 
 
 def pos16(t):

@@ -87,6 +87,30 @@ class TxtPosBwd(ctypes.Structure):
         [("pgrad_scale", c_float), ("B", c_int), ("Lt", c_int), ("L", c_int), ("Lv", c_int), ("d", c_int)]
 
 
+class LnFwd(ctypes.Structure):
+    """univtg_ln_fwd."""
+
+    _fields_ = [("in_", c_void_p), ("in16", c_void_p), ("in_fmt", c_int), ("ld_in", c_int), ("add16", c_void_p), ("ld_add16", c_int),
+                ("sum_out", c_void_p), ("rows", c_int), ("d", c_int), ("gamma", c_void_p), ("beta", c_void_p), ("eps", c_float),
+                ("fmt", c_int), ("lo", ctypes.c_int64), ("L", c_int), ("Lv", c_int), ("out32", c_void_p), ("out16", c_void_p),
+                ("out16p", c_void_p), ("ld16", c_int), ("pos", c_void_p), ("pos_txt", c_void_p), ("outc", c_void_p), ("mul32", c_void_p),
+                ("mean_out", c_void_p), ("rstd_out", c_void_p)]
+
+
+class TxtPosFwd(ctypes.Structure):
+    """univtg_txt_pos_fwd."""
+
+    _fields_ = [(n, c_void_p) for n in ("xt", "table", "gamma", "beta", "mul32", "pos", "mean_out", "rstd_out", "xpos16")] + \
+        [(n, c_int) for n in ("B", "Lt", "L", "Lv", "d", "fmt")] + [("lo", ctypes.c_int64)]
+
+
+class AttnFwd(ctypes.Structure):
+    """univtg_attn_fwd."""
+
+    _fields_ = [("qkv", c_void_p), ("key_mask", c_void_p), ("out", c_void_p), ("lse", c_void_p)] + \
+        [(n, c_int) for n in ("B", "L", "H", "dh", "fmt", "impl", "causal")]
+
+
 class ClipConfig(ctypes.Structure):
     """univtg_clip_config."""
 
@@ -167,6 +191,12 @@ SIGNATURES = {
     "univtg_op_attention": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int,
                                     c_void_p]),
     "univtg_op_attention_bwd": (c_int, [c_void_p] * 7 + [c_int, c_int, c_int, c_int, c_int, c_int, c_void_p]),
+    "univtg_op_layernorm_fwd": (c_int, [ctypes.POINTER(LnFwd), ctypes.POINTER(Rng), c_int, c_void_p, c_void_p]),
+    "univtg_op_txt_pos": (c_int, [ctypes.POINTER(TxtPosFwd), ctypes.POINTER(Rng), c_int, c_void_p]),
+    "univtg_op_sine_pos": (c_int, [c_void_p] * 5 + [c_int, c_int, c_int, c_int, ctypes.POINTER(Rng), c_int, c_void_p, c_void_p]),
+    "univtg_op_pool_saliency": (c_int, [c_void_p] * 9 + [c_int, c_int, c_int, c_int, c_void_p]),
+    "univtg_op_conv_head_final": (c_int, [c_void_p] * 8 + [c_int, c_int, c_int, c_int, c_void_p]),
+    "univtg_op_attention_fwd": (c_int, [ctypes.POINTER(AttnFwd), ctypes.POINTER(Rng), c_float, c_int, c_void_p, c_void_p]),
     "univtg_clip_num_params": (c_int, [ctypes.POINTER(ClipConfig)]),
     "univtg_clip_packed_bytes": (c_size_t, [ctypes.POINTER(ClipConfig)]),
     "univtg_clip_pack_weights": (c_int, [ctypes.POINTER(ClipConfig), ctypes.POINTER(c_void_p), c_int, c_int, c_void_p, c_void_p]),

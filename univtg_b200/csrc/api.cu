@@ -621,18 +621,7 @@ int run_forward(univtg_plan* P, const FwdBufs& W, const float* src_txt, const fl
   // ---- heads: conv layers (k=3, pad=1) as 3-tap GEMMs over the separated layout, then the final conv and the pooling ----
   auto conv_problem = [&](GemmProblem& p, const uint16_t* A, int lda, const uint16_t* Wc, int N, const float* bias, uint16_t* out,
                           int ldo, int bn) -> int {
-    init_problem(p);
-    p.M = P->Mh;
-    p.N = N;
-    p.taps = 3;
-    p.kblk_per_tap = d / 64;
-    // A tile row for tap t: buffer row m0 + t  (buffer row = logical row + 1)
-    p.ca = OperandCoord{0, 0, 0, 1, 0, 1, 1, 0};
-    // W2 [N, 3d]: column tap*d + k
-    p.cb = OperandCoord{0, 0, d, 1, 0, 1, 0, 0};
-    int r = make_tmap_op(&p.tm_a, A, (uint64_t)P->Mh + 2, (uint64_t)d, (uint64_t)lda, GEMM_BM, 64, ws_lo);
-    r |= make_tmap_op(&p.tm_b, Wc, (uint64_t)N, (uint64_t)3 * d, (uint64_t)3 * d, (uint32_t)bn, 64, pk_lo);
-    p.b_box_rows = bn;
+    const int r = conv_fwd_problem(p, P->Mh, A, lda, d, Wc, N, bn, ws_lo, pk_lo);
     p.bias = bias;
     p.act = ACT_RELU;
     p.rps_in = Lv + 1;
@@ -830,6 +819,215 @@ int univtg_op_layernorm(const float* in, int32_t rows, int32_t d, const float* g
   a.split = fmt == 2;
   a.lo = fmt == 2 ? (long long)rows * a.ld16 : 0;
   return launch_layernorm(a, (cudaStream_t)stream);
+}
+
+// ---- single forward operators: thin wrappers over the launchers run_forward uses; each checks on the host what its kernel assumes and
+// its routing does not (the vector kernels load fp32 operands as float4 and 16-bit ones as uint2). ----
+int univtg_op_layernorm_fwd(const univtg_ln_fwd* q, const univtg_rng* rng, int32_t mask_index, int32_t* kernel_used, void* stream) {
+  const char* fn = "univtg_op_layernorm_fwd";
+  UV_REQ(q != nullptr, "%s: null args", fn);
+  UV_REQ((q->in || q->in16) && q->gamma && q->beta, "%s: null in / in16, gamma or beta", fn);
+  UV_REQ(q->rows >= 1 && q->d >= 1, "%s: rows %d / d %d", fn, q->rows, q->d);
+  UV_REQ(q->ld_in >= q->d, "%s: ld_in %d smaller than d %d", fn, q->ld_in, q->d);
+  UV_REQ(!q->in16 || q->in_fmt == 0 || q->in_fmt == 1, "%s: in_fmt %d (0 fp16, 1 bf16)", fn, q->in_fmt);
+  UV_REQ(q->fmt >= 0 && q->fmt <= 2, "%s: fmt %d (0 fp16, 1 bf16, 2 fp16x3)", fn, q->fmt);
+  UV_REQ(!q->add16 || q->ld_add16 >= q->d, "%s: ld_add16 %d smaller than d %d", fn, q->ld_add16, q->d);
+  UV_REQ(!q->add16 || q->d % 4 != 0 || q->ld_add16 % 4 == 0, "%s: ld_add16 %d must be a multiple of 4 (64-bit loads)", fn, q->ld_add16);
+  UV_REQ(!q->sum_out || q->add16, "%s: sum_out needs add16", fn);
+  UV_REQ(!(q->out16 || q->out16p) || q->ld16 >= q->d, "%s: ld16 %d smaller than d %d", fn, q->ld16, q->d);
+  UV_REQ(q->L >= 0 && q->Lv >= 0 && q->Lv <= q->L && (q->L == 0 || q->rows % q->L == 0), "%s: L %d / Lv %d (rows %% L == 0)", fn, q->L,
+         q->Lv);
+  UV_REQ(!(q->pos || q->pos_txt || q->outc) || q->L >= 1, "%s: pos, pos_txt and outc need the token structure (L >= 1)", fn);
+  UV_REQ(!q->pos || q->out16p, "%s: pos is only used with out16p", fn);
+  UV_REQ(q->fmt != 2 || (q->lo > 0 && q->lo % 4 == 0), "%s: fmt 2 needs lo > 0, a multiple of 4", fn);
+  UV_REQ(q->fmt != 2 || (!q->mul32 && !(rng && rng->input_dropout > 0.f)), "%s: fmt 2 (fp16x3) takes no dropout (mul32 / rng)", fn);
+  UV_REQ(!rng || !(rng->input_dropout > 0.f) || mask_index >= 0, "%s: mask_index %d", fn, mask_index);
+  UV_REQ(al_(q->in, 16) && al_(q->gamma, 16) && al_(q->beta, 16) && al_(q->sum_out, 16) && al_(q->out32, 16) && al_(q->pos, 16) &&
+             al_(q->pos_txt, 16) && al_(q->mul32, 16) && al_(q->mean_out, 4) && al_(q->rstd_out, 4),
+         "%s: fp32 pointers must be 16-byte aligned", fn);
+  UV_REQ(al_(q->in16, 8) && al_(q->add16, 8) && al_(q->out16, 8) && al_(q->out16p, 8) && al_(q->outc, 8),
+         "%s: in16, add16, out16, out16p and outc must be 8-byte aligned", fn);
+  LnArgs a;
+  memset(&a, 0, sizeof(a));
+  a.in = q->in;
+  a.ld_in = q->ld_in;
+  a.in16 = reinterpret_cast<const uint16_t*>(q->in16);
+  a.in_fmt = q->in_fmt;
+  a.add16 = reinterpret_cast<const uint16_t*>(q->add16);
+  a.ld_add16 = q->ld_add16;
+  a.sum_out = q->sum_out;
+  a.rows = q->rows;
+  a.d = q->d;
+  a.gamma = q->gamma;
+  a.beta = q->beta;
+  a.eps = q->eps;
+  a.fmt = q->fmt == 2 ? 0 : q->fmt;
+  a.split = q->fmt == 2;
+  a.lo = q->fmt == 2 ? (long long)q->lo : 0;
+  a.L = q->L;
+  a.Lv = q->Lv;
+  a.out32 = q->out32;
+  a.out16 = reinterpret_cast<uint16_t*>(q->out16);
+  a.out16p = reinterpret_cast<uint16_t*>(q->out16p);
+  a.ld16 = (q->out16 || q->out16p) ? q->ld16 : q->d;
+  a.pos = q->pos;
+  a.pos_txt = q->pos_txt;
+  a.outc = reinterpret_cast<uint16_t*>(q->outc);
+  a.mul32 = q->mul32;
+  if (!a.mul32 && rng && rng->input_dropout > 0.f) a.drop = make_drop_spec(rng->seed, (unsigned int)mask_index, rng->input_dropout);
+  a.mean_out = q->mean_out;
+  a.rstd_out = q->rstd_out;
+  int used = -1;
+  const int rc = launch_layernorm(a, (cudaStream_t)stream, &used);
+  if (kernel_used) *kernel_used = used;
+  return rc;
+}
+
+int univtg_op_txt_pos(const univtg_txt_pos_fwd* q, const univtg_rng* rng, int32_t mask_index, void* stream) {
+  const char* fn = "univtg_op_txt_pos";
+  UV_REQ(q != nullptr, "%s: null args", fn);
+  UV_REQ(q->xt && q->table && q->gamma && q->beta && q->pos && q->xpos16, "%s: null xt, table, gamma, beta, pos or xpos16", fn);
+  UV_REQ((q->mean_out == nullptr) == (q->rstd_out == nullptr), "%s: mean_out and rstd_out must both be given or both be NULL", fn);
+  UV_REQ(q->B >= 1 && q->Lt >= 1 && q->Lv >= 0 && q->L >= q->Lv + q->Lt, "%s: B %d / Lt %d / L %d / Lv %d (L >= Lv + Lt)", fn, q->B,
+         q->Lt, q->L, q->Lv);
+  UV_REQ(q->fmt >= 0 && q->fmt <= 2, "%s: fmt %d (0 fp16, 1 bf16, 2 fp16x3)", fn, q->fmt);
+  UV_REQ(q->fmt != 2 || (q->lo > 0 && q->lo % 2 == 0), "%s: fmt 2 needs lo > 0, a multiple of 2", fn);
+  UV_REQ(q->fmt != 2 || (!q->mul32 && !(rng && rng->input_dropout > 0.f)), "%s: fmt 2 (fp16x3) takes no dropout (mul32 / rng)", fn);
+  UV_REQ(!rng || !(rng->input_dropout > 0.f) || mask_index >= 0, "%s: mask_index %d", fn, mask_index);
+  UV_REQ(al_(q->xt, 8) && al_(q->table, 8) && al_(q->gamma, 8) && al_(q->beta, 8) && al_(q->mul32, 8) && al_(q->pos, 8) &&
+             al_(q->mean_out, 4) && al_(q->rstd_out, 4) && al_(q->xpos16, 4),
+         "%s: fp32 pointers must be 8-byte and xpos16 4-byte aligned", fn);
+  TxtPosArgs a;
+  memset(&a, 0, sizeof(a));
+  a.xt = q->xt;
+  a.table = q->table;
+  a.gamma = q->gamma;
+  a.beta = q->beta;
+  a.mul32 = q->mul32;
+  if (!a.mul32 && rng && rng->input_dropout > 0.f) a.drop = make_drop_spec(rng->seed, (unsigned int)mask_index, rng->input_dropout);
+  a.pos = q->pos;
+  a.mean_out = q->mean_out;
+  a.rstd_out = q->rstd_out;
+  a.xpos16 = reinterpret_cast<uint16_t*>(q->xpos16);
+  a.B = q->B;
+  a.Lt = q->Lt;
+  a.L = q->L;
+  a.Lv = q->Lv;
+  a.d = q->d;
+  a.fmt = q->fmt == 2 ? 0 : q->fmt;
+  a.split = q->fmt == 2;
+  a.lo = q->fmt == 2 ? (long long)q->lo : 0;
+  return launch_txt_pos(a, (cudaStream_t)stream);
+}
+
+int univtg_op_sine_pos(const float* vid_mask, const float* txt_mask, const float* dim_t, float* pos, float* key_mask, int32_t B, int32_t Lv,
+                       int32_t Lt, int32_t d, const univtg_rng* rng, int32_t n_sites, float* dp_out, void* stream) {
+  const char* fn = "univtg_op_sine_pos";
+  UV_REQ(vid_mask && dim_t && pos, "%s: null vid_mask, dim_t or pos", fn);
+  UV_REQ(B >= 1 && Lv >= 1 && Lv <= 12288 && Lt >= 0, "%s: B %d / Lv %d / Lt %d (1 <= Lv <= 12288)", fn, B, Lv, Lt);
+  UV_REQ(d >= 2 && d % 2 == 0, "%s: d %d must be even (sin / cos column pairs)", fn, d);
+  UV_REQ(!key_mask || Lt == 0 || txt_mask, "%s: key_mask needs txt_mask", fn);
+  UV_REQ(!dp_out || (rng && n_sites >= 1), "%s: dp_out needs rng and n_sites >= 1", fn);
+  UV_REQ(al_(pos, 8) && al_(vid_mask, 4) && al_(txt_mask, 4) && al_(dim_t, 4) && al_(key_mask, 4) && al_(dp_out, 4),
+         "%s: pos must be 8-byte aligned", fn);
+  return launch_sine_pos(vid_mask, txt_mask, dim_t, pos, key_mask, B, Lv, Lt, d, (cudaStream_t)stream, dp_out, dp_out ? n_sites : 0,
+                         rng ? rng->seed : 0ull, rng ? 1.0f - rng->droppath : 1.f);
+}
+
+int univtg_op_pool_saliency(const float* x_txt, const float* x_vid, const float* txt_mask, const float* vid_mask, const float* w,
+                            float* pooled, float* saliency, float* alpha_out, float* logits, int32_t B, int32_t Lt, int32_t Lv, int32_t d,
+                            void* stream) {
+  const char* fn = "univtg_op_pool_saliency";
+  UV_REQ(x_txt && x_vid && txt_mask && vid_mask && w && pooled && saliency && logits, "%s: null pointer argument", fn);
+  UV_REQ(B >= 1 && Lt >= 1 && Lt <= 12288 && Lv >= 1, "%s: B %d / Lt %d / Lv %d (1 <= Lt <= 12288)", fn, B, Lt, Lv);
+  UV_REQ(d >= 4 && d % 4 == 0, "%s: d %d must be a positive multiple of 4 (128-bit loads)", fn, d);
+  UV_REQ(al_(x_txt, 16) && al_(x_vid, 16) && al_(w, 16) && al_(pooled, 16) && al_(saliency, 4) && al_(alpha_out, 4) && al_(logits, 4) &&
+             al_(txt_mask, 4) && al_(vid_mask, 4),
+         "%s: x_txt, x_vid, w and pooled must be 16-byte aligned", fn);
+  PoolSalArgs a;
+  a.x_txt = x_txt;
+  a.x_vid = x_vid;
+  a.txt_mask = txt_mask;
+  a.vid_mask = vid_mask;
+  a.w = w;
+  a.pooled = pooled;
+  a.saliency = saliency;
+  a.alpha_out = alpha_out;
+  a.logits_ws = logits;
+  a.B = B;
+  a.Lt = Lt;
+  a.Lv = Lv;
+  a.d = d;
+  return launch_pool_saliency(a, (cudaStream_t)stream);
+}
+
+int univtg_op_conv_head_final(const void* h_cls, const void* h_span, const float* w_cls, const float* w_span, const float* b_cls,
+                              const float* b_span, float* pred_logits, float* pred_spans, int32_t B, int32_t Lv, int32_t d, int32_t fmt,
+                              void* stream) {
+  const char* fn = "univtg_op_conv_head_final";
+  UV_REQ(h_cls && h_span && w_cls && w_span && b_cls && b_span && pred_logits && pred_spans, "%s: null pointer argument", fn);
+  UV_REQ(B >= 1 && Lv >= 1, "%s: B %d / Lv %d", fn, B, Lv);
+  UV_REQ(d >= 2 && d % 2 == 0, "%s: d %d must be even (32-bit loads)", fn, d);
+  UV_REQ(fmt >= 0 && fmt <= 2, "%s: fmt %d (0 fp16, 1 bf16, 2 fp16x3)", fn, fmt);
+  UV_REQ(al_(h_cls, 4) && al_(h_span, 4) && al_(w_cls, 4) && al_(w_span, 4) && al_(b_cls, 4) && al_(b_span, 4) && al_(pred_logits, 4) &&
+             al_(pred_spans, 4),
+         "%s: h_cls / h_span must be 4-byte aligned", fn);
+  HeadFinalArgs a;
+  a.h_cls = reinterpret_cast<const uint16_t*>(h_cls);
+  a.h_span = reinterpret_cast<const uint16_t*>(h_span);
+  a.w_cls = w_cls;
+  a.w_span = w_span;
+  a.b_cls = b_cls;
+  a.b_span = b_span;
+  a.pred_logits = pred_logits;
+  a.pred_spans = pred_spans;
+  a.B = B;
+  a.Lv = Lv;
+  a.d = d;
+  a.fmt = fmt == 2 ? 0 : fmt;
+  a.split = fmt == 2;
+  a.lo = fmt == 2 ? ((long long)B * (Lv + 1) + 2) * d : 0;
+  return launch_conv_head_final(a, (cudaStream_t)stream);
+}
+
+int univtg_op_attention_fwd(const univtg_attn_fwd* q, const univtg_rng* rng, float p, int32_t layer, int32_t* kernel_used, void* stream) {
+  const char* fn = "univtg_op_attention_fwd";
+  UV_REQ(q != nullptr, "%s: null args", fn);
+  UV_REQ(q->qkv && q->key_mask && q->out, "%s: null qkv, key_mask or out", fn);
+  UV_REQ(q->B >= 1 && q->L >= 1 && q->H >= 1 && q->dh >= 1, "%s: B %d / L %d / H %d / dh %d", fn, q->B, q->L, q->H, q->dh);
+  UV_REQ(q->fmt >= 0 && q->fmt <= 2, "%s: fmt %d (0 fp16, 1 bf16, 2 fp16x3)", fn, q->fmt);
+  UV_REQ(q->impl == 0 || q->impl == 1, "%s: impl %d (0 tensor cores, 1 SIMT)", fn, q->impl);
+  UV_REQ(q->impl == 1 || q->dh == 64 || q->dh == 128, "%s: tensor-core attention needs dh 64 or 128, got %d", fn, q->dh);
+  UV_REQ(q->impl == 0 || q->L <= 12288, "%s: SIMT attention stages L %d <= 12288 scores per warp", fn, q->L);
+  UV_REQ(!q->causal || (q->impl == 0 && q->dh == 64 && q->fmt != 2 && !(p > 0.f)), "%s: causal needs impl 0, dh 64, fmt 0/1, p 0", fn);
+  UV_REQ(p >= 0.f && p < 1.f && (!(p > 0.f) || (rng && q->fmt != 2 && layer >= 0)), "%s: p %g needs rng, fmt 0/1 and layer >= 0", fn,
+         (double)p);
+  UV_REQ(al_(q->qkv, 16) && al_(q->out, 4) && al_(q->key_mask, 4) && al_(q->lse, 4), "%s: qkv must be 16-byte and out 4-byte aligned",
+         fn);
+  AttnArgs a;
+  memset(&a, 0, sizeof(a));
+  const int d = q->H * q->dh;
+  a.key_mask = q->key_mask;
+  a.out = reinterpret_cast<uint16_t*>(q->out);
+  a.lse = q->lse;
+  a.scale = 1.0f / sqrtf((float)q->dh);
+  a.B = q->B;
+  a.L = q->L;
+  a.H = q->H;
+  a.dh = q->dh;
+  a.d = d;
+  a.fmt = q->fmt == 2 ? 0 : q->fmt;
+  a.split = q->fmt == 2;
+  a.causal = q->causal;
+  if (a.split) {
+    a.lo_qkv = (long long)q->B * q->L * 3 * d;
+    a.lo_out = (long long)q->B * q->L * d;
+  }
+  if (p > 0.f) a.drop = make_drop_spec(rng->seed, (unsigned int)layer, p);
+  if (kernel_used) *kernel_used = -1;
+  if (q->impl == 1) return launch_attention_simt(a, reinterpret_cast<const uint16_t*>(q->qkv), (cudaStream_t)stream, kernel_used);
+  if (make_tmap_op(&a.tm_qkv, q->qkv, (uint64_t)q->B * q->L, (uint64_t)3 * d, (uint64_t)3 * d, 128, 64, a.lo_qkv)) return 1;
+  return launch_attention(a, (cudaStream_t)stream, kernel_used);
 }
 
 int univtg_op_attention(const void* qkv, const float* key_mask, void* out, float* lse, int32_t B, int32_t L, int32_t H,

@@ -554,7 +554,7 @@ static int launch_tc_drop(const AttnArgs& a, cudaStream_t stream) {
   return a.drop.on ? launch_tc<DH, BF, 1>(a, stream) : launch_tc<DH, BF, 0>(a, stream);
 }
 
-int launch_attention_simt(const AttnArgs& a, const uint16_t* qkv, cudaStream_t stream) {
+int launch_attention_simt(const AttnArgs& a, const uint16_t* qkv, cudaStream_t stream, int* kernel_used) {
   AttnSimtArgs s{qkv, a.key_mask, a.out, a.lse, a.scale, a.B, a.L, a.H, a.dh, a.d, a.fmt, a.drop, a.lo_qkv, a.lo_out};
   const int warps = a.B * a.H * a.L;
   const size_t smem = (size_t)4 * a.L * sizeof(float);
@@ -571,17 +571,19 @@ int launch_attention_simt(const AttnArgs& a, const uint16_t* qkv, cudaStream_t s
     }
   }
   launch_k(kern, dim3((warps + 3) / 4), dim3(128), smem, stream, s);
+  if (kernel_used) *kernel_used = a.split ? ATT_SIMT_SPLIT : a.drop.on ? ATT_SIMT_DROP : ATT_SIMT;
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) set_error("attention_simt launch failed: %s", cudaGetErrorString(e));
   return (int)e;
 }
 
-int launch_attention(const AttnArgs& a, cudaStream_t stream) {
+int launch_attention(const AttnArgs& a, cudaStream_t stream, int* kernel_used) {
   if (a.causal) {
     if (a.dh != 64 || a.split || a.drop.on) {
       set_error("launch_attention: the causal mask needs dh = 64, fp16 or bf16 operands and no dropout");
       return (int)cudaErrorInvalidValue;
     }
+    if (kernel_used) *kernel_used = ATT_CAUSAL + (a.fmt ? 1 : 0);
     return a.fmt ? launch_tc_causal<1>(a, stream) : launch_tc_causal<0>(a, stream);
   }
   if (a.split) {
@@ -589,11 +591,14 @@ int launch_attention(const AttnArgs& a, cudaStream_t stream) {
       set_error("launch_attention: fp16x3 needs fmt 0 and no dropout");
       return (int)cudaErrorInvalidValue;
     }
+    if (kernel_used) *kernel_used = a.dh == 128 ? ATT_SPLIT128 : ATT_SPLIT64;
     if (a.dh == 128) return launch_tc_split<128>(a, stream);
     if (a.dh == 64) return launch_tc_split<64>(a, stream);
   }
+  if (kernel_used) *kernel_used = ATT_TC + (a.dh == 128 ? 4 : 0) + (a.fmt ? 2 : 0) + (a.drop.on ? 1 : 0);
   if (a.dh == 128) return a.fmt ? launch_tc_drop<128, 1>(a, stream) : launch_tc_drop<128, 0>(a, stream);
   if (a.dh == 64) return a.fmt ? launch_tc_drop<64, 1>(a, stream) : launch_tc_drop<64, 0>(a, stream);
+  if (kernel_used) *kernel_used = -1;
   set_error("launch_attention: tensor-core path needs dh in {64,128}, got %d", a.dh);
   return (int)cudaErrorInvalidValue;
 }

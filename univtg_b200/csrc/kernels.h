@@ -35,6 +35,9 @@ struct GemmProblem {
   int b_box_rows;    // rows of tm_b's TMA box (K-major B): must equal the launch's bn (bn/2 for cluster pairs); checked at launch
   int M, N;
   int taps;          // 1 = plain; 3 = k=3 conv expressed as 3 K segments
+                     // Forward conv (conv_fwd_problem, plan.h) over the conv-head layout [B*(Lv+1)+2, C] (buffer row = logical row + 1):
+                     // A rows 0 and M+1 and every sample's separator row must hold zeros; with rps_in = rps_out = Lv+1, row_off = 1 and
+                     // zero_sep the epilogue writes buffer rows 1..M (separators as exact zeros) and never rows 0 and M+1.
   int kblk_per_tap;  // 64-wide k-blocks per tap
   int ksplit;        // >=1; k-blocks are split over `ksplit` tiles that accumulate atomically into out32, which the caller must have
                      // zeroed (or filled with what the sum should be added to).  ksplit > 1 and `accumulate` are rejected together

@@ -17,6 +17,16 @@ using namespace uv;
 namespace {
 
 inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
+
+// Host-side argument checks of the single-operator entry points: the message names the offending argument.
+#define UV_REQ(cond, ...)      \
+  do {                         \
+    if (!(cond)) {             \
+      set_error(__VA_ARGS__);  \
+      return 1;                \
+    }                          \
+  } while (0)
+inline bool al_(const void* p, int bytes) { return (reinterpret_cast<uintptr_t>(p) & (uintptr_t)(bytes - 1)) == 0; }
 inline int pad64(int k) { return (k + 63) / 64 * 64; }
 
 // ------------------------------------------------------------------------------------------------
@@ -63,6 +73,10 @@ bool check_cfg(const univtg_config* c) {
   }
   if (c->hidden_dim <= 0 || c->hidden_dim % 64 != 0) {
     set_error("hidden_dim %d must be a positive multiple of 64", c->hidden_dim);
+    return false;
+  }
+  if (c->hidden_dim > 3072) {
+    set_error("hidden_dim %d exceeds 3072, the widest LayerNorm that adds the residual branch in the same kernel", c->hidden_dim);
     return false;
   }
   if (c->nheads <= 0 || c->hidden_dim % c->nheads != 0) {
@@ -428,6 +442,25 @@ int setup_gemm(GemmProblem& p, Mat16 A, int a_mn, Mat16 B, int b_mn, int M, int 
     p.cb = OperandCoord{0, 1, 0, 0, 0, 0, 0, 1};
   }
   return rc;
+}
+
+// k=3 Conv1d (padding 1) forward in the conv-head layout (buffer row = logical row + 1; rows 0 and Mh + 1 and every sample's
+// separator row of X are zeros): Y[m] = sum_t X[m + t - 1] W[:, :, t] over Mh logical rows.  A = X [Mh + 2, Cin] (pitch lda,
+// K-major, row-shifted by the tap), B = packed W [N, 3 Cin] (K-major, w2[o, t * Cin + c] = W[o, c, t]); K = 3 taps x Cin
+// (Cin % 64 == 0).  lo_a / lo_b > 0: fp16x3 operands whose lo planes lie that many elements after X / W.
+int conv_fwd_problem(GemmProblem& p, int Mh, const uint16_t* X, int lda, int Cin, const uint16_t* Wp, int N, int bn, long long lo_a = 0,
+                     long long lo_b = 0) {
+  init_problem(p);
+  p.M = Mh;
+  p.N = N;
+  p.taps = 3;
+  p.kblk_per_tap = Cin / 64;
+  p.ca = OperandCoord{0, 0, 0, 1, 0, 1, 1, 0};    // rows m0 + t (buffer row of logical row m0 + t - 1), cols k
+  p.cb = OperandCoord{0, 0, Cin, 1, 0, 1, 0, 0};  // cols t * Cin + k, rows n0
+  int r = make_tmap_op(&p.tm_a, X, (uint64_t)Mh + 2, (uint64_t)Cin, (uint64_t)lda, GEMM_BM, 64, lo_a);
+  r |= make_tmap_op(&p.tm_b, Wp, (uint64_t)N, (uint64_t)3 * Cin, (uint64_t)3 * Cin, (uint32_t)bn, 64, lo_b);
+  p.b_box_rows = bn;
+  return r;
 }
 
 // k=3 Conv1d backward in the conv-head layout (buffer row = logical row + 1; rows 0, Mh + 1 and every sample's separator row are

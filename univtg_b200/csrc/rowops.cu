@@ -364,53 +364,70 @@ __global__ void __launch_bounds__(128) layernorm_rows_block2_kernel(const LnArgs
 }
 
 template <bool SPLIT>
-static int launch_layernorm_impl(const LnArgs& a, cudaStream_t stream) {
+static int launch_layernorm_impl(const LnArgs& a, cudaStream_t stream, int* kernel_used) {
   const int threads = 256;
   const int blocks = (a.rows * 32 + threads - 1) / threads;
   const bool vec_ok = (a.ld_in % 4 == 0) && (a.ld16 == a.d) &&
                       (a.in16 ? (reinterpret_cast<uintptr_t>(a.in16) & 7) == 0 : (reinterpret_cast<uintptr_t>(a.in) & 15) == 0);
+  int k;
   if (a.pos_txt != nullptr) {  // LayerNorm 2 of an encoder layer with learned text positions (out16p of the next layer)
     if (!a.out16p || a.L <= 0 || a.d > 128 * 24) {
       set_error("layernorm: text positions need the structured q/k operand and d <= 3072");
       return (int)cudaErrorInvalidValue;
     }
-    if (vec_ok && a.d == 1024) launch_k(layernorm_rows_vec_kernel<8, true, SPLIT>, dim3(blocks), dim3(threads), 0, stream, a);
-    else if (vec_ok && a.d == 512) launch_k(layernorm_rows_vec_kernel<4, true, SPLIT>, dim3(blocks), dim3(threads), 0, stream, a);
-    else if (vec_ok && a.d == 256) launch_k(layernorm_rows_vec_kernel<2, true, SPLIT>, dim3(blocks), dim3(threads), 0, stream, a);
-    else if (a.d <= 128 * 8) launch_k(layernorm_rows_block_kernel<8, true, SPLIT>, dim3(a.rows), dim3(128), 0, stream, a);
-    else launch_k(layernorm_rows_block_kernel<24, true, SPLIT>, dim3(a.rows), dim3(128), 0, stream, a);
-  } else if (vec_ok && a.d == 1024) launch_k(layernorm_rows_vec_kernel<8, false, SPLIT>, dim3(blocks), dim3(threads), 0, stream, a);
-  else if (vec_ok && a.d == 512) launch_k(layernorm_rows_vec_kernel<4, false, SPLIT>, dim3(blocks), dim3(threads), 0, stream, a);
-  else if (vec_ok && a.d == 256) launch_k(layernorm_rows_vec_kernel<2, false, SPLIT>, dim3(blocks), dim3(threads), 0, stream, a);
+    if (vec_ok && a.d == 1024) k = LN_VEC8_TXT;
+    else if (vec_ok && a.d == 512) k = LN_VEC4_TXT;
+    else if (vec_ok && a.d == 256) k = LN_VEC2_TXT;
+    else if (a.d <= 128 * 8) k = LN_BLOCK8_TXT;
+    else k = LN_BLOCK24_TXT;
+  } else if (vec_ok && a.d == 1024) k = LN_VEC8;
+  else if (vec_ok && a.d == 512) k = LN_VEC4;
+  else if (vec_ok && a.d == 256) k = LN_VEC2;
   else if (a.d > 1024 && a.d <= 1024 * 3 && a.d % 2 == 0 && a.ld_in % 2 == 0 && a.ld16 % 2 == 0 && a.out16 && !a.out32 &&
            !a.out16p && !a.outc && !a.add16 && (a.in16 ? (reinterpret_cast<uintptr_t>(a.in16) & 3) == 0 : (reinterpret_cast<uintptr_t>(a.in) & 7) == 0) &&
            (reinterpret_cast<uintptr_t>(a.gamma) & 7) == 0 && (reinterpret_cast<uintptr_t>(a.beta) & 7) == 0 &&
            (!a.mul32 || (reinterpret_cast<uintptr_t>(a.mul32) & 7) == 0))
-    launch_k(layernorm_rows_block2_kernel<12, SPLIT>, dim3(a.rows), dim3(128), 0, stream, a);
-  else if (a.d <= 128 * 8) launch_k(layernorm_rows_block_kernel<8, false, SPLIT>, dim3(a.rows), dim3(128), 0, stream, a);
-  else if (a.d <= 128 * 24) launch_k(layernorm_rows_block_kernel<24, false, SPLIT>, dim3(a.rows), dim3(128), 0, stream, a);
+    k = LN_BLOCK2_12;
+  else if (a.d <= 128 * 8) k = LN_BLOCK8;
+  else if (a.d <= 128 * 24) k = LN_BLOCK24;
   else {
     if (a.add16) {
       set_error("layernorm: fused branch add needs d <= 3072");
       return (int)cudaErrorInvalidValue;
     }
-    launch_k(layernorm_rows_generic_kernel<SPLIT>, dim3(blocks), dim3(threads), 0, stream, a);
+    k = LN_GENERIC;
   }
+  const dim3 vec_grid(blocks), vec_block(threads), row_grid(a.rows), row_block(128);
+  switch (k) {
+    case LN_VEC8: launch_k(layernorm_rows_vec_kernel<8, false, SPLIT>, vec_grid, vec_block, 0, stream, a); break;
+    case LN_VEC4: launch_k(layernorm_rows_vec_kernel<4, false, SPLIT>, vec_grid, vec_block, 0, stream, a); break;
+    case LN_VEC2: launch_k(layernorm_rows_vec_kernel<2, false, SPLIT>, vec_grid, vec_block, 0, stream, a); break;
+    case LN_VEC8_TXT: launch_k(layernorm_rows_vec_kernel<8, true, SPLIT>, vec_grid, vec_block, 0, stream, a); break;
+    case LN_VEC4_TXT: launch_k(layernorm_rows_vec_kernel<4, true, SPLIT>, vec_grid, vec_block, 0, stream, a); break;
+    case LN_VEC2_TXT: launch_k(layernorm_rows_vec_kernel<2, true, SPLIT>, vec_grid, vec_block, 0, stream, a); break;
+    case LN_BLOCK8: launch_k(layernorm_rows_block_kernel<8, false, SPLIT>, row_grid, row_block, 0, stream, a); break;
+    case LN_BLOCK24: launch_k(layernorm_rows_block_kernel<24, false, SPLIT>, row_grid, row_block, 0, stream, a); break;
+    case LN_BLOCK8_TXT: launch_k(layernorm_rows_block_kernel<8, true, SPLIT>, row_grid, row_block, 0, stream, a); break;
+    case LN_BLOCK24_TXT: launch_k(layernorm_rows_block_kernel<24, true, SPLIT>, row_grid, row_block, 0, stream, a); break;
+    case LN_BLOCK2_12: launch_k(layernorm_rows_block2_kernel<12, SPLIT>, row_grid, row_block, 0, stream, a); break;
+    default: launch_k(layernorm_rows_generic_kernel<SPLIT>, vec_grid, vec_block, 0, stream, a); break;
+  }
+  if (kernel_used) *kernel_used = k + (SPLIT ? LN_SPLIT : 0);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) set_error("layernorm launch failed: %s", cudaGetErrorString(e));
   return (int)e;
 }
 
-int launch_layernorm(const LnArgs& a, cudaStream_t stream) {
+int launch_layernorm(const LnArgs& a, cudaStream_t stream, int* kernel_used) {
   if (a.rows <= 0) return 0;
   if (a.split) {
     if (a.fmt != 0 || a.mul32 != nullptr || a.drop.on) {
       set_error("layernorm: fp16x3 output needs fmt 0 and no dropout");
       return (int)cudaErrorInvalidValue;
     }
-    return launch_layernorm_impl<true>(a, stream);
+    return launch_layernorm_impl<true>(a, stream, kernel_used);
   }
-  return launch_layernorm_impl<false>(a, stream);
+  return launch_layernorm_impl<false>(a, stream, kernel_used);
 }
 
 // ------------------------------------------------------------------------------------------------

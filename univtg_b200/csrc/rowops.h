@@ -37,7 +37,13 @@ struct LnArgs {
   int split;           // 1: fp16x3 (fmt 0, inference): add16 is read and out16 / out16p / outc are written as hi / lo pairs
   long long lo;        // split: elements from each of those buffers to its lo plane
 };
-int launch_layernorm(const LnArgs& a, cudaStream_t stream);
+// Instantiation launch_layernorm routed a call to (kernel_used): vec<NV> keeps d = 128 NV in registers, block<EPT> takes
+// d <= 128 EPT one row per CTA, block2 the wide projector input, generic any d; _TXT adds pos_txt; + LN_SPLIT for fp16x3.
+enum LnKernel {
+  LN_VEC8 = 0, LN_VEC4, LN_VEC2, LN_VEC8_TXT, LN_VEC4_TXT, LN_VEC2_TXT, LN_BLOCK8, LN_BLOCK24, LN_BLOCK8_TXT, LN_BLOCK24_TXT,
+  LN_BLOCK2_12, LN_GENERIC, LN_SPLIT = 12, LN_NUM_KERNELS = 24
+};
+int launch_layernorm(const LnArgs& a, cudaStream_t stream, int* kernel_used = nullptr);
 
 // Learned text positions (txt_position_embed, reference model/position_encoding.py:19-41), one warp per text row r = b*Lt + l:
 //   pos[r] = drop(LayerNorm(xt[r] + table[l])) (eps 1e-5), and the text row b*L + Lv + l of xpos16 becomes 16-bit(xt[r] + pos[r])
@@ -109,9 +115,13 @@ struct AttnArgs {
   long long lo_qkv, lo_out;  // split: elements from qkv / out to their lo planes
   int causal;             // 1: query i attends to keys j <= i only (dh = 64, tensor cores, no dropout, no split)
 };
-int launch_attention(const AttnArgs& a, cudaStream_t stream);
+// Instantiation a launch ran (kernel_used): ATT_TC + 4 (dh == 128) + 2 bf16 + dropout, the causal kernel per format, the fp16x3
+// kernel per head size, and the three SIMT kernels.
+enum AttnKernel { ATT_TC = 0, ATT_CAUSAL = 8, ATT_SPLIT64 = 10, ATT_SPLIT128 = 11, ATT_SIMT = 12, ATT_SIMT_DROP = 13, ATT_SIMT_SPLIT = 14,
+                  ATT_NUM_KERNELS = 15 };
+int launch_attention(const AttnArgs& a, cudaStream_t stream, int* kernel_used = nullptr);
 // SIMT variant for head sizes outside {64,128}; reads qkv through a plain pointer.
-int launch_attention_simt(const AttnArgs& a, const uint16_t* qkv, cudaStream_t stream);
+int launch_attention_simt(const AttnArgs& a, const uint16_t* qkv, cudaStream_t stream, int* kernel_used = nullptr);
 // out [B, H, L, L] f32: the attention-dropout multipliers of `spec` (row = query, column = key), as the kernels apply them
 int launch_attention_dropout_mask(const DropSpec& spec, int B, int H, int L, float* out, cudaStream_t stream);
 

@@ -896,15 +896,8 @@ int univtg_op_attention_bwd(const void* qkv, const void* dO, const void* O, cons
 }
 
 // ---- single backward operators: thin wrappers over the launchers univtg_backward uses.  Each checks on the host what its kernel
-// assumes (null pointers, vector widths, alignment, size limits) and names the offending argument before anything is launched. ----
-#define UV_REQ(cond, ...)      \
-  do {                         \
-    if (!(cond)) {             \
-      set_error(__VA_ARGS__);  \
-      return 1;                \
-    }                          \
-  } while (0)
-static bool al_(const void* p, int bytes) { return (reinterpret_cast<uintptr_t>(p) & (uintptr_t)(bytes - 1)) == 0; }
+// assumes (null pointers, vector widths, alignment, size limits; UV_REQ, plan.h) and names the offending argument before anything is
+// launched. ----
 
 int univtg_op_gemm_group(univtg_gemm_problem* problems, int32_t num, int32_t fmt, int32_t bn, int32_t cluster, int32_t* full,
                          void* stream) {
@@ -956,8 +949,16 @@ int univtg_op_gemm_group(univtg_gemm_problem* problems, int32_t num, int32_t fmt
       UV_REQ(q.a_mn && q.b_mn && q.tap >= 0 && q.tap <= 2, "%s: problem %d: conv wgrad needs a_mn = b_mn = 1 and tap in 0..2", fn, i);
       rc = conv_wgrad_problem(p, q.K, reinterpret_cast<const uint16_t*>(q.a), q.lda, q.M, reinterpret_cast<const uint16_t*>(q.b), q.ldb,
                               q.N, q.tap, bn, fg, fw);
+    } else if (q.conv == 3) {
+      UV_REQ(!q.a_mn && !q.b_mn && q.K % 192 == 0, "%s: problem %d: forward conv needs a_mn = b_mn = 0 and K = 3 Cin with Cin %% 64 == 0",
+             fn, i);
+      UV_REQ(q.lda >= q.K / 3 && q.ldb == q.K, "%s: problem %d: forward conv needs lda >= Cin and weight pitch ldb = K", fn, i);
+      UV_REQ(cluster == 1, "%s: problem %d: forward conv runs without clusters", fn, i);
+      rc = conv_fwd_problem(p, q.M, reinterpret_cast<const uint16_t*>(q.a), q.lda, q.K / 3, reinterpret_cast<const uint16_t*>(q.b), q.N, bn);
+      p.a_fmt = q.a_fmt;
+      p.b_fmt = q.b_fmt;
     } else {
-      UV_REQ(q.conv == 0, "%s: problem %d: conv %d (0 plain, 1 dgrad, 2 wgrad)", fn, i, q.conv);
+      UV_REQ(q.conv == 0, "%s: problem %d: conv %d (0 plain, 1 dgrad, 2 wgrad, 3 forward)", fn, i, q.conv);
       const Mat16 A = q.a_mn ? Mat16{reinterpret_cast<const uint16_t*>(q.a), q.K, q.M, q.lda}
                              : Mat16{reinterpret_cast<const uint16_t*>(q.a), q.M, q.K, q.lda};
       const Mat16 Bm = q.b_mn ? Mat16{reinterpret_cast<const uint16_t*>(q.b), q.K, q.N, q.ldb}
