@@ -473,6 +473,25 @@ int univtg_eval_mr(const double* pred, const int32_t* n_pred, const double* gt, 
 int univtg_eval_hl(const double* sal, const int32_t* n_sal, const uint16_t* labels, const int32_t* n_clips, int32_t Q, int32_t S,
                    int32_t C, double* scratch, double* ap, double* hit, void* stream);
 
+/* Per-(video, annotator) AP of the reference's TVSum / YouTube highlight evaluation (main/dataset.py DatasetHL.evaluate), IEEE
+ * double, equal to the reference's Python floats bit for bit; univtg_b200/metrics.py evaluate_hl packs and averages.
+ *   scores [V,S] f32: row v holds the n_score[v] (0..S, S <= 4096) scores the reference argsorts, ranked as torch.argsort(
+ *   descending=True) on the CPU ranks them (libstdc++ std::sort, ties included).  labels [V,C,A] f32: n_label[v] (n_score[v]..C,
+ *   C <= 4096) rows of A (1..32) annotator columns; a clip is positive for annotator a when its label is > the lower median of
+ *   column a (median = 1, TVSum) or > 0 (median = 0, YouTube).  ap [V,A] = the reference's AP recursion over the first n_cut[v]
+ *   (0..n_score[v]) ranked clips, 0 when none of them is positive. */
+int univtg_eval_hl_topk(const float* scores, const int32_t* n_score, const int32_t* n_cut, const float* labels,
+                        const int32_t* n_label, int32_t V, int32_t S, int32_t C, int32_t A, int32_t median, double* ap,
+                        void* stream);
+/* Maximum-weight bipartite matching of QFVS semantic evaluation (eval/qfvs.py calculate_semantic_matching), one per query.
+ * Query q matches the machine-summary shots a[a_off[q] .. a_off[q+1]) with the ground-truth shots b[b_off[q] .. b_off[q+1]),
+ * each a 64-bit mask of its tags (1..max_side per side, max_side <= 1024); the weight of a pair is popcount(x & y) /
+ * popcount(x | y) (0 when both are empty).  s [Q] f64 = the total weight of a maximum-weight matching (Hungarian method, fp64
+ * potentials).  The sides are read from the offsets on the device; a query with an empty side or a side longer than max_side
+ * gets s = NaN, so the caller passes the largest side it packed. */
+int univtg_qfvs_match(const uint64_t* a, const int32_t* a_off, const uint64_t* b, const int32_t* b_off, int32_t Q,
+                      int32_t max_side, double* s, void* stream);
+
 /* LayerNorm rows: in [rows,d] f32 -> out32 [rows,d] f32 and/or out16 [rows,ld16] 16-bit (zero padded). */
 int univtg_op_layernorm(const float* in, int32_t rows, int32_t d, const float* gamma, const float* beta, float eps,
                         int32_t fmt, float* out32, void* out16, int32_t ld16, void* stream);

@@ -16,7 +16,11 @@ submission, duplicate qids, a query without predicted windows, a ground-truth en
 windows, int(duration / 2) outside 1..4096, empty or out-of-range relevant_clip_ids, an empty or (within the first
 int(duration / 2) clips) non-finite predicted saliency list.  A qid mismatch under match_number=True raises AssertionError, as
 the reference does.  Nothing is printed.  CUDA only.
+
+evaluate_hl (bottom of this module) does the same for the TVSum / YouTube highlight evaluation of main/dataset.py.
 """
+import json
+import os
 from collections import OrderedDict
 from itertools import chain
 
@@ -245,3 +249,143 @@ def eval_submission(submission, ground_truth, verbose=True, match_number=True):
     final["brief"] = brief
     final.update(sorted(metrics.items()))
     return final
+
+
+# ---- TVSum / YouTube highlight detection: main/dataset.py DatasetHL.evaluate --------------------------------------------
+TVSUM_ANNOTATORS = 20
+MAX_ANNOTATORS = 32
+HL_SCORE_DTYPES = (torch.float32, torch.float16, torch.bfloat16)  # convert to fp32 without changing order or ties
+
+
+def _hl_rows(blob):
+    rows = []
+    for score in blob:
+        row = score[0]
+        if not torch.is_tensor(row):
+            raise TypeError("evaluate_hl: blob entries must be tensors (the reference argsorts score[0] with torch)")
+        if row.dim() != 1:
+            raise ValueError(f"evaluate_hl: score[0] must be one score row, got shape {list(row.shape)}")
+        if row.dtype not in HL_SCORE_DTYPES:
+            raise ValueError(f"evaluate_hl: scores must be float32, float16 or bfloat16, got {row.dtype}")
+        if row.numel() > MAX_CLIPS:
+            raise ValueError(f"evaluate_hl: more than {MAX_CLIPS} scores in one row")
+        rows.append(row.detach())
+    return rows
+
+
+def pack_hl_labels(dataset, n_videos, lengths, k=5):
+    """-> (labels [V,C,A] f32, n_label [V] i32, n_cut [V] i32, median flag) for the first n_videos videos of `dataset` in its
+    current state.  TVSum: the first 20 columns of `anno`, thresholded on the device at their lower median, n_cut =
+    len(list[:k]); YouTube: [1 if s > 0 else 0 for s in match] in one column, the whole list."""
+    name = dataset.dset_name
+    if name not in ("tvsum", "youtube"):
+        raise NotImplementedError(f"evaluate_hl: dset_name {name!r}")
+    cols, rows_n = [], []
+    for idx in range(n_videos):
+        lab = dataset.label[dataset.get_video_id(idx)]
+        if name == "tvsum":
+            a = np.asarray(lab["anno"], dtype=np.float32)
+            if a.ndim != 2 or a.shape[1] < TVSUM_ANNOTATORS:
+                raise IndexError(f"evaluate_hl: anno of video {idx} has shape {list(a.shape)}, the reference reads 20 columns")
+            a = a[:, :TVSUM_ANNOTATORS]
+        else:
+            a = np.array([1 if s > 0 else 0 for s in lab["match"]], dtype=np.float32).reshape(-1, 1)
+        if lengths[idx] > len(a):
+            raise IndexError(f"evaluate_hl: score row {idx} has {lengths[idx]} entries, its video {len(a)} labels")
+        if len(a) > MAX_CLIPS:
+            raise ValueError(f"evaluate_hl: more than {MAX_CLIPS} labelled clips in one video")
+        if not np.isfinite(a).all():
+            raise ValueError(f"evaluate_hl: non-finite labels in video {idx}")
+        cols.append(a)
+        rows_n.append(len(a))
+    A = cols[0].shape[1]
+    C = max(1, max(rows_n))
+    labels = np.zeros((n_videos, C, A), dtype=np.float32)
+    for v, a in enumerate(cols):
+        labels[v, :len(a)] = a
+    if name == "tvsum":
+        n_cut = [len(range(n)[:k]) for n in lengths]
+    else:
+        n_cut = list(lengths)
+    return labels, np.array(rows_n, dtype=np.int32), np.array(n_cut, dtype=np.int32), int(name == "tvsum")
+
+
+def hl_topk_ap(rows, labels, n_label, n_cut, median):
+    """univtg_eval_hl_topk on finite score rows (1-D tensors on any device) and packed labels -> ap [V, A] float64 numpy."""
+    if not torch.cuda.is_available():
+        raise RuntimeError("univtg_b200: evaluate_hl runs on CUDA only (no CPU path)")
+    lib = _lib.load_library()
+    V, C, A = labels.shape
+    n_score = np.array([r.numel() for r in rows], dtype=np.int32)
+    dev = torch.device("cuda", torch.cuda.current_device())
+    with torch.cuda.device(dev):
+        S = max(1, int(n_score.max()))
+        scores = torch.zeros(V, S, dtype=torch.float32, device=dev)
+        for v, r in enumerate(rows):
+            scores[v, :r.numel()] = r.to(device=dev, dtype=torch.float32)
+        hbuf, hoff = _stage([n_score, n_cut, labels, n_label])
+        dbuf = torch.from_numpy(hbuf).to(dev)
+        ap = torch.empty(V, A, dtype=torch.float64, device=dev)
+        ib = dbuf.data_ptr()
+        _lib.check(lib.univtg_eval_hl_topk(_lib.ptr(scores), _lib.c_void_p(ib + hoff[0]), _lib.c_void_p(ib + hoff[1]),
+                                           _lib.c_void_p(ib + hoff[2]), _lib.c_void_p(ib + hoff[3]), V, S, C, A, median,
+                                           _lib.ptr(ap), _lib.stream_ptr()), "univtg_eval_hl_topk")
+        return ap.cpu().numpy()
+
+
+def _write_hl_jsonl(dataset, blob, save_dir):
+    """The reference's per-video prediction file, <save_dir>/<dset_name>/<domain>.jsonl."""
+    with open(os.path.join(save_dir, dataset.dset_name, dataset.domain + ".jsonl"), "w") as f:
+        for idx, score in enumerate(blob):
+            video_id = dataset.get_video_id(idx)
+            lab = dataset.label[video_id]
+            entry = {"vid": video_id, "pred": score[0].tolist(), "gt": dataset.get_saliency(idx).tolist(),
+                     "duration": int(lab["frames"]) / int(lab["fps"]), "domain": lab["domain"], "fps": lab["fps"]}
+            if dataset.dset_name == "tvsum":
+                entry.update({"title": lab["title"]})
+            if dataset.dset_name == "youtube":
+                entry.update({"clip": lab["clip"]})
+            f.write(json.dumps(entry) + "\n")
+
+
+def evaluate_hl(dataset, blob, k=5, save_dir=None):
+    """main/dataset.py DatasetHL.evaluate on the device: `evaluate_hl(train_val_dataset, scores)` for
+    `train_val_dataset.evaluate(scores)`.  Returns the same {'mAP': round(mean AP, 5)}.
+
+    dataset: anything with dset_name ('tvsum' / 'youtube'), domain, label (video id -> dict with 'anno' [clips, >= 20] or
+    'match' [clips]) and get_video_id(idx) in its 'val' state; get_saliency(idx) is read only for save_dir.
+    blob: the list eval_epoch collects, one tensor per eval batch, on the CPU or CUDA.  As in the reference, row 0 of entry idx
+    is scored against video idx - with eval_bsz 1 that is every video; with the default eval_bsz 100 it is not the video that
+    row belongs to, and only len(blob) videos are evaluated.  This is kept as the reference has it so results stay comparable.
+
+    The ranking is the reference's torch.argsort(descending=True) on the CPU (ties included), TVSum labels are > the lower median
+    of each annotator's column, the APs are computed per (video, annotator) by univtg_eval_hl_topk bit for bit, and the means
+    are the reference's own Python sums (over videos, then over annotators) and round().
+
+    Raises, before any launch: IndexError for a score row longer than its video's labels (or anno with fewer than 20 columns),
+    ZeroDivisionError for an empty blob, TypeError for non-tensor entries, ValueError for non-finite scores or labels, score
+    dtypes other than float32 / float16 / bfloat16 and more than 4,096 clips.  With save_dir the reference's jsonl file is
+    written first, as the reference does.  CUDA only."""
+    if dataset.dset_name not in ("tvsum", "youtube"):
+        raise NotImplementedError(f"evaluate_hl: dset_name {dataset.dset_name!r}")
+    if save_dir is not None:
+        _write_hl_jsonl(dataset, blob, save_dir)
+    rows = _hl_rows(blob)
+    if not rows:
+        raise ZeroDivisionError("evaluate_hl: empty blob")
+    by_device = {}
+    for r in rows:
+        by_device.setdefault(r.device, []).append(r.float())
+    if not all(bool(torch.isfinite(torch.cat(rs)).all()) for rs in by_device.values()):
+        raise ValueError("evaluate_hl: non-finite scores")
+    labels, n_label, n_cut, median = pack_hl_labels(dataset, len(rows), [r.numel() for r in rows], k)
+    ap = hl_topk_ap(rows, labels, n_label, n_cut, median)
+    if median:
+        collected = []
+        for i in range(TVSUM_ANNOTATORS):
+            video_ap = ap[:, i].tolist()
+            collected.append(sum(video_ap) / len(video_ap))
+    else:
+        collected = ap[:, 0].tolist()
+    mean_ap = sum(collected) / len(collected)
+    return dict(mAP=round(mean_ap, 5))

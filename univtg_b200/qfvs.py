@@ -8,7 +8,10 @@ main/train_qfvs.py and main/inference_qfvs.py load through the usual `model_id` 
 The model is the MR/HL `Model` (the reference's QFVS model has the same parameters, state_dict keys and forward); only the
 criterion differs.  Its losses run in the CUDA library (univtg_qfvs_loss_forward / univtg_qfvs_loss_backward) without a host
 synchronisation, where the reference's masked_select, count slice and zero-sum branches synchronise four times per call.
+
+calculate_semantic_matching (bottom of this module) is the drop-in for eval/qfvs.py's evaluation of one oracle summary.
 """
+import numpy as np
 import torch
 
 from . import _lib
@@ -116,3 +119,77 @@ def build_model(args):
     qcrit = QFVSCriterion(weight_dict=crit.weight_dict, losses=crit.losses, eos_coef=crit.eos_coef, temperature=args.temperature,
                           span_loss_type=crit.span_loss_type, max_v_l=crit.max_v_l, saliency_margin=crit.saliency_margin)
     return model, qcrit.to(crit.empty_weight.device)
+
+
+# ---- semantic evaluation: eval/qfvs.py calculate_semantic_matching ----------------------------------------------------------
+MAX_SIDE = 1024  # shots per summary
+MAX_TAGS = 64    # tag columns (Tags.mat has 48)
+
+
+def tag_masks(rows):
+    """Shot-tag rows [n, <= 64] of 0 / 1 -> n uint64 masks (bit c = tag column c)."""
+    t = np.asarray(rows)
+    if t.ndim != 2:
+        raise ValueError(f"semantic matching: the selected tag rows must form a matrix, got shape {list(t.shape)}")
+    if t.shape[1] > MAX_TAGS:
+        raise ValueError(f"semantic matching: more than {MAX_TAGS} tag columns")
+    if not np.isin(t, (0, 1)).all():
+        raise ValueError("semantic matching: tags must be 0 or 1")
+    bits = np.packbits(t.astype(bool), axis=1, bitorder="little")
+    out = np.zeros((len(t), 8), dtype=np.uint8)
+    out[:, :bits.shape[1]] = bits
+    return out.view("<u8").reshape(-1)
+
+
+def match_sums(pairs):
+    """univtg_qfvs_match on [(machine masks, gt masks), ...] (each 1..1024 uint64 masks) -> total matched weight per pair."""
+    sides = [len(x) for p in pairs for x in p]
+    if min(sides) < 1 or max(sides) > MAX_SIDE:
+        raise ValueError(f"semantic matching: each summary must hold 1..{MAX_SIDE} shots")
+    if not torch.cuda.is_available():
+        raise RuntimeError("univtg_b200: calculate_semantic_matching runs on CUDA only (no CPU path)")
+    lib = _lib.load_library()
+    a = np.concatenate([p[0] for p in pairs]).astype(np.uint64)
+    b = np.concatenate([p[1] for p in pairs]).astype(np.uint64)
+    a_off = np.concatenate([[0], np.cumsum([len(p[0]) for p in pairs])]).astype(np.int32)
+    b_off = np.concatenate([[0], np.cumsum([len(p[1]) for p in pairs])]).astype(np.int32)
+    host = np.concatenate([x.view(np.uint8) for x in (a, b, a_off, b_off)])
+    dev = torch.device("cuda", torch.cuda.current_device())
+    with torch.cuda.device(dev):
+        buf = torch.from_numpy(host).to(dev)
+        s = torch.empty(len(pairs), dtype=torch.float64, device=dev)
+        base = buf.data_ptr()
+        oa, ob = 0, a.nbytes
+        oao = ob + b.nbytes
+        obo = oao + a_off.nbytes
+        _lib.check(lib.univtg_qfvs_match(_lib.c_void_p(base + oa), _lib.c_void_p(base + oao), _lib.c_void_p(base + ob),
+                                         _lib.c_void_p(base + obo), len(pairs), max(sides), _lib.ptr(s), _lib.stream_ptr()),
+                   "univtg_qfvs_match")
+        return s.cpu().numpy()
+
+
+def calculate_semantic_matching(machine_summary, gt_summary, video_shots_tag, video_id):
+    """eval/qfvs.py calculate_semantic_matching on the device; same arguments, same (precision, recall, f1) of np.float64.
+
+    machine_summary / gt_summary: shot indices into video_shots_tag[video_id] (a [shots, tags] 0 / 1 matrix, as
+    load_videos_tag returns), indexed with numpy's rules; machine_summary may be the CUDA `top_index` of score.topk as it is.
+    The weight of a (machine, gt) pair is the semantic IoU of their tag sets; the total weight s of a maximum-weight matching
+    comes from univtg_qfvs_match, then p = s / len(machine), r = s / len(gt), f1 = 2*p*r/(p+r) in numpy scalars as the reference
+    computes them.  The reference adds the matched weights in networkx's set order, which depends on the string hash seed, so
+    s agrees with it to the last bits only.  All weights 0 gives (0.0, 0.0, nan), as in the reference.
+
+    Raises, before any launch: IndexError for an index outside the tag rows, ValueError for an empty summary (the reference's
+    scikit-learn error), non-binary tags, more than 64 tag columns or more than 1,024 shots in a summary.  CUDA only."""
+    tags = np.asarray(video_shots_tag[video_id])
+    if torch.is_tensor(machine_summary):
+        machine_summary = machine_summary.cpu().numpy()
+    a_rows, b_rows = tags[machine_summary], tags[gt_summary]
+    for rows, what in ((a_rows, "machine"), (b_rows, "ground-truth")):
+        if rows.ndim == 2 and rows.shape[0] == 0:
+            raise ValueError(f"Found array with 0 sample(s) (shape={rows.shape}) while a minimum of 1 is required: empty {what} summary")
+    a, b = tag_masks(a_rows), tag_masks(b_rows)
+    s = np.float64(match_sums([(a, b)])[0])
+    precision = s / a_rows.shape[0]
+    recall = s / b_rows.shape[0]
+    f1 = 2 * precision * recall / (precision + recall)
+    return precision, recall, f1

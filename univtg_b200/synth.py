@@ -472,3 +472,130 @@ def make_eval_case(seed, n_queries=40, n_windows=10, durations=(150, 149, 148, 6
         k = max(1, n_queries // 5)
         sub, gt = sub[k:], gt[:-k]
     return {"submission": sub, "ground_truth": gt, "match_number": match_number}
+
+
+# ---- TVSum / YouTube highlight evaluation (main/dataset.py DatasetHL.evaluate) --------------------------------------------
+class HLEvalDataset:
+    """The part of the reference's DatasetHL that its evaluate() reads, in the 'val' state: dset_name, domain, label,
+    get_video_id and get_saliency (the latter as main/dataset.py:828-851 computes it)."""
+
+    def __init__(self, dset_name, domain, label, video_ids):
+        self.dset_name, self.domain, self.label = dset_name, domain, label
+        self.video_id = {"train": [], "val": list(video_ids)}
+        self.state = "val"
+
+    def get_video_id(self, idx):
+        return self.video_id[self.state][idx]
+
+    def get_saliency(self, idx):
+        lab = self.label[self.get_video_id(idx)]
+        if self.dset_name == "tvsum":
+            s = torch.Tensor(lab["anno"])
+            return torch.Tensor((s - s.mean()).mean(dim=1))
+        return torch.Tensor([1 if s > 0 else 0 for s in lab["match"]])
+
+
+def make_hl_eval_case(seed, dset_name="tvsum", n_videos=6, clips=(40, 75, 120, 17, 16, 3), shorter=0.3, batch=(1, 3),
+                      tie_frac=0.5):
+    """A deterministic (Python `random`) TVSum or YouTube evaluation input: the label dict of DatasetHL and the score blob
+    eval_epoch collects.
+
+    Video idx has a clip count from `clips`.  TVSum: `anno` [clips, 20] of integers 1..5 (some columns constant, so every label
+    is 0; some with a few high values, so the top 5 holds few positives).  YouTube: `match` of -1 / 0 / 1 / 2 (some videos with
+    no positive clip).  Blob entry idx is a [B, L] float32 tensor (B from `batch`) whose row 0 scores video idx: L is the clip
+    count, or with probability `shorter` fewer clips.  With probability `tie_frac` a row's scores are multiples of 1/8 (many
+    ties, in runs longer than 16 clips for long videos), else fp16-rounded uniforms.
+    Returns {"dataset": HLEvalDataset, "blob": [tensor], "labels": [anno or match per video]}."""
+    rng = random.Random(seed)
+    label, ids, labels, blob = {}, [], [], []
+    for idx in range(n_videos):
+        n = clips[idx % len(clips)]
+        vid = f"{dset_name}_{seed}_{idx}"
+        meta = {"frames": 30 * 2 * n + rng.randrange(60), "fps": 30, "domain": "BK" if dset_name == "tvsum" else "dog"}
+        if dset_name == "tvsum":
+            anno = []
+            kinds = [rng.random() for _ in range(20)]
+            for _ in range(n):
+                row = []
+                for c in range(20):
+                    if kinds[c] < 0.15:
+                        row.append(3)
+                    elif kinds[c] < 0.35:
+                        row.append(5 if rng.random() < 0.1 else 1)
+                    else:
+                        row.append(rng.randint(1, 5))
+                anno.append(row)
+            meta.update(anno=anno, title=f"title {idx}")
+            labels.append(anno)
+        else:
+            none = rng.random() < 0.15
+            match = [rng.choice([-1, 0]) if none else rng.choice([-1, 0, 1, 1, 2]) for _ in range(n)]
+            meta.update(match=match, clip=f"clip{idx}")
+            labels.append(match)
+        label[vid] = meta
+        ids.append(vid)
+        L = rng.randint(0, n) if rng.random() < shorter else n
+        B = rng.randint(*batch)
+        rows = []
+        for _ in range(B):
+            if rng.random() < tie_frac:
+                rows.append([rng.randrange(-8, 9) / 8 for _ in range(L)])
+            else:
+                rows.append([_half(rng.uniform(-2, 2)) for _ in range(L)])
+        blob.append(torch.tensor(rows, dtype=torch.float32).reshape(B, L))
+    return {"dataset": HLEvalDataset(dset_name, "BK" if dset_name == "tvsum" else "dog", label, ids), "blob": blob,
+            "labels": labels}
+
+
+# ---- QFVS semantic matching (eval/qfvs.py calculate_semantic_matching) ----------------------------------------------------
+def make_shot_tags(seed, n_shots, n_tags=48, max_set=31, zero_frac=0.01):
+    """[n_shots, n_tags] uint8 0 / 1 with the statistics of the reference's Tags.mat: 1..max_set tags per shot, most shots with
+    a few popular tags (so many pairs overlap and weights repeat), about zero_frac shots without any tag."""
+    import numpy as np
+
+    rng = random.Random(seed)
+    popular = [1.0 / (c + 1) for c in range(n_tags)]
+    order = list(range(n_tags))
+    rng.shuffle(order)
+    out = np.zeros((n_shots, n_tags), dtype=np.uint8)
+    for i in range(n_shots):
+        if rng.random() < zero_frac:
+            continue
+        k = min(max_set, 1 + int(rng.expovariate(1 / 4)))
+        cols = set()
+        while len(cols) < k:
+            cols.add(order[rng.choices(range(n_tags), weights=popular)[0]])
+        out[i, sorted(cols)] = 1
+    return out
+
+
+def make_qfvs_match_case(seed, n_shots, n_machine, n_gt, zero_frac=0.01):
+    """Tags of one video and a machine / ground-truth summary pair (sorted shot indices, as topk + the oracle summary files
+    give them; both may share shots).  Returns {"tags", "machine", "gt"}."""
+    rng = random.Random(seed + 1)
+    tags = make_shot_tags(seed, n_shots, zero_frac=zero_frac)
+    machine = sorted(rng.sample(range(n_shots), n_machine))
+    gt = sorted(rng.sample(range(n_shots), n_gt))
+    return {"tags": tags, "machine": machine, "gt": gt}
+
+
+def make_qfvs_permutation_case(seed, n, extra=0, n_tags=48):
+    """A matching with a known optimum: n distinct non-empty tag sets built around a shared core (many pairs overlap heavily);
+    the ground truth is the same n shots in a hidden order plus `extra` shots that overlap them less.  Identical pairs weigh 1
+    and every other pair less, so the maximum total weight is exactly n.  Returns {"tags", "machine", "gt", "optimum"}."""
+    import numpy as np
+
+    rng = random.Random(seed)
+    core = rng.sample(range(n_tags), 8)
+    seen, rows = set(), []
+    while len(rows) < n + extra:
+        cols = frozenset(rng.sample(core, rng.randint(3, 6)) + rng.sample(range(n_tags), rng.randint(1, 6)))
+        if cols not in seen:
+            seen.add(cols)
+            rows.append(sorted(cols))
+    tags = np.zeros((n + extra, n_tags), dtype=np.uint8)
+    for i, cols in enumerate(rows):
+        tags[i, cols] = 1
+    gt = list(range(n + extra))
+    rng.shuffle(gt)
+    return {"tags": tags, "machine": list(range(n)), "gt": gt, "optimum": float(n)}
