@@ -27,6 +27,7 @@ Reference lines each function follows (paths relative to the UniVTG repository r
 import math
 
 import torch
+import torch.nn.functional as F
 
 _ERF_C = 1.0 / math.sqrt(2.0)
 
@@ -233,7 +234,12 @@ def criterion(outputs, targets, eos_coef=0.1, temperature=0.07, losses=("spans",
         w = torch.zeros_like(p)
         w[valid] = eos_coef
         w[fg] = 1.0
-        bce = -(y * torch.log(p).clamp(min=-100) + (1 - y) * torch.log(1 - p).clamp(min=-100)) * w
+        # torch's BCE: logs clamped at -100, backward w (p - y) / max(p (1 - p), 1e-12), finite at p = 0 and p = 1.  It refuses to
+        # run inside an autocast region (bench.py's bf16-autocast baseline runs this criterion), so it is evaluated outside one,
+        # in fp32 or wider.
+        with torch.autocast(p.device.type, enabled=False):
+            pw = p if p.dtype == torch.float64 else p.float()
+            bce = F.binary_cross_entropy(pw, y.to(pw.dtype), weight=w.to(pw.dtype), reduction="none")
         res["loss_f"] = (bce * valid.to(dtype)).sum() / valid.sum()
     if "saliency" in losses:
         sal = t["saliency_scores"]

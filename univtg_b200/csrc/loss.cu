@@ -156,9 +156,10 @@ __global__ void __launch_bounds__(1024) loss_finish_kernel(const LossArgs a) {
       if (valid) {
         const float lp = fmaxf(logf(p), -100.f), l1p = fmaxf(logf(1.f - p), -100.f);
         lf += -(y * lp + (1.f - y) * l1p) * wt;
-        gf = wt * (p - y) / fmaxf(p * (1.f - p), 1e-12f) / n_valid;
+        gf = wt * (p - y) / fmaxf(p * (1.f - p), 1e-12f);
       }
-      a.g_logits_f[i] = gf;
+      // the reference's (bce * mask).sum() / mask.sum(): 0 at masked clips, NaN everywhere (0 / 0) without any valid clip
+      a.g_logits_f[i] = gf / n_valid;
     }
   }
   lb = block_sum(lb, s_red);

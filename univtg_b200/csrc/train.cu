@@ -1240,6 +1240,31 @@ int univtg_droppath_scales(const univtg_rng* rng, int32_t n_sites, int32_t batch
 
 size_t univtg_loss_scratch_bytes(int32_t B, int32_t Lv) { return make_loss_scratch(B, Lv, nullptr).total; }
 
+namespace {
+// What the criterion kernels (loss.cu) assume of their shapes: float4 rows (d % 4 == 0), at least one sample and one clip, and
+// (Lv + 2B) floats of dynamic shared memory for loss_bwd_txt within the default 48 KiB.
+bool loss_shape_ok(const char* fn, int32_t B, int32_t Lv, int32_t d) {
+  if (B < 1 || Lv < 1 || d < 4 || d % 4 != 0 || (int64_t)B * Lv > INT32_MAX / 32) {
+    set_error("%s: bad shape B %d, Lv %d, d %d (d must be a positive multiple of 4)", fn, B, Lv, d);
+    return false;
+  }
+  if ((size_t)(Lv + 2 * B) * sizeof(float) > 48 * 1024 || B > 1536) {  // dynamic shared memory of loss_bwd_txt / loss_bwd_vid
+    set_error("%s: B %d, Lv %d exceed the backward kernels' shared memory", fn, B, Lv);
+    return false;
+  }
+  return true;
+}
+
+// the loss kernels read and write vid_mem_proj / txt_mem_proj rows and their gradients as float4
+bool loss_aligned(const char* fn, const char* name, const void* p) {
+  if (reinterpret_cast<uintptr_t>(p) % 16 != 0) {
+    set_error("%s: %s must be 16-byte aligned", fn, name);
+    return false;
+  }
+  return true;
+}
+}  // namespace
+
 int univtg_loss_forward(const float* pred_logits, const float* pred_spans, const float* vid_mem_proj, const float* txt_mem_proj,
                         const float* timestamp, const float* timestamp_mask, const float* timestamp_window,
                         const float* span_labels_nn, const float* saliency_scores, const int64_t* saliency_pos_idx, int32_t B,
@@ -1249,10 +1274,14 @@ int univtg_loss_forward(const float* pred_logits, const float* pred_spans, const
     set_error("univtg_loss_forward: null argument");
     return 1;
   }
+  const char* fn = "univtg_loss_forward";
   if (B > 256) {
-    set_error("univtg_loss_forward: batch %d > 256 not supported by the single-block reduction", B);
+    set_error("%s: batch %d > 256 not supported by the single-block reduction", fn, B);
     return 1;
   }
+  if (!loss_shape_ok(fn, B, Lv, d) || !loss_aligned(fn, "vid_mem_proj", vid_mem_proj) ||
+      !loss_aligned(fn, "txt_mem_proj", txt_mem_proj))
+    return 1;
   const LossScratch s = make_loss_scratch(B, Lv, reinterpret_cast<uint8_t*>(scratch));
   LossArgs a;
   a.pred_logits = pred_logits;
@@ -1290,6 +1319,15 @@ int univtg_loss_backward(const float* w5, const float* vid_mem_proj, const float
     set_error("univtg_loss_backward: null argument");
     return 1;
   }
+  const char* fn = "univtg_loss_backward";
+  if (B > 256) {
+    set_error("%s: batch %d > 256 not supported by the single-block reduction", fn, B);
+    return 1;
+  }
+  if (!loss_shape_ok(fn, B, Lv, d) || !loss_aligned(fn, "vid_mem_proj", vid_mem_proj) ||
+      !loss_aligned(fn, "txt_mem_proj", txt_mem_proj) || !loss_aligned(fn, "d_vid_mem_proj", d_vid_mem_proj) ||
+      !loss_aligned(fn, "d_txt_mem_proj", d_txt_mem_proj))
+    return 1;
   const LossScratch s = make_loss_scratch(B, Lv, const_cast<uint8_t*>(reinterpret_cast<const uint8_t*>(scratch)));
   LossBwdArgs a;
   a.w = w5;
@@ -1315,20 +1353,6 @@ int univtg_loss_backward(const float* w5, const float* vid_mem_proj, const float
   return launch_loss_backward(a, (cudaStream_t)stream);
 }
 
-namespace {
-bool qfvs_loss_shape_ok(const char* fn, int32_t B, int32_t Lv, int32_t d) {
-  if (B < 1 || Lv < 1 || d < 4 || d % 4 != 0 || (int64_t)B * Lv > INT32_MAX / 32) {
-    set_error("%s: bad shape B %d, Lv %d, d %d (d must be a positive multiple of 4)", fn, B, Lv, d);
-    return false;
-  }
-  if ((size_t)(Lv + 2 * B) * sizeof(float) > 48 * 1024 || B > 1536) {  // dynamic shared memory of loss_bwd_txt / loss_bwd_vid
-    set_error("%s: B %d, Lv %d exceed the backward kernels' shared memory", fn, B, Lv);
-    return false;
-  }
-  return true;
-}
-}  // namespace
-
 int univtg_qfvs_loss_forward(const float* pred_logits, const float* vid_mem_proj, const float* txt_mem_proj, const float* src_vid_mask,
                              const uint8_t* mask_gt, const float* saliency_scores, int32_t has_pos_labels, int32_t B, int32_t Lv,
                              int32_t d, float temperature, float* losses5, void* scratch, void* stream) {
@@ -1336,7 +1360,10 @@ int univtg_qfvs_loss_forward(const float* pred_logits, const float* vid_mem_proj
     set_error("univtg_qfvs_loss_forward: null argument");
     return 1;
   }
-  if (!qfvs_loss_shape_ok("univtg_qfvs_loss_forward", B, Lv, d)) return 1;
+  const char* fn = "univtg_qfvs_loss_forward";
+  if (!loss_shape_ok(fn, B, Lv, d) || !loss_aligned(fn, "vid_mem_proj", vid_mem_proj) ||
+      !loss_aligned(fn, "txt_mem_proj", txt_mem_proj))
+    return 1;
   const LossScratch s = make_loss_scratch(B, Lv, reinterpret_cast<uint8_t*>(scratch));
   QfvsLossArgs a;
   a.pred_logits = pred_logits;
@@ -1367,7 +1394,11 @@ int univtg_qfvs_loss_backward(const float* w5, const float* vid_mem_proj, const 
     set_error("univtg_qfvs_loss_backward: null argument");
     return 1;
   }
-  if (!qfvs_loss_shape_ok("univtg_qfvs_loss_backward", B, Lv, d)) return 1;
+  const char* fn = "univtg_qfvs_loss_backward";
+  if (!loss_shape_ok(fn, B, Lv, d) || !loss_aligned(fn, "vid_mem_proj", vid_mem_proj) ||
+      !loss_aligned(fn, "txt_mem_proj", txt_mem_proj) || !loss_aligned(fn, "d_vid_mem_proj", d_vid_mem_proj) ||
+      !loss_aligned(fn, "d_txt_mem_proj", d_txt_mem_proj))
+    return 1;
   const LossScratch s = make_loss_scratch(B, Lv, reinterpret_cast<uint8_t*>(scratch));
   LossBwdArgs a;
   a.w = w5;
