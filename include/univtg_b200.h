@@ -600,6 +600,32 @@ int univtg_op_attention_bwd(const void* qkv, const void* dO, const void* O, cons
                             float* delta_ws, float* dqkv32, int32_t B, int32_t L, int32_t H, int32_t dh, int32_t fmt_act,
                             int32_t impl, void* stream);
 
+/* delta [B, H, L] f32 = rowsum over each head's dh channels of dO o O (dO, O 16-bit [B*L, H*dh], formats fmt_do / fmt_o 0/1).
+ * vec_used (optional): 1 when the 128-bit vector path ran (dh a power-of-two multiple of 8 up to 256, 16-byte aligned dO and O),
+ * 0 for the scalar path. */
+int univtg_op_attn_delta(const void* dO, int32_t fmt_do, const void* O, int32_t fmt_o, float* delta, int32_t B, int32_t L, int32_t H,
+                         int32_t dh, int32_t* vec_used, void* stream);
+
+/* Attention core backward with every option of the kernels, routed as univtg_backward routes it.  qkv [B*L, 3d] and dO [B*L, d]
+ * 16-bit (fmt 0/1, 16-byte aligned); key_mask [B, L]; lse and delta [B, H, L] f32 (delta = univtg_op_attn_delta); dqkv32 [B*L, 3d]
+ * f32; dqkv16 (optional, impl 0 and L <= 128) [B*L, 3d] 16-bit.  impl 0 tensor cores (dh 64 / 128), 1 SIMT (any dh, L up to the
+ * device's opt-in shared memory / 32 bytes).  p > 0: the attention dropout of encoder layer `layer` of rng, as the forward drew it.
+ * kernel_used (optional): 4 (dh 128) + 2 (bf16) + dropout = 0..7 tensor cores, 8 + dropout SIMT.  dq_mode (optional): 0 dQ | dK | dV
+ * written to dqkv16 (dqkv32 untouched), 1 written to dqkv32 with dQ stored (one key tile), 2 dqkv32 zeroed and dQ accumulated
+ * atomically (several key tiles, or SIMT). */
+typedef struct univtg_attn_bwd {
+  const void* qkv;
+  const void* dO;
+  const float* key_mask;
+  const float* lse;
+  const float* delta;
+  float* dqkv32;
+  void* dqkv16;
+  int32_t B, L, H, dh, fmt, impl;
+} univtg_attn_bwd;
+int univtg_op_attention_bwd_full(const univtg_attn_bwd* args, const univtg_rng* rng, float p, int32_t layer, int32_t* kernel_used,
+                                 int32_t* dq_mode, void* stream);
+
 /* ---- CLIP feature extraction (inference only): the ViT image tower and the text tower of OpenAI CLIP
  * (reference run_on_video/clip/model.py: VisualTransformer 202-236, encode_text 339-352), which produce the video and query
  * features the grounding model consumes.  Every head is 64 wide (heads = width / 64, model.py:268); LayerNorm eps 1e-5. ---- */

@@ -14,6 +14,7 @@ import math
 import pytest
 import torch
 
+from tests.attn_bwd_ref import attn_reference, key_mask_gap, val16
 from tests.bounds import U, all_nan, cfac, check, report_fixture, ulp16
 from tests.test_backward_ops_gpu import DT, P, conv_buf, epilogue, gen, lib, nan, problem, randn, rnd16, run_group, check_rows
 from univtg_b200 import _lib
@@ -29,11 +30,6 @@ def hilo(x32):
     """fp16x3 pair of fp32 values: hi = fp16(x), lo = fp16(x - hi)."""
     hi = x32.half()
     return hi, (x32 - hi.float()).half()
-
-
-def val16(hi, lo=None):
-    """fp64 value of a 16-bit operand (hi + lo for an fp16x3 pair)."""
-    return hi.double() if lo is None else hi.double() + lo.double()
 
 
 def check16(fam, name, hi, lo, ref, S, K, fmt):
@@ -546,52 +542,6 @@ def test_gemm_conv_forward_heads(fmt, Lv):
 
 
 # ================================================= attention forward =================================================
-def key_mask_gap(B, L, g):
-    """The product's key mask cat(vid_mask, txt_mask): valid clips, padded clips, valid text, padded text (per sample)."""
-    km = torch.ones((B, L))
-    if L < 8:
-        return km
-    for b in range(B):
-        lv = L * 2 // 3
-        nv = max(1, lv - 5 * b - 3)
-        km[b, nv:lv] = 0
-        nt = max(1, (L - lv) - 2 * b)
-        km[b, lv + nt:] = 0
-    return km
-
-
-def attn_reference(qkv, lo, km, B, L, H, dh, fmt, causal=False, mul=None):
-    """fp64 attention from the exact operands, with the bounds of the output and of lse."""
-    d = H * dh
-    Qkv = val16(qkv, lo).view(B, L, 3, H, dh)
-    q, k, v = (Qkv[:, :, i].permute(0, 2, 1, 3) for i in range(3))  # [B, H, L, dh]
-    scale = float(torch.tensor(1.0 / math.sqrt(dh), dtype=torch.float32))
-    s = torch.einsum("bhid,bhjd->bhij", q, k) * scale
-    Ss = torch.einsum("bhid,bhjd->bhij", q.abs(), k.abs()) * scale
-    valid = (km.cuda() != 0)[:, None, None, :].expand(B, H, L, L)
-    if causal:
-        valid = valid & torch.ones((L, L), dtype=torch.bool, device="cuda").tril()
-    s = torch.where(valid, s, float("-inf"))
-    m = s.max(-1, keepdim=True).values
-    p = torch.exp(s - m)
-    l = p.sum(-1, keepdim=True)
-    lse = (m + torch.log(l))[..., 0]
-    pm = p * mul if mul is not None else p
-    o = torch.einsum("bhij,bhjd->bhid", pm, v) / l
-    split = fmt == 2
-    u16 = 2.0 ** -21 if split else (2.0 ** -11 if fmt == 0 else 2.0 ** -8)
-    floor = 0.0 if fmt == 1 else 2.0 ** -25
-    # score error: fp32 products over dh (+ the lo x lo term fp16x3 drops) and the rounded exponent scale
-    es = torch.where(valid, cfac(dh) * U * Ss + 4 * U * s.abs().nan_to_num(0.0, 0.0, 0.0) + (2.0 ** -22 * Ss if split else 0.0), 0.0)
-    c = cfac(L)
-    pa = pm.abs()
-    num = torch.einsum("bhij,bhjd->bhid", (c * U + u16) * pa + 2 * pa * es + floor * valid, v.abs())
-    den = ((2 * p * es).sum(-1, keepdim=True) + c * U * l)
-    bo = (num + o.abs() * den) / l
-    Slse = es.max(-1).values / (cfac(L * dh) * U) + lse.abs() + 1.0
-    return o.permute(0, 2, 1, 3).reshape(B * L, d), bo.permute(0, 2, 1, 3).reshape(B * L, d), lse, Slse
-
-
 def run_attention(B, L, H, dh, fmt, impl, causal=0, km=None, p=0.0, seed=0):
     d = H * dh
     g = gen(seed)

@@ -111,6 +111,13 @@ class AttnFwd(ctypes.Structure):
         [(n, c_int) for n in ("B", "L", "H", "dh", "fmt", "impl", "causal")]
 
 
+class AttnBwd(ctypes.Structure):
+    """univtg_attn_bwd."""
+
+    _fields_ = [(n, c_void_p) for n in ("qkv", "dO", "key_mask", "lse", "delta", "dqkv32", "dqkv16")] + \
+        [(n, c_int) for n in ("B", "L", "H", "dh", "fmt", "impl")]
+
+
 class ClipConfig(ctypes.Structure):
     """univtg_clip_config."""
 
@@ -193,6 +200,9 @@ SIGNATURES = {
     "univtg_op_attention": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int,
                                     c_void_p]),
     "univtg_op_attention_bwd": (c_int, [c_void_p] * 7 + [c_int, c_int, c_int, c_int, c_int, c_int, c_void_p]),
+    "univtg_op_attn_delta": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
+    "univtg_op_attention_bwd_full": (c_int, [ctypes.POINTER(AttnBwd), ctypes.POINTER(Rng), c_float, c_int, c_void_p, c_void_p,
+                                             c_void_p]),
     "univtg_op_layernorm_fwd": (c_int, [ctypes.POINTER(LnFwd), ctypes.POINTER(Rng), c_int, c_void_p, c_void_p]),
     "univtg_op_txt_pos": (c_int, [ctypes.POINTER(TxtPosFwd), ctypes.POINTER(Rng), c_int, c_void_p]),
     "univtg_op_sine_pos": (c_int, [c_void_p] * 5 + [c_int, c_int, c_int, c_int, ctypes.POINTER(Rng), c_int, c_void_p, c_void_p]),

@@ -281,18 +281,20 @@ static int launch_bwd_tc(const AttnBwdArgs& a, cudaStream_t stream) {
 }
 
 template <int DH, int BF>
-static int launch_bwd_tc_drop(const AttnBwdArgs& a, cudaStream_t stream) {
+static int launch_bwd_tc_drop(const AttnBwdArgs& a, cudaStream_t stream, int* kernel_used) {
+  if (kernel_used) *kernel_used = (DH == 128 ? 4 : 0) + 2 * BF + (a.drop.on ? 1 : 0);
   return a.drop.on ? launch_bwd_tc<DH, BF, 1>(a, stream) : launch_bwd_tc<DH, BF, 0>(a, stream);
 }
 
-int launch_attention_bwd(const AttnBwdArgs& a, cudaStream_t stream) {
+int launch_attention_bwd(const AttnBwdArgs& a, cudaStream_t stream, int* kernel_used) {
+  if (kernel_used) *kernel_used = -1;
   if (a.fmt_act != a.fmt_grad) {
     set_error("launch_attention_bwd: activations and gradients must share one 16-bit format (got %d and %d)", a.fmt_act, a.fmt_grad);
     return (int)cudaErrorInvalidValue;
   }
   const bool bf = a.fmt_act != 0;
-  if (a.dh == 128) return bf ? launch_bwd_tc_drop<128, 1>(a, stream) : launch_bwd_tc_drop<128, 0>(a, stream);
-  if (a.dh == 64) return bf ? launch_bwd_tc_drop<64, 1>(a, stream) : launch_bwd_tc_drop<64, 0>(a, stream);
+  if (a.dh == 128) return bf ? launch_bwd_tc_drop<128, 1>(a, stream, kernel_used) : launch_bwd_tc_drop<128, 0>(a, stream, kernel_used);
+  if (a.dh == 64) return bf ? launch_bwd_tc_drop<64, 1>(a, stream, kernel_used) : launch_bwd_tc_drop<64, 0>(a, stream, kernel_used);
   set_error("launch_attention_bwd: tensor-core path needs dh in {64,128}, got %d", a.dh);
   return (int)cudaErrorInvalidValue;
 }

@@ -559,12 +559,13 @@ __global__ void __launch_bounds__(256) attn_delta_kernel(const uint16_t* __restr
 }
 
 int launch_attn_delta(const uint16_t* dO, int fmt_do, const uint16_t* O, int fmt_o, float* delta, int B, int L, int H, int dh,
-                      cudaStream_t stream) {
+                      cudaStream_t stream, int* vec_used) {
   const int rows = B * L;
   const int d = H * dh;
   // vector path: 8 channels per lane, 2^k lanes per head, every 256-channel step of a warp covers whole heads
   const int vec = (dh % 8 == 0) && ((dh / 8) & (dh / 8 - 1)) == 0 && dh <= 256 && (d % 8 == 0) && (256 % dh == 0 || dh == 256) &&
                   ((reinterpret_cast<uintptr_t>(dO) | reinterpret_cast<uintptr_t>(O)) & 15) == 0;
+  if (vec_used) *vec_used = vec;
   launch_k(attn_delta_kernel, dim3((rows * 32 + 255) / 256), dim3(256), 0, stream, dO, fmt_do, O, fmt_o, delta, B, L, H, dh, vec ? 1 : 0);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) set_error("attn_delta launch failed: %s", cudaGetErrorString(e));
@@ -631,10 +632,11 @@ __global__ void __launch_bounds__(128) attention_bwd_simt_kernel(const AttnBwdAr
   }
 }
 
-int launch_attention_bwd_simt(const AttnBwdArgs& a, cudaStream_t stream) {
+int launch_attention_bwd_simt(const AttnBwdArgs& a, cudaStream_t stream, int* kernel_used) {
   const int warps = a.B * a.H * a.L;
-  const size_t smem = (size_t)4 * 2 * a.L * sizeof(float);
+  const size_t smem = attention_bwd_simt_smem(a.L);
   auto kern = a.drop.on ? attention_bwd_simt_kernel<1> : attention_bwd_simt_kernel<0>;
+  if (kernel_used) *kernel_used = 8 + (a.drop.on ? 1 : 0);
   if (smem > 48 * 1024) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) {

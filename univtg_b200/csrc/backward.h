@@ -57,9 +57,9 @@ int launch_tap_interleave(const float* src, float* dst, int N, int C, cudaStream
 int launch_colsum16(const uint16_t* in16, int ld, int rows, int cols, int fmt, float* colsum, float scale, cudaStream_t stream,
                     TxtRows txt = TxtRows{nullptr, 0, 0, 0});
 
-// delta[b, h, i] = sum_c dO[b, i, h, c] * O[b, i, h, c]
+// delta[b, h, i] = sum_c dO[b, i, h, c] * O[b, i, h, c].  vec_used (optional): 1 when the 128-bit vector path ran, 0 scalar.
 int launch_attn_delta(const uint16_t* dO, int fmt_do, const uint16_t* O, int fmt_o, float* delta, int B, int L, int H, int dh,
-                      cudaStream_t stream);
+                      cudaStream_t stream, int* vec_used = nullptr);
 
 struct AttnBwdArgs {
   CUtensorMap tm_qkv;  // [B*L, 3d] 16-bit activations (Q | K | V), box {64, 128}
@@ -79,8 +79,12 @@ struct AttnBwdArgs {
   uint16_t* dqkv16;       // [B*L, 3d] or null
   DropSpec drop;          // the forward's attention dropout (drop.on): dV += (P o M)^T dO, dS = P o (M o dP - delta)
 };
-int launch_attention_bwd(const AttnBwdArgs& a, cudaStream_t stream);       // wgmma, dh in {64, 128}
-int launch_attention_bwd_simt(const AttnBwdArgs& a, cudaStream_t stream);  // any dh; needs dqkv32 pre-zeroed
+// kernel_used (optional): which instantiation ran, the numbering univtg_op_attention_bwd_full reports:
+// wgmma 4 (dh 128) + 2 (bf16) + dropout = 0..7, SIMT 8 + dropout.
+int launch_attention_bwd(const AttnBwdArgs& a, cudaStream_t stream, int* kernel_used = nullptr);       // wgmma, dh in {64, 128}
+int launch_attention_bwd_simt(const AttnBwdArgs& a, cudaStream_t stream, int* kernel_used = nullptr);  // any dh; dqkv32 pre-zeroed
+// Dynamic shared memory of the SIMT kernel: p and dS of L keys for each of its 4 warps.
+inline size_t attention_bwd_simt_smem(int L) { return (size_t)4 * 2 * L * sizeof(float); }
 
 // ---- conv heads: last layer (1 / 2 output channels) ----
 struct HeadFinalBwdArgs {

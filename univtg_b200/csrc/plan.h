@@ -386,6 +386,40 @@ inline int gemm_launch(univtg_plan* P, GemmGroup& g, int bn, int sms, cudaStream
   prof_mark(P, st, 1);
   return rc;
 }
+
+// Longest sequence the SIMT attention backward can stage (attention_bwd_simt_smem = 32 L bytes) in the device's opt-in shared
+// memory per block.  Without a device to ask, the sm_90 value (227 KB, the only target the library is built for) is used.
+inline int attention_bwd_simt_max_L() {
+  int dev = 0, optin = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev) != cudaSuccess ||
+      optin <= 0) {
+    cudaGetLastError();
+    optin = 227 * 1024;
+  }
+  return (int)((size_t)optin / attention_bwd_simt_smem(1));
+}
+
+// Routing of the attention core backward, shared by univtg_backward and the single-operator entry points.  `a` holds everything but
+// dq_atomic, dqkv16 and the tensor maps.  tc: wgmma kernel (dh 64 / 128), else the SIMT kernel.  dQ | dK | dV go
+//   dq_mode 0: straight to the 16-bit operand dqkv16 (tc, one key tile L <= 128, dqkv16 given); dqkv32 is not written,
+//   dq_mode 1: to dqkv32, dQ stored (tc, one key tile, no dqkv16),
+//   dq_mode 2: to dqkv32 after a memset, dQ accumulated atomically (several key tiles, or SIMT).
+// P (optional): the plan whose profiling marks bracket the wgmma launch.
+inline int attention_bwd_route(AttnBwdArgs& a, bool tc, uint16_t* dqkv16, cudaStream_t st, int* dq_mode, int* kernel_used = nullptr,
+                               univtg_plan* P = nullptr) {
+  const int M = a.B * a.L, d = a.d;
+  a.dq_atomic = (!tc || a.L > 128) ? 1 : 0;
+  a.dqkv16 = a.dq_atomic ? nullptr : dqkv16;
+  if (dq_mode) *dq_mode = a.dq_atomic ? 2 : (a.dqkv16 ? 0 : 1);
+  if (a.dq_atomic) cudaMemsetAsync(a.dqkv32, 0, (size_t)M * 3 * d * 4, st);
+  if (!tc) return launch_attention_bwd_simt(a, st, kernel_used);
+  if (make_tmap_2d(&a.tm_qkv, a.qkv, (uint64_t)M, (uint64_t)3 * d, (uint64_t)3 * d, 128, 64)) return 1;
+  if (make_tmap_2d(&a.tm_do, a.dO, (uint64_t)M, (uint64_t)d, (uint64_t)d, 128, 64)) return 1;
+  if (P) prof_mark(P, st, 3);
+  const int rc = launch_attention_bwd(a, st, kernel_used);
+  if (P) prof_mark(P, st, 2);
+  return rc;
+}
 }  // namespace
 
 namespace {

@@ -151,6 +151,16 @@ int univtg_prepare_workspace(const univtg_config* cfg, const univtg_shape* shape
 
 size_t univtg_train_workspace_bytes(const univtg_config* cfg, const univtg_shape* shape) {
   if (!check_cfg(cfg) || !check_shape(shape) || refuse_split(*cfg, "univtg_train_workspace_bytes")) return 0;
+  const int dh = cfg->hidden_dim / cfg->nheads, L = shape->l_vid + shape->l_txt;
+  if (dh != 64 && dh != 128) {  // the SIMT attention backward holds a whole row of L scores per warp in shared memory
+    const int max_L = attention_bwd_simt_max_L();
+    if (L > max_L) {
+      set_error("univtg_train_workspace_bytes: L = l_vid + l_txt = %d exceeds %d, the longest sequence the SIMT attention backward "
+                "(head size %d, not 64 or 128) can stage in shared memory",
+                L, max_L, dh);
+      return 0;
+    }
+  }
   return make_train_ws(*cfg, *shape, make_layout(*cfg), nullptr).total;
 }
 
@@ -575,22 +585,11 @@ int univtg_backward(univtg_plan* P, void* ws, const float* src_txt, const float*
       a.fmt_act = fmt;
       a.fmt_grad = FMT_G;
       if (P->attn_dropout > 0.f) a.drop = make_drop_spec(rng->seed, (unsigned int)l, P->attn_dropout);  // the forward's masks
-      const bool tc = (P->dh == 64 || P->dh == 128);
-      const int num_kv = (L + 127) / 128;
-      a.dq_atomic = (!tc || num_kv > 1) ? 1 : 0;
-      fused16 = !a.dq_atomic;  // one key tile: the kernel emits the 16-bit operands and the in_proj_bias gradient itself
-      if (fused16) a.dqkv16 = T.dqkv16;  // (the in_proj_bias column sums are a separate pass)
-      if (a.dq_atomic) cudaMemsetAsync(T.dqkv32, 0, (size_t)M * 3 * d * 4, st);
-      if (tc) {
-        if (make_tmap_2d(&a.tm_qkv, T.qkv16[l], (uint64_t)M, (uint64_t)3 * d, (uint64_t)3 * d, 128, 64)) return 1;
-        if (make_tmap_2d(&a.tm_do, T.dO16, (uint64_t)M, (uint64_t)d, (uint64_t)d, 128, 64)) return 1;
-        prof_mark(P, st, 3);
-        rc = launch_attention_bwd(a, st);
-        prof_mark(P, st, 2);
-      } else {
-        rc = launch_attention_bwd_simt(a, st);
-      }
+      // one key tile on tensor cores: the kernel emits the 16-bit operands itself (the in_proj_bias column sums are a separate pass)
+      int dq_mode = 2;
+      rc = attention_bwd_route(a, P->dh == 64 || P->dh == 128, T.dqkv16, st, &dq_mode, nullptr, P);
       if (rc) return rc;
+      fused16 = dq_mode == 0;
     }
     // (with text positions the same pass also copies the text rows of [dq | dk] into TP.dqk16)
     if (!fused16) rc = launch_cvt16_colsum(T.dqkv32, 3 * d, T.dqkv16, 3 * d, M, 3 * d, FMT_G, G_layer(l, 1), INV, st, txt_rows);
@@ -866,7 +865,7 @@ int univtg_op_attention_bwd(const void* qkv, const void* dO, const void* O, cons
   }
   if (refuse_fmt2(fmt_act, "univtg_op_attention_bwd")) return 1;
   cudaStream_t st = (cudaStream_t)stream;
-  const int d = H * dh, M = B * L;
+  const int d = H * dh;
   int rc = launch_attn_delta(reinterpret_cast<const uint16_t*>(dO), fmt_act, reinterpret_cast<const uint16_t*>(O), fmt_act,
                              delta_ws, B, L, H, dh, st);
   if (rc) return rc;
@@ -886,13 +885,61 @@ int univtg_op_attention_bwd(const void* qkv, const void* dO, const void* O, cons
   a.d = d;
   a.fmt_act = fmt_act;
   a.fmt_grad = fmt_act;
-  const bool tc = impl == 0;
-  a.dq_atomic = (!tc || (L + 127) / 128 > 1) ? 1 : 0;
-  if (a.dq_atomic) cudaMemsetAsync(dqkv32, 0, (size_t)M * 3 * d * 4, st);
-  if (!tc) return launch_attention_bwd_simt(a, st);
-  if (make_tmap_2d(&a.tm_qkv, qkv, (uint64_t)M, (uint64_t)3 * d, (uint64_t)3 * d, 128, 64)) return 1;
-  if (make_tmap_2d(&a.tm_do, dO, (uint64_t)M, (uint64_t)d, (uint64_t)d, 128, 64)) return 1;
-  return launch_attention_bwd(a, st);
+  return attention_bwd_route(a, impl == 0, nullptr, st, nullptr);
+}
+
+int univtg_op_attn_delta(const void* dO, int32_t fmt_do, const void* O, int32_t fmt_o, float* delta, int32_t B, int32_t L, int32_t H,
+                         int32_t dh, int32_t* vec_used, void* stream) {
+  const char* fn = "univtg_op_attn_delta";
+  UV_REQ(dO && O && delta, "%s: null dO, O or delta", fn);
+  UV_REQ((fmt_do == 0 || fmt_do == 1) && (fmt_o == 0 || fmt_o == 1), "%s: fmt_do %d / fmt_o %d (0 fp16, 1 bf16)", fn, fmt_do, fmt_o);
+  UV_REQ(B >= 1 && L >= 1 && H >= 1 && dh >= 1, "%s: B %d / L %d / H %d / dh %d must be positive", fn, B, L, H, dh);
+  int vec = -1;
+  const int rc = launch_attn_delta(reinterpret_cast<const uint16_t*>(dO), fmt_do, reinterpret_cast<const uint16_t*>(O), fmt_o, delta, B,
+                                   L, H, dh, (cudaStream_t)stream, &vec);
+  if (vec_used) *vec_used = vec;
+  return rc;
+}
+
+int univtg_op_attention_bwd_full(const univtg_attn_bwd* q, const univtg_rng* rng, float p, int32_t layer, int32_t* kernel_used,
+                                 int32_t* dq_mode, void* stream) {
+  const char* fn = "univtg_op_attention_bwd_full";
+  UV_REQ(q != nullptr, "%s: null args", fn);
+  UV_REQ(q->qkv && q->dO && q->key_mask && q->lse && q->delta && q->dqkv32, "%s: null qkv, dO, key_mask, lse, delta or dqkv32", fn);
+  UV_REQ(q->B >= 1 && q->L >= 1 && q->H >= 1 && q->dh >= 1, "%s: B %d / L %d / H %d / dh %d must be positive", fn, q->B, q->L, q->H,
+         q->dh);
+  UV_REQ(q->fmt == 0 || q->fmt == 1, "%s: fmt %d (0 fp16, 1 bf16)", fn, q->fmt);
+  UV_REQ(q->impl == 0 || q->impl == 1, "%s: impl %d (0 tensor cores, 1 SIMT)", fn, q->impl);
+  UV_REQ(q->impl == 1 || q->dh == 64 || q->dh == 128, "%s: tensor-core attention backward needs dh 64 or 128, got %d", fn, q->dh);
+  UV_REQ(!q->dqkv16 || (q->impl == 0 && q->L <= 128), "%s: dqkv16 needs impl 0 and a single key tile (L %d <= 128)", fn, q->L);
+  UV_REQ(al_(q->qkv, 16) && al_(q->dO, 16), "%s: qkv and dO must be 16-byte aligned", fn);
+  UV_REQ(al_(q->key_mask, 4) && al_(q->lse, 4) && al_(q->delta, 4) && al_(q->dqkv32, 8) && al_(q->dqkv16, 4),
+         "%s: key_mask / lse / delta must be 4-byte, dqkv32 8-byte and dqkv16 4-byte aligned", fn);
+  UV_REQ(p >= 0.f && p < 1.f && (!(p > 0.f) || (rng && layer >= 0)), "%s: p %g must be in [0, 1) and p > 0 needs rng and layer >= 0",
+         fn, (double)p);
+  if (q->impl == 1) {
+    const int max_L = attention_bwd_simt_max_L();
+    UV_REQ(q->L <= max_L, "%s: SIMT backward stages 32 L bytes of shared memory: L %d exceeds %d", fn, q->L, max_L);
+  }
+  AttnBwdArgs a;
+  memset(&a, 0, sizeof(a));
+  const int d = q->H * q->dh;
+  a.qkv = reinterpret_cast<const uint16_t*>(q->qkv);
+  a.dO = reinterpret_cast<const uint16_t*>(q->dO);
+  a.key_mask = q->key_mask;
+  a.lse = q->lse;
+  a.delta = q->delta;
+  a.dqkv32 = q->dqkv32;
+  a.scale = 1.0f / sqrtf((float)q->dh);
+  a.B = q->B;
+  a.L = q->L;
+  a.H = q->H;
+  a.dh = q->dh;
+  a.d = d;
+  a.fmt_act = a.fmt_grad = q->fmt;
+  if (p > 0.f) a.drop = make_drop_spec(rng->seed, (unsigned int)layer, p);
+  if (kernel_used) *kernel_used = -1;
+  return attention_bwd_route(a, q->impl == 0, reinterpret_cast<uint16_t*>(q->dqkv16), (cudaStream_t)stream, dq_mode, kernel_used);
 }
 
 // ---- single backward operators: thin wrappers over the launchers univtg_backward uses.  Each checks on the host what its kernel
