@@ -678,6 +678,28 @@ int univtg_clip_encode_text(const univtg_clip_config* cfg, const void* packed, c
  * bit 1 = pooled. */
 int univtg_clip_num_launches(const univtg_clip_config* cfg, int32_t tower, int32_t text_outputs);
 
+/* ---- CLIP-teacher pseudo labels (reference teacher/clip2label.py): per video the top-k classes by the sum over clips of the
+ * clip-class cosines (ties to the lower class index), and per chosen class the curve float32(cos) // th with the runs of its
+ * maximum that end before the last clip.  Cosines use a / max(||a||, 1e-8) and are computed in fp64 from the f32 features.
+ * cls: [C, D] f32 class features, D <= 1024. ---- */
+size_t univtg_teacher_class_bytes(int32_t C, int32_t D);
+/* Normalised class table (fp16x3 planes and fp64 norms) into cls_ws (univtg_teacher_class_bytes); kept for every later call. */
+int univtg_teacher_prepare_classes(const float* cls, int32_t C, int32_t D, void* cls_ws, void* stream);
+/* Workspace for one univtg_teacher_label call of V videos with S clips in total (includes a [V, C rounded up to 16] f32 matrix). */
+size_t univtg_teacher_chunk_bytes(int32_t V, int64_t S, int32_t C, int32_t D);
+/* feats [S, D] f32 (videos concatenated), offsets [V + 1] int32 on the device, every video 1..65535 clips (checked by the
+ * caller); topk in 1..16, finite th >= 2^-30 (so that |bins| <= 1 / th + 1 fit in int32).
+ * out: int32 [2 V topk + 2 S topk + 1], zeroed and then written as
+ *   idx  [V, topk]  chosen class per rank (-1 when C < topk),
+ *   nwin [V, topk]  windows per rank (0: no window, the line is skipped),
+ *   win  [S, topk]  rows off_v .. off_v + nwin - 1: (first clip << 16) | last clip of each window (uint32),
+ *   bins [S, topk]  float32(cos) // th of every clip (INT32_MIN stands for -0.0),
+ *   and the number of videos that were rescored over every class because the approximate ranking could not be certified. */
+int univtg_teacher_label(const float* cls, const void* cls_ws, int32_t C, int32_t D, const float* feats, const int32_t* offsets,
+                         int32_t V, int64_t S, int32_t topk, double th, void* ws, size_t ws_bytes, int32_t* out, void* stream);
+/* Host only: out[i] = x[i] // th with Python's float floor division, the function the curves use on the device. */
+int univtg_debug_py_floordiv(const double* x, int64_t n, double th, double* out);
+
 #ifdef __cplusplus
 }
 #endif

@@ -218,6 +218,12 @@ SIGNATURES = {
     "univtg_clip_encode_text": (c_int, [ctypes.POINTER(ClipConfig), c_void_p, c_void_p, c_int, c_int, c_void_p, c_size_t, c_void_p,
                                         c_void_p, c_void_p]),
     "univtg_clip_num_launches": (c_int, [ctypes.POINTER(ClipConfig), c_int, c_int]),
+    "univtg_teacher_class_bytes": (c_size_t, [c_int, c_int]),
+    "univtg_teacher_prepare_classes": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p]),
+    "univtg_teacher_chunk_bytes": (c_size_t, [c_int, ctypes.c_int64, c_int, c_int]),
+    "univtg_teacher_label": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, ctypes.c_int64, c_int,
+                                     ctypes.c_double, c_void_p, c_size_t, c_void_p, c_void_p]),
+    "univtg_debug_py_floordiv": (c_int, [c_void_p, ctypes.c_int64, ctypes.c_double, c_void_p]),
 }
 
 

@@ -599,3 +599,129 @@ def make_qfvs_permutation_case(seed, n, extra=0, n_tags=48):
     gt = list(range(n + extra))
     rng.shuffle(gt)
     return {"tags": tags, "machine": list(range(n)), "gt": gt, "optimum": float(n)}
+
+
+# ---- CLIP-teacher pseudo labels (teacher/clip2label.py) ------------------------------------------------------------------
+TEACHER_SPECIAL_NAMES = ("Sprenger's tulip", "Crème brûlée", 'A "quoted" name', "Back\\slash")
+
+
+def _teacher_unsafe(feat, cls64, dup_rows, topk, th):
+    """True when the CPU reference could disagree with the float64 labels on this video: a top-(k+1) class is a duplicated row
+    (CPU torch.sort is not stable), two distinct top-(k+1) sums lie within 1e-5 T, or a top-(k+1) cosine (other than an exact
+    0) lies within 1e-6 of a bin edge."""
+    import numpy as np
+
+    v = feat.astype(np.float64)
+    v = v / np.maximum(np.linalg.norm(v, axis=1, keepdims=True), 1e-8)
+    mm = v @ cls64.T
+    s = mm.sum(0)
+    top = np.argsort(-s, kind="stable")[:topk + 1]
+    if dup_rows.intersection(top.tolist()):
+        return True
+    st = np.sort(s[top])
+    if (np.diff(st) < 1e-5 * len(feat)).any():
+        return True
+    x = mm[:, top]
+    edge = np.abs(x - np.round(x / th) * th)
+    return bool(((edge < 1e-6) & (x != 0)).any())
+
+
+def make_teacher_case(seed, n_classes=300, dim=64, n_videos=12, clips=(2, 60), lengths=(), dup=0, dup_top=False, copies=0,
+                      edges=True, parallel=True, safe=False, topk=5, th=0.05):
+    """Seeded inputs of the CLIP-teacher labelling: a class table, class names and videos whose clips mix a few class
+    directions (Gaussian bumps over time) with noise, so the curves have peaks and windows.
+
+    n_videos random videos with T drawn from `clips`, then one per entry of `lengths`; with `edges` also T = 1 (always
+    skipped), a ramp whose maximum is only at the last clip, identical clips (all-equal curves), a video with zero rows, and
+    (`parallel`) one whose clips are exact multiples of a class row (cosine 1, bin 19 at th 0.05).  `dup` class rows copy
+    others (the OIDv6 list has 12 duplicated names); with `dup_top` the first video is about a duplicated row, so the copy
+    and the original tie inside its top-k.  `copies` more rows copy the first video's main class.  With `safe`, videos are
+    redrawn until the CPU reference cannot disagree (_teacher_unsafe), duplicated rows stay out of every top-(k+1), and
+    parallel / dup_top / copies are refused.  Returns {"classes", "names", "features", "vids", "dup_rows"}."""
+    import numpy as np
+
+    if safe and (parallel and edges or dup_top or copies):
+        raise ValueError("make_teacher_case: safe cases cannot have parallel clips, dup_top or copies")
+    rng = np.random.default_rng(seed)
+    C, D = n_classes, dim
+    cls = (rng.standard_normal((C, D)) * rng.uniform(0.5, 2.0, (C, 1))).astype(np.float32)
+    names = [f"class {i}" for i in range(C)]
+    for i, n in enumerate(TEACHER_SPECIAL_NAMES[:C]):
+        names[i] = n
+    dup_rows = set()
+    src_dup = None
+    if dup:
+        rows = rng.choice(C, 2 * dup, replace=False)
+        for s, d in zip(rows[:dup], rows[dup:]):
+            cls[d] = cls[s]
+            names[d] = names[s]
+            dup_rows.update((int(s), int(d)))
+        src_dup = int(rows[0])
+    main = None
+    if copies:
+        main = int(rng.integers(C))
+        others = rng.choice(np.setdiff1d(np.arange(C), [main]), copies, replace=False)
+        cls[others] = cls[main]
+        for o in others:
+            names[int(o)] = names[main]
+    cls64 = cls.astype(np.float64)
+    cls64 /= np.maximum(np.linalg.norm(cls64, axis=1, keepdims=True), 1e-8)
+    unit = cls64.astype(np.float32)
+    allowed = np.setdiff1d(np.arange(C), sorted(dup_rows)) if safe else np.arange(C)
+
+    def mix(T, topics=None, noise=None):
+        k = len(topics) if topics is not None else min(int(rng.integers(1, 4)), len(allowed))
+        if topics is None:
+            topics = rng.choice(allowed, k, replace=False)
+        t = np.arange(T)[:, None]
+        mu, sd = rng.uniform(0, T, k), rng.uniform(1.0, max(2.0, T / 3), k)
+        w = rng.uniform(0.5, 2.0, k) * np.exp(-(t - mu) ** 2 / (2 * sd ** 2)) + rng.uniform(0.0, 0.5, k)
+        sig = rng.uniform(0.3, 1.0) if noise is None else noise
+        x = w @ unit[topics] + sig * rng.standard_normal((T, D)) / math.sqrt(D)
+        return (x * rng.uniform(5.0, 15.0)).astype(np.float32)
+
+    specs = [("rand", int(rng.integers(clips[0], clips[1] + 1))) for _ in range(n_videos)] + [("rand", int(T)) for T in lengths]
+    if edges:
+        specs += [("one", 1), ("ramp", 12), ("equal", 8), ("zero", 20)] + ([("parallel", 10)] if parallel else [])
+    feats, vids = [], []
+    for i, (kind, T) in enumerate(specs):
+        for _ in range(200):
+            if kind == "one":
+                f = mix(1)
+            elif kind == "ramp":
+                c = rng.choice(allowed)
+                f = ((np.arange(T)[:, None] + 1.0) * unit[c] + 0.3 * rng.standard_normal((T, D)) / math.sqrt(D)).astype(np.float32)
+            elif kind == "equal":
+                f = np.repeat(mix(1), T, axis=0)
+            elif kind == "zero":
+                f = mix(T)
+                f[[3, 7, 8]] = 0.0
+            elif kind == "parallel":
+                c = int(rng.choice(allowed))
+                f = mix(T, topics=np.array([c]))
+                f[2:5] = cls[c] * 2.0
+            elif i == 0 and dup_top:
+                f = mix(T, topics=np.array([src_dup]), noise=0.3)
+            elif i == 0 and copies:
+                f = mix(T, topics=np.array([main]), noise=0.3)
+            else:
+                f = mix(T)
+            if not safe or not _teacher_unsafe(f, cls64, dup_rows, topk, th):
+                break
+        else:
+            raise RuntimeError(f"make_teacher_case: no safe draw for video {i} ({kind}, T={T})")
+        feats.append(f)
+        vids.append(f"v{seed}_{i:04d}_{kind}")
+    return {"classes": cls, "names": names, "features": feats, "vids": vids, "dup_rows": sorted(dup_rows)}
+
+
+def teacher_case_sha256(case):
+    import hashlib
+    import json
+
+    h = hashlib.sha256(case["classes"].tobytes())
+    h.update(json.dumps([case["names"], case["vids"]]).encode())
+    for f in case["features"]:
+        h.update(str(f.shape).encode())
+        h.update(f.tobytes())
+    return h.hexdigest()
