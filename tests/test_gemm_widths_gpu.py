@@ -10,6 +10,7 @@ last column tile.  Outputs are pre-filled with NaN; columns [N, ld) must still h
 S = |A| |B|^T + |bias| and c = 4 (ceil(log2 K) + 1), plus half an ulp for 16-bit results.
 """
 import ctypes
+import itertools
 import math
 
 import pytest
@@ -124,3 +125,52 @@ def test_gemm_width_fp16x3(bn):
     assert torch.isfinite(out32).all() and (err <= bound).all(), f"bn {bn}: worst err / bound {float((err / bound).max()):.3g}"
     assert not torch.isnan(out16).any()
     assert torch.equal(out16[0], out32.half())
+
+
+OP_CASES = [c for c in itertools.product((0, 1), (0, 1), (0, 1), (1, 2), (1, 2)) if not (c[4] == 2 and c[2])]  # clusters: K-major B
+
+
+@pytest.mark.parametrize("fmt,a_mn,b_mn,ksplit,cluster", OP_CASES)
+def test_op_gemm_matches_group(fmt, a_mn, b_mn, ksplit, cluster):
+    """univtg_op_gemm (cluster 1) and univtg_op_gemm_cluster (cluster 2) run the kernel with the same parameters as
+    univtg_op_gemm_group on the equivalent problem, so their outputs agree bit for bit.  With ksplit 2 the two partial sums are
+    added with atomics: within one fp32 ulp of the magnitude.  An MN-major operand's pitch is its M / N: both multiples of 8."""
+    bn, Mo = 192, 336
+    N = 2 * bn - 16
+    g = torch.Generator().manual_seed(16 * fmt + 8 * a_mn + 4 * b_mn + 2 * ksplit + cluster)
+    dt = DT[fmt]
+    a = torch.randn(Mo, K, generator=g).to(dt)
+    b = (torch.randn(N, K, generator=g) * 0.1).to(dt)
+    a_buf = (a.t() if a_mn else a).contiguous().cuda()
+    b_buf = (b.t() if b_mn else b).contiguous().cuda()
+    bias = torch.randn(N, generator=g).cuda()
+    alpha = 0.5
+
+    def outputs():  # split-K accumulates into a zeroed out32 and cannot store out16
+        if ksplit > 1:
+            return torch.zeros(Mo, N, device="cuda"), None
+        return torch.full((Mo, N), float("nan"), device="cuda"), torch.full((Mo, N), float("nan"), dtype=dt, device="cuda")
+
+    o32, o16 = outputs()
+    fn = lib().univtg_op_gemm_cluster if cluster == 2 else lib().univtg_op_gemm
+    _lib.check(fn(_lib.ptr(a_buf), _lib.ptr(b_buf), Mo, N, K, a_mn, b_mn, fmt, bn, ksplit, _lib.ptr(bias), 0, alpha, _lib.ptr(o32),
+                  _lib.ptr(o16), _lib.stream_ptr()), "op_gemm")
+    r32, r16 = outputs()
+    p = _lib.GemmProblem()
+    p.ksplit, p.a_fmt, p.b_fmt, p.out_fmt, p.alpha, p.colsum_scale = ksplit, -1, -1, -1, alpha, 1.0
+    p.a, p.lda, p.a_mn = a_buf.data_ptr(), Mo if a_mn else K, a_mn
+    p.b, p.ldb, p.b_mn = b_buf.data_ptr(), N if b_mn else K, b_mn
+    p.M, p.N, p.K = Mo, N, K
+    p.bias, p.out32, p.ld32, p.out16, p.ld16 = bias.data_ptr(), r32.data_ptr(), N, r16.data_ptr() if r16 is not None else None, N
+    _lib.check(lib().univtg_op_gemm_group((_lib.GemmProblem * 1)(p), 1, fmt, bn, cluster, None, _lib.stream_ptr()), "op_gemm_group")
+    torch.cuda.synchronize()
+    name = f"fmt{fmt}/a_mn{a_mn}/b_mn{b_mn}/ksplit{ksplit}/cl{cluster}"
+    assert torch.isfinite(o32).all() and torch.isfinite(r32).all(), f"{name}: out32 not fully written"
+    if ksplit == 1:
+        assert torch.equal(o32, r32), f"{name}: out32 differs from univtg_op_gemm_group"
+        assert torch.isfinite(o16).all() and torch.equal(o16, r16), f"{name}: out16 differs from univtg_op_gemm_group"
+    else:
+        ad, bd = a.double().cuda(), b.double().cuda()
+        S = alpha * (ad.abs() @ bd.abs().t()) + bias.double().abs()
+        err = (o32.double() - r32.double()).abs()
+        assert (err <= 2 * U * S).all(), f"{name}: worst difference / (2^-23 S) {float((err / (2 * U * S)).max()):.3g}"

@@ -17,7 +17,7 @@ int univtg_abi_version(void) { return UNIVTG_ABI_VERSION; }
 
 int univtg_num_params(const univtg_config* cfg) {
   if (!check_cfg(cfg)) return -1;
-  return 8 * cfg->n_input_proj + 1 + 12 * cfg->enc_layers + 12 + 1;
+  return ParamIndex(*cfg).count();
 }
 
 size_t univtg_packed_bytes(const univtg_config* cfg) {
@@ -47,41 +47,39 @@ static int pack_impl(const univtg_config* cfg, const float* const* params, int32
   pk.st = (cudaStream_t)stream;
   pk.tab.n = 0;
   pk.skip_matrices = mode == 1;
-  int idx = 0;
-  const int type_idx = 8 * cfg->n_input_proj;  // token_type_embeddings.weight [2, d]
-  const float* type_emb = params[type_idx];
+  const ParamIndex ix(*cfg);
+  const float* type_emb = params[ix.type()];  // token_type_embeddings.weight [2, d]
   for (int s = 0; s < 2; ++s) {
     const ProjPacked* pp = s == 0 ? L.vid : L.txt;
     for (int i = 0; i < cfg->n_input_proj; ++i) {
-      pk.vec(params[idx + 0], pp[i].ln_w, pp[i].din);
-      pk.vec(params[idx + 1], pp[i].ln_b, pp[i].din);
-      pk.rows(params[idx + 2], pp[i].w16, d, pp[i].din, pp[i].kpad);
+      const float* const* pr = params + (s == 0 ? ix.vid(i, 0) : ix.txt(i, 0));
+      pk.vec(pr[0], pp[i].ln_w, pp[i].din);
+      pk.vec(pr[1], pp[i].ln_b, pp[i].din);
+      pk.rows(pr[2], pp[i].w16, d, pp[i].din, pp[i].kpad);
       const bool last = (i == cfg->n_input_proj - 1);
       // token_type_embeddings: index 1 for video tokens, 0 for text tokens (model/univtg.py:114-115)
-      pk.vec(params[idx + 3], pp[i].bias, d, last ? type_emb + (s == 0 ? d : 0) : nullptr);
-      idx += 4;
+      pk.vec(pr[3], pp[i].bias, d, last ? type_emb + (s == 0 ? d : 0) : nullptr);
     }
   }
-  idx += 1;  // type embedding consumed above
   for (int l = 0; l < cfg->enc_layers; ++l) {
     const LayerPacked& lp = L.layer[l];
-    pk.rows(params[idx + 0], lp.w_in, 3 * d, d, d);
-    pk.vec(params[idx + 1], lp.b_in, 3 * d);
-    pk.rows(params[idx + 2], lp.w_out, d, d, d);
-    pk.vec(params[idx + 3], lp.b_out, d);
-    pk.rows(params[idx + 4], lp.w1, ff, d, d);
-    pk.vec(params[idx + 5], lp.b1, ff);
-    pk.rows(params[idx + 6], lp.w2, d, ff, ff);
-    pk.vec(params[idx + 7], lp.b2, d);
-    pk.vec(params[idx + 8], lp.n1w, d);
-    pk.vec(params[idx + 9], lp.n1b, d);
-    pk.vec(params[idx + 10], lp.n2w, d);
-    pk.vec(params[idx + 11], lp.n2b, d);
-    idx += 12;
+    const float* const* pr = params + ix.layer(l, 0);
+    pk.rows(pr[0], lp.w_in, 3 * d, d, d);
+    pk.vec(pr[1], lp.b_in, 3 * d);
+    pk.rows(pr[2], lp.w_out, d, d, d);
+    pk.vec(pr[3], lp.b_out, d);
+    pk.rows(pr[4], lp.w1, ff, d, d);
+    pk.vec(pr[5], lp.b1, ff);
+    pk.rows(pr[6], lp.w2, d, ff, ff);
+    pk.vec(pr[7], lp.b2, d);
+    pk.vec(pr[8], lp.n1w, d);
+    pk.vec(pr[9], lp.n1b, d);
+    pk.vec(pr[10], lp.n2w, d);
+    pk.vec(pr[11], lp.n2b, d);
   }
   // span_embed.layers.{0,1,2}, class_embed.layers.{0,1,2}
-  const float* const* sp = params + idx;
-  const float* const* cl = params + idx + 6;
+  const float* const* sp = params + ix.span(0);
+  const float* const* cl = params + ix.cls(0);
   // fused first conv: rows [0,d) = class_embed.layers.0, rows [d,2d) = span_embed.layers.0
   pk.conv(cl[0], L.conv1_w, d, d);
   pk.conv(sp[0], L.conv1_w + (size_t)d * 3 * d * 2, d, d);
@@ -95,8 +93,7 @@ static int pack_impl(const univtg_config* cfg, const float* const* params, int32
   pk.vec(cl[5], L.conv3c_b, 1);
   pk.conv_f32(sp[4], L.conv3s_w, 2, d);
   pk.vec(sp[5], L.conv3s_b, 2);
-  idx += 12;
-  pk.vec(params[idx], L.pool_w, d);
+  pk.vec(params[ix.pool()], L.pool_w, d);
   pk.flush();
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) {
@@ -366,13 +363,7 @@ int run_forward(univtg_plan* P, const FwdBufs& W, const float* src_txt, const fl
   const long long pk_lo = P->pk_lo, ws_lo = P->ws_lo;
   int rc = 0;
   GemmGroup g;
-  auto group = [&](int num) {
-    memset(&g, 0, sizeof(g));
-    g.num = num;
-    g.fmt = fmt;
-    g.split = split;
-    g.lo16 = ws_lo;
-  };
+  auto group = [&](int num) { reset_group(g, num, fmt, split, ws_lo); };
   // every launch is followed by a profiling mark of its kind: 0 row kernel, 1 tensor-core GEMM, 2 attention
   auto marked = [&](int r, int kind) {
     if (r == 0) prof_mark(P, st, kind);
@@ -725,36 +716,16 @@ static int op_gemm_impl(const void* a, const void* b, int32_t M, int32_t N, int3
     return 1;
   }
   GemmGroup g;
-  memset(&g, 0, sizeof(g));
-  g.num = 1;
-  g.fmt = split ? 0 : fmt;
+  reset_group(g, 1, split ? 0 : fmt, split ? 1 : 0, split ? (long long)M * N : 0);
   g.cluster = cluster;
-  g.split = split ? 1 : 0;
-  g.lo16 = split ? (long long)M * N : 0;
   GemmProblem& p = g.p[0];
-  init_problem(p);
-  p.M = M;
-  p.N = N;
-  p.a_mn = a_mn;
-  p.b_mn = b_mn;
-  p.kblk_per_tap = (K + 63) / 64;
-  p.ksplit = ksplit < 1 ? 1 : ksplit;
-  int rc = 0;
-  if (!a_mn) {
-    rc |= make_tmap_op(&p.tm_a, a, (uint64_t)M, (uint64_t)K, (uint64_t)K, GEMM_BM, 64, split ? (long long)M * K : 0);
-  } else {
-    rc |= make_tmap_2d(&p.tm_a, a, (uint64_t)K, (uint64_t)M, (uint64_t)M, 64, 64);
-    p.ca = OperandCoord{0, 1, 0, 0, 0, 0, 0, 1};  // c0 = m0, c1 = k
-  }
-  if (!b_mn) {
-    rc |= make_tmap_op(&p.tm_b, b, (uint64_t)N, (uint64_t)K, (uint64_t)K, (uint32_t)(cluster == 2 ? bn / 2 : bn), 64,
-                       split ? (long long)N * K : 0);
-    p.b_box_rows = cluster == 2 ? bn / 2 : bn;
-  } else {
-    rc |= make_tmap_b_mn(p, b, (uint64_t)K, (uint64_t)N, (uint64_t)N, bn);
-    p.cb = OperandCoord{0, 1, 0, 0, 0, 0, 0, 1};
-  }
+  const uint16_t *a16 = reinterpret_cast<const uint16_t*>(a), *b16 = reinterpret_cast<const uint16_t*>(b);
+  const Mat16 A = a_mn ? Mat16{a16, K, M, M} : Mat16{a16, M, K, K};
+  const Mat16 Bm = b_mn ? Mat16{b16, K, N, N} : Mat16{b16, N, K, K};
+  const int rc = setup_gemm(p, A, a_mn, Bm, b_mn, M, N, K, cluster == 2 ? bn / 2 : bn, split ? (long long)M * K : 0,
+                            split ? (long long)N * K : 0);
   if (rc) return rc;
+  p.ksplit = ksplit < 1 ? 1 : ksplit;
   p.bias = bias;
   p.act = act;
   p.alpha = alpha;

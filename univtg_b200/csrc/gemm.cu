@@ -652,9 +652,6 @@ typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t,
                                   const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
                                   CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 
-int make_tmap_2d_uncached(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols, uint64_t ld_elems, uint32_t box_rows,
-                          uint32_t box_cols);
-
 static EncodeTiledFn get_encode_fn() {
   static EncodeTiledFn fn = nullptr;
   if (fn) return fn;
@@ -698,117 +695,65 @@ static inline TmapSlot* tmap_slot(const TmapKey& k) {
   return g_tmap_cache ? &g_tmap_cache[h & (kTmapCacheSlots - 1)] : nullptr;
 }
 
-int make_tmap_2d(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols, uint64_t ld_elems, uint32_t box_rows,
-                 uint32_t box_cols) {
-  const TmapKey key{base, rows, cols, ld_elems, box_rows, box_cols, 2u, 0};
+// The tensor map of `key` from the cache, or encoded over 16-bit elements (128-byte swizzle, zero fill out of bounds) and stored.
+// dims / box: innermost first; strides: bytes between consecutive entries of dims 1 .. rank - 1.
+static int make_tmap_cached(CUtensorMap* out, const TmapKey& key, cuuint32_t rank, const cuuint64_t* dims, const cuuint64_t* strides,
+                            const cuuint32_t* box) {
   TmapSlot* slot = tmap_slot(key);
   if (slot != nullptr && slot->used && slot->key == key) {
     *out = slot->map;
     return 0;
   }
-  const int rc = make_tmap_2d_uncached(out, base, rows, cols, ld_elems, box_rows, box_cols);
-  if (rc == 0 && slot != nullptr) {
+  EncodeTiledFn fn = get_encode_fn();
+  if (!fn) return 1;
+  const char* what = key.kind == 4 ? "fp16x3 pair" : key.kind == 3 ? "3-D MN-major B" : "2-D";
+  bool aligned = (reinterpret_cast<uintptr_t>(key.base) & 15) == 0;
+  for (cuuint32_t i = 0; i + 1 < rank; ++i) aligned = aligned && strides[i] % 16 == 0;
+  if (!aligned) {
+    set_error("tensor map (%s): base %p, pitch %llu B and lo-plane offset %llu B must be 16-byte aligned", what, key.base,
+              (unsigned long long)(key.ld * 2), (unsigned long long)(key.plane * 2));
+    return 2;
+  }
+  const cuuint32_t estr[3] = {1, 1, 1};
+  CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_UINT16, rank, const_cast<void*>(key.base), dims, strides, box, estr,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) {
+    set_error("cuTensorMapEncodeTiled (%s) failed: CUresult %d (rows %llu cols %llu ld %llu lo %llu box %ux%u)", what, (int)r,
+              (unsigned long long)key.rows, (unsigned long long)key.cols, (unsigned long long)key.ld, (unsigned long long)key.plane,
+              key.box_rows, key.box_cols);
+    return 3;
+  }
+  if (slot != nullptr) {
     slot->key = key;
     slot->map = *out;
     slot->used = true;
   }
-  return rc;
+  return 0;
 }
 
-int make_tmap_2d_uncached(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols, uint64_t ld_elems, uint32_t box_rows,
-                          uint32_t box_cols) {
-  EncodeTiledFn fn = get_encode_fn();
-  if (!fn) return 1;
-  if ((reinterpret_cast<uintptr_t>(base) & 15) != 0 || (ld_elems * 2) % 16 != 0) {
-    set_error("tensor map: base %p / pitch %llu B not 16-byte aligned", base, (unsigned long long)(ld_elems * 2));
-    return 2;
-  }
-  cuuint64_t dims[2] = {cols, rows};
-  cuuint64_t strides[1] = {ld_elems * 2};
-  cuuint32_t box[2] = {box_cols, box_rows};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_UINT16, 2, const_cast<void*>(base), dims, strides, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    set_error("cuTensorMapEncodeTiled failed: CUresult %d (rows %llu cols %llu ld %llu box %ux%u)", (int)r,
-              (unsigned long long)rows, (unsigned long long)cols, (unsigned long long)ld_elems, box_rows, box_cols);
-    return 3;
-  }
-  return 0;
+int make_tmap_2d(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols, uint64_t ld_elems, uint32_t box_rows,
+                 uint32_t box_cols) {
+  const cuuint64_t dims[2] = {cols, rows}, strides[1] = {ld_elems * 2};
+  const cuuint32_t box[2] = {box_cols, box_rows};
+  return make_tmap_cached(out, TmapKey{base, rows, cols, ld_elems, box_rows, box_cols, 2u, 0}, 2, dims, strides, box);
 }
 
 int make_tmap_split(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols, uint64_t ld_elems, uint32_t box_rows,
                     uint32_t box_cols, uint64_t lo_elems) {
-  const TmapKey key{base, rows, cols, ld_elems, box_rows, box_cols, 4u, lo_elems};
-  TmapSlot* slot = tmap_slot(key);
-  if (slot != nullptr && slot->used && slot->key == key) {
-    *out = slot->map;
-    return 0;
-  }
-  EncodeTiledFn fn = get_encode_fn();
-  if (!fn) return 1;
-  if ((reinterpret_cast<uintptr_t>(base) & 15) != 0 || (ld_elems * 2) % 16 != 0 || (lo_elems * 2) % 16 != 0) {
-    set_error("tensor map: base %p / pitch %llu B / lo-plane offset %llu B not 16-byte aligned", base, (unsigned long long)(ld_elems * 2),
-              (unsigned long long)(lo_elems * 2));
-    return 2;
-  }
-  cuuint64_t dims[3] = {cols, rows, 2};
-  cuuint64_t strides[2] = {ld_elems * 2, lo_elems * 2};
-  cuuint32_t box[3] = {box_cols, box_rows, 1};
-  cuuint32_t estr[3] = {1, 1, 1};
-  CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_UINT16, 3, const_cast<void*>(base), dims, strides, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    set_error("cuTensorMapEncodeTiled (fp16x3 pair) failed: CUresult %d (rows %llu cols %llu ld %llu lo %llu box %ux%u)", (int)r,
-              (unsigned long long)rows, (unsigned long long)cols, (unsigned long long)ld_elems, (unsigned long long)lo_elems, box_rows,
-              box_cols);
-    return 3;
-  }
-  if (slot != nullptr) {
-    slot->key = key;
-    slot->map = *out;
-    slot->used = true;
-  }
-  return 0;
+  const cuuint64_t dims[3] = {cols, rows, 2}, strides[2] = {ld_elems * 2, lo_elems * 2};
+  const cuuint32_t box[3] = {box_cols, box_rows, 1};
+  return make_tmap_cached(out, TmapKey{base, rows, cols, ld_elems, box_rows, box_cols, 4u, lo_elems}, 3, dims, strides, box);
 }
 
-int make_tmap_b_mn(GemmProblem& p, const void* base, uint64_t rows, uint64_t cols, uint64_t ld_elems, int bn, bool allow_3d) {
+int make_tmap_b_mn(GemmProblem& p, const void* base, uint64_t rows, uint64_t cols, uint64_t ld_elems, int bn) {
   p.b_3d = 0;
-  if (!allow_3d || cols % 64 != 0 || bn % 64 != 0 || bn < 64) return make_tmap_2d(&p.tm_b, base, rows, cols, ld_elems, 64, 64);
-  const TmapKey key{base, rows, cols, ld_elems, (uint32_t)bn, 64u, 3u, 0};
-  TmapSlot* slot = tmap_slot(key);
-  if (slot != nullptr && slot->used && slot->key == key) {
-    p.tm_b = slot->map;
-    p.b_3d = bn / 64;
-    return 0;
-  }
-  EncodeTiledFn fn = get_encode_fn();
-  if (!fn) return 1;
-  if ((reinterpret_cast<uintptr_t>(base) & 15) != 0 || (ld_elems * 2) % 16 != 0) {
-    set_error("tensor map: base %p / pitch %llu B not 16-byte aligned", base, (unsigned long long)(ld_elems * 2));
-    return 2;
-  }
-  cuuint64_t dims[3] = {64, rows, cols / 64};
-  cuuint64_t strides[2] = {ld_elems * 2, 128};
-  cuuint32_t box[3] = {64, 64, (cuuint32_t)(bn / 64)};
-  cuuint32_t estr[3] = {1, 1, 1};
-  CUresult r = fn(&p.tm_b, CU_TENSOR_MAP_DATA_TYPE_UINT16, 3, const_cast<void*>(base), dims, strides, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    set_error("cuTensorMapEncodeTiled (3-D MN-major B) failed: CUresult %d (rows %llu cols %llu ld %llu bn %d)", (int)r,
-              (unsigned long long)rows, (unsigned long long)cols, (unsigned long long)ld_elems, bn);
-    return 3;
-  }
-  p.b_3d = bn / 64;
-  if (slot != nullptr) {
-    slot->key = key;
-    slot->map = p.tm_b;
-    slot->used = true;
-  }
-  return 0;
+  if (cols % 64 != 0 || bn % 64 != 0 || bn < 64) return make_tmap_2d(&p.tm_b, base, rows, cols, ld_elems, 64, 64);
+  const cuuint64_t dims[3] = {64, rows, cols / 64}, strides[2] = {ld_elems * 2, 128};
+  const cuuint32_t box[3] = {64, 64, (cuuint32_t)(bn / 64)};
+  const int rc = make_tmap_cached(&p.tm_b, TmapKey{base, rows, cols, ld_elems, (uint32_t)bn, 64u, 3u, 0}, 3, dims, strides, box);
+  if (rc == 0) p.b_3d = bn / 64;
+  return rc;
 }
 
 int launch_gemm_group(GemmGroup& g, int bn, int num_sms, cudaStream_t stream, int* used_full) {

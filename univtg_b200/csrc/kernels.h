@@ -106,7 +106,7 @@ struct TileChoice {
 TileChoice choose_tile(const int* Ms, const int* Ns, const int* kblocks, int num, int num_sms, int step, int max_split);
 // MN-major B operand [rows = K, cols = N] (N contiguous): a 3-D view {64, K, N/64} lets one TMA instruction fetch the whole
 // 64 x bn tile of a k-block (fewer TMA operations per k-block than one 2-D box per 64-wide block); needs cols % 64 == 0.
-int make_tmap_b_mn(GemmProblem& p, const void* base, uint64_t rows, uint64_t cols, uint64_t ld_elems, int bn, bool allow_3d = true);
+int make_tmap_b_mn(GemmProblem& p, const void* base, uint64_t rows, uint64_t cols, uint64_t ld_elems, int bn);
 
 // Encode a 2-D tensor map over a row-major 16-bit matrix [rows, cols] with row pitch `ld` elements,
 // box {box_cols, box_rows}, 128-byte swizzle, zero fill out of bounds.  Returns 0 on success.

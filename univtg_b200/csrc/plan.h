@@ -57,6 +57,22 @@ struct PackedLayout {
   size_t total;
 };
 
+// Order of the parameter tensors (univtg_pack_weights' params, univtg_backward's grads): per projector layer [ln.weight, ln.bias,
+// W, b], video layers then text layers; token_type_embeddings; 12 tensors per encoder layer; span_embed.layers.{0,1,2} (weight,
+// bias each), then class_embed's; weightedpool.weight.
+struct ParamIndex {
+  int np, nl;
+  explicit ParamIndex(const univtg_config& c) : np(c.n_input_proj), nl(c.enc_layers) {}
+  int vid(int i, int k) const { return 4 * i + k; }
+  int txt(int i, int k) const { return 4 * np + 4 * i + k; }
+  int type() const { return 8 * np; }
+  int layer(int l, int k) const { return 8 * np + 1 + 12 * l + k; }
+  int span(int k) const { return layer(nl, k); }
+  int cls(int k) const { return span(6 + k); }
+  int pool() const { return span(12); }
+  int count() const { return pool() + 1; }
+};
+
 struct Cursor {
   size_t off = 0;
   size_t take(size_t bytes) {
@@ -387,6 +403,15 @@ inline int gemm_launch(univtg_plan* P, GemmGroup& g, int bn, int sms, cudaStream
   return rc;
 }
 
+// Empties `g` for `num` problems in 16-bit format `fmt`; split / lo16: fp16x3 (GemmGroup).
+inline void reset_group(GemmGroup& g, int num, int fmt, int split = 0, long long lo16 = 0) {
+  memset(&g, 0, sizeof(g));
+  g.num = num;
+  g.fmt = fmt;
+  g.split = split;
+  g.lo16 = lo16;
+}
+
 // Longest sequence the SIMT attention backward can stage (attention_bwd_simt_smem = 32 L bytes) in the device's opt-in shared
 // memory per block.  Without a device to ask, the sm_90 value (227 KB, the only target the library is built for) is used.
 inline int attention_bwd_simt_max_L() {
@@ -397,6 +422,28 @@ inline int attention_bwd_simt_max_L() {
     optin = 227 * 1024;
   }
   return (int)((size_t)optin / attention_bwd_simt_smem(1));
+}
+
+// Arguments of the attention core backward over qkv [B*L, 3d] and dO [B*L, d], both in 16-bit format `fmt` (d = H dh), for
+// attention_bwd_route; the caller adds the dropout spec.
+inline AttnBwdArgs attention_bwd_args(const void* qkv, const void* dO, const float* key_mask, const float* lse, const float* delta,
+                                      float* dqkv32, int B, int L, int H, int dh, int fmt) {
+  AttnBwdArgs a;
+  memset(&a, 0, sizeof(a));
+  a.qkv = reinterpret_cast<const uint16_t*>(qkv);
+  a.dO = reinterpret_cast<const uint16_t*>(dO);
+  a.key_mask = key_mask;
+  a.lse = lse;
+  a.delta = delta;
+  a.dqkv32 = dqkv32;
+  a.scale = 1.0f / sqrtf((float)dh);
+  a.B = B;
+  a.L = L;
+  a.H = H;
+  a.dh = dh;
+  a.d = H * dh;
+  a.fmt_act = a.fmt_grad = fmt;
+  return a;
 }
 
 // Routing of the attention core backward, shared by univtg_backward and the single-operator entry points.  `a` holds everything but
@@ -498,19 +545,16 @@ int conv_fwd_problem(GemmProblem& p, int Mh, const uint16_t* X, int lda, int Cin
 }
 
 // k=3 Conv1d backward in the conv-head layout (buffer row = logical row + 1; rows 0, Mh + 1 and every sample's separator row are
-// zeros).  fmt_g / fmt_w: formats of the gradient / weight-or-activation operand.
+// zeros).
 // dgrad: dX[m] = sum_t' dY[m + t' - 1] W[:, :, 2 - t'] over Mh logical rows.  A = dY [Mh + 2, Kc] (pitch ldy, K-major, row-shifted
 // by the tap), B = packed W [Kc, 3 * Cin] (MN-major, w2[o, t * Cin + c] = W[o, c, t]); N = Cin, K = 3 taps x Kc (Kc % 64 == 0).
-int conv_dgrad_problem(GemmProblem& p, int Mh, const uint16_t* dY, int ldy, int Kc, const uint16_t* Wp, int Cin, int bn, int fmt_g,
-                       int fmt_w) {
+int conv_dgrad_problem(GemmProblem& p, int Mh, const uint16_t* dY, int ldy, int Kc, const uint16_t* Wp, int Cin, int bn) {
   init_problem(p);
   p.M = Mh;
   p.N = Cin;
   p.taps = 3;
   p.kblk_per_tap = Kc / 64;
   p.b_mn = 1;
-  p.a_fmt = fmt_g;
-  p.b_fmt = fmt_w;
   p.ca = OperandCoord{0, 0, 0, 1, 0, 1, 1, 0};           // rows m0 + t', cols k
   p.cb = OperandCoord{2 * Cin, 1, -Cin, 0, 0, 0, 0, 1};  // cols n0 + (2 - t') * Cin, rows k (out channel)
   int r = make_tmap_2d(&p.tm_a, dY, (uint64_t)Mh + 2, (uint64_t)Kc, (uint64_t)ldy, GEMM_BM, 64);
@@ -519,15 +563,12 @@ int conv_dgrad_problem(GemmProblem& p, int Mh, const uint16_t* dY, int ldy, int 
 }
 // wgrad of tap t: dW[n, c, t] = sum_m dY[m, n] X[m + t - 1, c] over Mh logical rows.  A = dY [Mh + 2, Nc] (pitch ldy, MN-major),
 // B = X [Mh + 2, Cin] (pitch ldx, MN-major, row-shifted by t); M = Nc, N = Cin, K = Mh.
-int conv_wgrad_problem(GemmProblem& p, int Mh, const uint16_t* dY, int ldy, int Nc, const uint16_t* X, int ldx, int Cin, int t, int bn,
-                       int fmt_g, int fmt_w) {
+int conv_wgrad_problem(GemmProblem& p, int Mh, const uint16_t* dY, int ldy, int Nc, const uint16_t* X, int ldx, int Cin, int t, int bn) {
   init_problem(p);
   p.M = Nc;
   p.N = Cin;
   p.a_mn = 1;
   p.b_mn = 1;
-  p.a_fmt = fmt_g;
-  p.b_fmt = fmt_w;
   p.kblk_per_tap = (Mh + 63) / 64;
   p.ca = OperandCoord{0, 1, 0, 0, 1, 0, 0, 1};  // cols m0 (out channel), rows 1 + k
   p.cb = OperandCoord{0, 1, 0, 0, t, 0, 0, 1};  // cols n0 (in channel), rows t + k

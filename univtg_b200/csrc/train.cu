@@ -207,7 +207,8 @@ int univtg_backward(univtg_plan* P, void* ws, const float* src_txt, const float*
   }
   if (refuse_split(P->cfg, "univtg_backward")) return 1;
   const univtg_config& c = P->cfg;
-  const int n_params = univtg_num_params(&c) + (P->txt_pos_on ? 3 : 0);  // + txt_position_embed.* with learned text positions
+  const ParamIndex ix(c);
+  const int n_params = ix.count() + (P->txt_pos_on ? 3 : 0);  // + txt_position_embed.* with learned text positions
   if (n_grads != n_params) {
     set_error("univtg_backward: expected %d gradient tensors (text positions %s), got %d", n_params, P->txt_pos_on ? "on" : "off",
               n_grads);
@@ -230,22 +231,12 @@ int univtg_backward(univtg_plan* P, void* ws, const float* src_txt, const float*
   // persistent GEMM grids assume every CTA is resident at once; when a gradient all-reduce runs beside the backward its CTAs
   // hold some SMs, and a full-width grid would wait for them (a second wave): launch on the SMs that are left
   const int sms = (P->num_sms_bwd > 0 && P->num_sms_bwd < P->num_sms) ? P->num_sms_bwd : P->num_sms;
-  const int FMT_G = fmt;                 // gradient operand format == activation operand format
   const float GS = grad_scale;           // loss scale carried by every intermediate gradient
   const float INV = 1.0f / grad_scale;   // applied wherever a parameter gradient is written
 
   int rc = 0;
   GemmGroup g;
-  // parameter-gradient index map (univtg_pack_weights order)
   const int np = c.n_input_proj;
-  auto G_vid = [&](int i, int k) { return grads[4 * i + k]; };
-  auto G_txt = [&](int i, int k) { return grads[4 * np + 4 * i + k]; };
-  float* G_type = grads[8 * np];
-  auto G_layer = [&](int l, int k) { return grads[8 * np + 1 + 12 * l + k]; };
-  const int hb = 8 * np + 1 + 12 * c.enc_layers;
-  auto G_span = [&](int k) { return grads[hb + k]; };
-  auto G_cls = [&](int k) { return grads[hb + 6 + k]; };
-  float* G_pool = grads[hb + 12];
   const bool txt_pos = P->txt_pos_on != 0;
   const TxtPosWs TP = txt_pos ? make_txt_pos_ws(c, P->shp, P->txt_pos.scratch) : TxtPosWs{};
   const TxtRows txt_rows = txt_pos ? TxtRows{TP.dqk16, L, Lv, 2 * d} : TxtRows{nullptr, 0, 0, 0};
@@ -267,17 +258,17 @@ int univtg_backward(univtg_plan* P, void* ws, const float* src_txt, const float*
     a.dz = T.dz;
     a.dh_cls = T.dhc2;
     a.dh_span = T.dhs2;
-    a.gw_cls = G_cls(4);
-    a.gb_cls = G_cls(5);
-    a.gw_span = G_span(4);
-    a.gb_span = G_span(5);
-    a.cs_cls = G_cls(3);   // bias gradient of class_embed.layers.1 = column sums of d(hidden 2)
-    a.cs_span = G_span(3);
+    a.gw_cls = grads[ix.cls(4)];
+    a.gb_cls = grads[ix.cls(5)];
+    a.gw_span = grads[ix.span(4)];
+    a.gb_span = grads[ix.span(5)];
+    a.cs_cls = grads[ix.cls(3)];   // bias gradient of class_embed.layers.1 = column sums of d(hidden 2)
+    a.cs_span = grads[ix.span(3)];
     a.B = B;
     a.Lv = Lv;
     a.d = d;
     a.fmt_act = fmt;
-    a.fmt_grad = FMT_G;
+    a.fmt_grad = fmt;
     a.in_scale = GS;
     a.pgrad_scale = INV;
     rc = launch_head_final_bwd(a, st);
@@ -285,12 +276,12 @@ int univtg_backward(univtg_plan* P, void* ws, const float* src_txt, const float*
 
     // conv layout helpers (conv_dgrad_problem / conv_wgrad_problem, plan.h): buffer row = logical row + 1
     auto conv_dgrad = [&](GemmProblem& p, const uint16_t* dY, int ldy, int Kc /*out channels*/, const uint16_t* Wp /*[Kc, 3*Cin]*/,
-                          int Cin, int bnn) -> int { return conv_dgrad_problem(p, Mh, dY, ldy, Kc, Wp, Cin, bnn, FMT_G, fmt); };
+                          int Cin, int bnn) -> int { return conv_dgrad_problem(p, Mh, dY, ldy, Kc, Wp, Cin, bnn); };
     // wgrad of one tap, written as a tap-major plane of T.wtap (launch_tap_interleave then builds the [N, C, 3] layout with 256-bit
     // stores here instead of stride-3 scalars)
     const TileChoice t_cw = tile_for(sms, 64, 8, MNK{d, d, Mh}, MNK{d, d, Mh}, MNK{d, d, Mh});
     auto conv_wgrad = [&](GemmProblem& p, const uint16_t* dY, int ldy, int Nc, const uint16_t* X, int ldx, int Cin, int t) -> int {
-      const int r = conv_wgrad_problem(p, Mh, dY, ldy, Nc, X, ldx, Cin, t, t_cw.bn, FMT_G, fmt);
+      const int r = conv_wgrad_problem(p, Mh, dY, ldy, Nc, X, ldx, Cin, t, t_cw.bn);
       p.out32 = T.wtap + (size_t)t * Nc * Cin;
       p.ld32 = Cin;
       p.alpha = INV;
@@ -301,14 +292,10 @@ int univtg_backward(univtg_plan* P, void* ws, const float* src_txt, const float*
     const int bn_c1d = tile_for(sms, 64, 1, MNK{Mh, d, 6 * d}).bn;
     // (splitting the k-blocks of the layer-1 dgrad - 76 tiles of 96 k-blocks - over idle SMs saves ~8 us but reduces into the stream
     // gradient with atomics, which makes every gradient upstream of the heads order-dependent in its last bits: not taken)
-    const int bn_cw = t_cw.bn;
-    const int bn = bn_c2d;
     // ---- conv layer 2 (two heads): dgrad -> dh1 [Mh+2, 2d] (class cols [0,d), span cols [d,2d)), ReLU mask of h1 ----
-    memset(&g, 0, sizeof(g));
-    g.num = 2;
-    g.fmt = fmt;
-    rc |= conv_dgrad(g.p[0], T.dhc2, d, d, W16(Lw.conv2c_w), d, bn);
-    rc |= conv_dgrad(g.p[1], T.dhs2, d, d, W16(Lw.conv2s_w), d, bn);
+    reset_group(g, 2, fmt);
+    rc |= conv_dgrad(g.p[0], T.dhc2, d, d, W16(Lw.conv2c_w), d, bn_c2d);
+    rc |= conv_dgrad(g.p[1], T.dhs2, d, d, W16(Lw.conv2s_w), d, bn_c2d);
     if (rc) return rc;
     for (int s = 0; s < 2; ++s) {
       GemmProblem& p = g.p[s];
@@ -320,30 +307,25 @@ int univtg_backward(univtg_plan* P, void* ws, const float* src_txt, const float*
       p.ld_mask = 2 * d;
       p.out16 = T.dh1 + s * d;
       p.ld16 = 2 * d;
-      p.out_fmt = FMT_G;
-      p.colsum = s == 0 ? G_cls(1) : G_span(1);  // bias gradient of conv layer 0 (saves a separate column-sum pass)
+      p.colsum = grads[s == 0 ? ix.cls(1) : ix.span(1)];  // bias gradient of conv layer 0 (saves a separate column-sum pass)
       p.colsum_scale = INV;
     }
     rc = gemm_launch(P, g, bn_c2d, sms, st);
     if (rc) return rc;
     // wgrad conv layer 2: 2 heads x 3 taps
     for (int s = 0; s < 2; ++s) {
-      memset(&g, 0, sizeof(g));
-      g.num = 3;
-      g.fmt = fmt;
+      reset_group(g, 3, fmt);
       for (int t = 0; t < 3; ++t)
         rc |= conv_wgrad(g.p[t], s == 0 ? T.dhc2 : T.dhs2, d, d, T.h1 + s * d, 2 * d, d, t);
       if (rc) return rc;
       if (t_cw.ksplit > 1) cudaMemsetAsync(T.wtap, 0, (size_t)3 * d * d * 4, st);  // split-K accumulates into the planes
-      rc = gemm_launch(P, g, bn_cw, sms, st);
+      rc = gemm_launch(P, g, t_cw.bn, sms, st);
       if (rc) return rc;
-      rc = launch_tap_interleave(T.wtap, s == 0 ? G_cls(2) : G_span(2), d, d, st);
+      rc = launch_tap_interleave(T.wtap, grads[s == 0 ? ix.cls(2) : ix.span(2)], d, d, st);
       if (rc) return rc;
     }
     // ---- conv layer 1 (fused N = 2d): dgrad -> stream gradient of the video rows ----
-    memset(&g, 0, sizeof(g));
-    g.num = 1;
-    g.fmt = fmt;
+    reset_group(g, 1, fmt);
     rc = conv_dgrad(g.p[0], T.dh1, 2 * d, 2 * d, W16(Lw.conv1_w), d, bn_c1d);
     if (rc) return rc;
     g.p[0].rps_in = Lv + 1;
@@ -356,15 +338,13 @@ int univtg_backward(univtg_plan* P, void* ws, const float* src_txt, const float*
     if (rc) return rc;
     // wgrad conv layer 1: class rows [0,d) and span rows [d,2d) of the fused weight
     for (int s = 0; s < 2; ++s) {
-      memset(&g, 0, sizeof(g));
-      g.num = 3;
-      g.fmt = fmt;
+      reset_group(g, 3, fmt);
       for (int t = 0; t < 3; ++t) rc |= conv_wgrad(g.p[t], T.dh1 + s * d, 2 * d, d, T.hA, d, d, t);
       if (rc) return rc;
       if (t_cw.ksplit > 1) cudaMemsetAsync(T.wtap, 0, (size_t)3 * d * d * 4, st);
-      rc = gemm_launch(P, g, bn_cw, sms, st);
+      rc = gemm_launch(P, g, t_cw.bn, sms, st);
       if (rc) return rc;
-      rc = launch_tap_interleave(T.wtap, s == 0 ? G_cls(0) : G_span(0), d, d, st);
+      rc = launch_tap_interleave(T.wtap, grads[s == 0 ? ix.cls(0) : ix.span(0)], d, d, st);
       if (rc) return rc;
     }
   }
@@ -382,7 +362,7 @@ int univtg_backward(univtg_plan* P, void* ws, const float* src_txt, const float*
     a.w = F32(Lw.pool_w);
     a.g_pooled = g_txt_mem_proj;
     a.dx_txt = T.dxt_pool;
-    a.gw = G_pool;
+    a.gw = grads[ix.pool()];
     a.out_scale = GS;
     a.B = B;
     a.Lt = Lt;
@@ -393,6 +373,33 @@ int univtg_backward(univtg_plan* P, void* ws, const float* src_txt, const float*
   stage_done(0);  // conv heads + weightedpool.weight
 
   // ================================================ encoder ================================================
+  // LayerNorm backward of a residual block: dx (grad of the LayerNorm output) -> dy (grad of x + s * branch), branch operand s * dy
+  // in dbr16; parameter gradients dgamma / dbeta, and dbias = column sums of s * dy (bias gradient of the branch's last linear)
+  auto ln_bwd = [&](const float* y, const float* mean, const float* rstd, const float* gamma, const float* s, float* dgamma,
+                    float* dbeta, float* dbias) -> int {
+    LnBwdArgs a;
+    memset(&a, 0, sizeof(a));
+    a.dout = T.dx;
+    a.ld_dout = d;
+    a.y = y;
+    a.ld_y = d;
+    a.mean = mean;
+    a.rstd = rstd;
+    a.gamma = gamma;
+    a.rows = M;
+    a.d = d;
+    a.row_scale = s;
+    a.L = L;
+    a.dy32 = T.dy;
+    a.dbr16 = T.dbr16;
+    a.ld16 = d;
+    a.fmt16 = fmt;
+    a.dgamma = dgamma;
+    a.dbeta = dbeta;
+    a.colsum = dbias;
+    a.pgrad_scale = INV;
+    return launch_layernorm_bwd(a, st);
+  };
   for (int l = c.enc_layers - 1; l >= 0; --l) {
     const LayerPacked& lp = Lw.layer[l];
     const float* s1 = droppath_scale ? droppath_scale + (size_t)(2 * l) * B : nullptr;
@@ -401,56 +408,28 @@ int univtg_backward(univtg_plan* P, void* ws, const float* src_txt, const float*
               bn_ddo = tile_for(sms, 64, 1, MNK{M, d, d}).bn, bn_ddq = tile_for(sms, 64, 1, MNK{M, d, 3 * d}).bn;
     const TileChoice t_wo = tile_for(sms, 64, 16, MNK{d, d, M}), t_wq = tile_for(sms, 64, 16, MNK{2 * d, d, M}, MNK{d, d, M}),
                      t_wf = tile_for(sms, 64, 16, MNK{d, ff, M}, MNK{ff, d, M});
-    const int bn_wo = t_wo.bn, bn_wq = t_wq.bn;
     // ---- LN2 backward: dx (grad of the layer output) -> dy (grad of x1 + s2 * F), branch operand s2 * dy ----
-    {
-      LnBwdArgs a;
-      memset(&a, 0, sizeof(a));
-      a.dout = T.dx;
-      a.ld_dout = d;
-      a.y = T.y2[l];
-      a.ld_y = d;
-      a.mean = T.mean2[l];
-      a.rstd = T.rstd2[l];
-      a.gamma = F32(lp.n2w);
-      a.rows = M;
-      a.d = d;
-      a.row_scale = s2;
-      a.L = L;
-      a.dy32 = T.dy;
-      a.dbr16 = T.dbr16;
-      a.ld16 = d;
-      a.fmt16 = FMT_G;
-      a.dgamma = G_layer(l, 10);
-      a.dbeta = G_layer(l, 11);
-      a.colsum = G_layer(l, 7);  // linear2.bias
-      a.pgrad_scale = INV;
-      rc = launch_layernorm_bwd(a, st);
-      if (rc) return rc;
-    }
+    rc = ln_bwd(T.y2[l], T.mean2[l], T.rstd2[l], F32(lp.n2w), s2, grads[ix.layer(l, 10)], grads[ix.layer(l, 11)],
+                grads[ix.layer(l, 7)]);  // linear2.bias
+    if (rc) return rc;
     // ---- FFN2: dgrad -> d(hpre) = (dF W2) * gelu'(hpre) (saved 16-bit derivative);  wgrad dW2 = dF^T h ----
     // ---- FFN1: dgrad d(x1) = dhpre W1 + dy (residual);          wgrad dW1 = dhpre^T x1 ----
     // (the data-gradient and weight-gradient GEMMs that read the same dY are separate launches chained by programmatic
     //  dependent launch; sharing one launch was slower per step on the earlier GPU generation and has not been re-measured)
     auto ffn2_dgrad = [&](GemmProblem& p, int bnn) -> int {
       int r = setup_gemm(p, Mat16{T.dbr16, M, d, d}, 0, Mat16{W16(lp.w2), d, ff, ff}, 1, M, ff, d, bnn);
-      p.a_fmt = FMT_G;
-      p.b_fmt = fmt;
       p.mask16 = T.dgelu16[l];  // d(hpre) = (dF W2) * GELU'(hpre), the derivative saved by the forward as a 16-bit operand
       p.ld_mask = ff;
       p.mask_mul = 1;
       p.out16 = T.dhpre16;
       p.ld16 = ff;
-      p.out_fmt = FMT_G;
-      p.colsum = G_layer(l, 5);  // linear1.bias
+      p.colsum = grads[ix.layer(l, 5)];  // linear1.bias
       p.colsum_scale = INV;
       return r;
     };
     auto ffn2_wgrad = [&](GemmProblem& p, int bnn, int ks) -> int {
       int r = setup_gemm(p, Mat16{T.dbr16, M, d, d}, 1, Mat16{T.h16[l], M, ff, ff}, 1, d, ff, M, bnn);
-      p.a_fmt = FMT_G;
-      p.b_fmt = fmt;
-      p.out32 = G_layer(l, 6);  // linear2.weight [d, ff]
+      p.out32 = grads[ix.layer(l, 6)];  // linear2.weight [d, ff]
       p.ld32 = ff;
       p.alpha = INV;
       p.ksplit = ks;
@@ -458,8 +437,6 @@ int univtg_backward(univtg_plan* P, void* ws, const float* src_txt, const float*
     };
     auto ffn1_dgrad = [&](GemmProblem& p, int bnn) -> int {
       int r = setup_gemm(p, Mat16{T.dhpre16, M, ff, ff}, 0, Mat16{W16(lp.w1), ff, d, d}, 1, M, d, ff, bnn);
-      p.a_fmt = FMT_G;
-      p.b_fmt = fmt;
       p.resid = T.dy;
       p.ld_resid = d;
       p.out32 = T.dx;
@@ -468,122 +445,68 @@ int univtg_backward(univtg_plan* P, void* ws, const float* src_txt, const float*
     };
     auto ffn1_wgrad = [&](GemmProblem& p, int bnn, int ks) -> int {
       int r = setup_gemm(p, Mat16{T.dhpre16, M, ff, ff}, 1, Mat16{T.x1_16[l], M, d, d}, 1, ff, d, M, bnn);
-      p.a_fmt = FMT_G;
-      p.b_fmt = fmt;
-      p.out32 = G_layer(l, 4);  // linear1.weight [ff, d]
+      p.out32 = grads[ix.layer(l, 4)];  // linear1.weight [ff, d]
       p.ld32 = d;
       p.alpha = INV;
       p.ksplit = ks;
       return r;
     };
     {
-      memset(&g, 0, sizeof(g));
-      g.num = 1;
-      g.fmt = fmt;
+      reset_group(g, 1, fmt);
       rc = ffn2_dgrad(g.p[0], bn_dff);
       if (rc) return rc;
       rc = gemm_launch(P, g, bn_dff, sms, st);
       if (rc) return rc;
 
-      memset(&g, 0, sizeof(g));
-      g.num = 2;
-      g.fmt = fmt;
+      reset_group(g, 2, fmt);
       rc |= ffn2_wgrad(g.p[0], t_wf.bn, t_wf.ksplit);
       rc |= ffn1_wgrad(g.p[1], t_wf.bn, t_wf.ksplit);
       if (rc) return rc;
       rc = gemm_launch(P, g, t_wf.bn, sms, st);
       if (rc) return rc;
-      memset(&g, 0, sizeof(g));
-      g.num = 1;
-      g.fmt = fmt;
+      reset_group(g, 1, fmt);
       rc = ffn1_dgrad(g.p[0], bn_dd1);
       if (rc) return rc;
       rc = gemm_launch(P, g, bn_dd1, sms, st);
       if (rc) return rc;
     }
     // ---- LN1 backward ----
-    {
-      LnBwdArgs a;
-      memset(&a, 0, sizeof(a));
-      a.dout = T.dx;
-      a.ld_dout = d;
-      a.y = T.y1[l];
-      a.ld_y = d;
-      a.mean = T.mean1[l];
-      a.rstd = T.rstd1[l];
-      a.gamma = F32(lp.n1w);
-      a.rows = M;
-      a.d = d;
-      a.row_scale = s1;
-      a.L = L;
-      a.dy32 = T.dy;
-      a.dbr16 = T.dbr16;
-      a.ld16 = d;
-      a.fmt16 = FMT_G;
-      a.dgamma = G_layer(l, 8);
-      a.dbeta = G_layer(l, 9);
-      a.colsum = G_layer(l, 3);  // out_proj.bias
-      a.pgrad_scale = INV;
-      rc = launch_layernorm_bwd(a, st);
-      if (rc) return rc;
-    }
+    rc = ln_bwd(T.y1[l], T.mean1[l], T.rstd1[l], F32(lp.n1w), s1, grads[ix.layer(l, 8)], grads[ix.layer(l, 9)],
+                grads[ix.layer(l, 3)]);  // out_proj.bias
+    if (rc) return rc;
     // ---- out-proj: dgrad -> dO (16-bit); wgrad dWo = dA^T attn ----
     auto out_dgrad = [&](GemmProblem& p, int bnn) -> int {
       int r = setup_gemm(p, Mat16{T.dbr16, M, d, d}, 0, Mat16{W16(lp.w_out), d, d, d}, 1, M, d, d, bnn);
-      p.a_fmt = FMT_G;
-      p.b_fmt = fmt;
       p.out16 = T.dO16;
       p.ld16 = d;
-      p.out_fmt = FMT_G;
       return r;
     };
     auto out_wgrad = [&](GemmProblem& p, int bnn, int ks) -> int {
       int r = setup_gemm(p, Mat16{T.dbr16, M, d, d}, 1, Mat16{T.attn16[l], M, d, d}, 1, d, d, M, bnn);
-      p.a_fmt = FMT_G;
-      p.b_fmt = fmt;
-      p.out32 = G_layer(l, 2);
+      p.out32 = grads[ix.layer(l, 2)];
       p.ld32 = d;
       p.alpha = INV;
       p.ksplit = ks;
       return r;
     };
     {
-      memset(&g, 0, sizeof(g));
-      g.num = 1;
-      g.fmt = fmt;
+      reset_group(g, 1, fmt);
       rc = out_dgrad(g.p[0], bn_ddo);
       if (rc) return rc;
       rc = gemm_launch(P, g, bn_ddo, sms, st);
       if (rc) return rc;
-      memset(&g, 0, sizeof(g));
-      g.num = 1;
-      g.fmt = fmt;
-      rc = out_wgrad(g.p[0], bn_wo, t_wo.ksplit);
+      reset_group(g, 1, fmt);
+      rc = out_wgrad(g.p[0], t_wo.bn, t_wo.ksplit);
       if (rc) return rc;
-      rc = gemm_launch(P, g, bn_wo, sms, st);
+      rc = gemm_launch(P, g, t_wo.bn, sms, st);
       if (rc) return rc;
     }
     // ---- attention core backward -> dqkv32 -> dqkv16 (+ in_proj_bias gradient) ----
-    rc = launch_attn_delta(T.dO16, FMT_G, T.attn16[l], fmt, T.delta, B, L, P->H, P->dh, st);
+    rc = launch_attn_delta(T.dO16, fmt, T.attn16[l], fmt, T.delta, B, L, P->H, P->dh, st);
     if (rc) return rc;
     bool fused16 = false;
     {
-      AttnBwdArgs a;
-      memset(&a, 0, sizeof(a));
-      a.qkv = T.qkv16[l];
-      a.dO = T.dO16;
-      a.key_mask = T.key_mask;
-      a.lse = T.lse[l];
-      a.delta = T.delta;
-      a.dqkv32 = T.dqkv32;
-      a.scale = 1.0f / sqrtf((float)P->dh);
-      a.B = B;
-      a.L = L;
-      a.H = P->H;
-      a.dh = P->dh;
-      a.d = d;
-      a.fmt_act = fmt;
-      a.fmt_grad = FMT_G;
+      AttnBwdArgs a = attention_bwd_args(T.qkv16[l], T.dO16, T.key_mask, T.lse[l], T.delta, T.dqkv32, B, L, P->H, P->dh, fmt);
       if (P->attn_dropout > 0.f) a.drop = make_drop_spec(rng->seed, (unsigned int)l, P->attn_dropout);  // the forward's masks
       // one key tile on tensor cores: the kernel emits the 16-bit operands itself (the in_proj_bias column sums are a separate pass)
       int dq_mode = 2;
@@ -592,14 +515,12 @@ int univtg_backward(univtg_plan* P, void* ws, const float* src_txt, const float*
       fused16 = dq_mode == 0;
     }
     // (with text positions the same pass also copies the text rows of [dq | dk] into TP.dqk16)
-    if (!fused16) rc = launch_cvt16_colsum(T.dqkv32, 3 * d, T.dqkv16, 3 * d, M, 3 * d, FMT_G, G_layer(l, 1), INV, st, txt_rows);
-    else rc = launch_colsum16(T.dqkv16, 3 * d, M, 3 * d, FMT_G, G_layer(l, 1), INV, st, txt_rows);  // in_proj_bias gradient
+    if (!fused16) rc = launch_cvt16_colsum(T.dqkv32, 3 * d, T.dqkv16, 3 * d, M, 3 * d, fmt, grads[ix.layer(l, 1)], INV, st, txt_rows);
+    else rc = launch_colsum16(T.dqkv16, 3 * d, M, 3 * d, fmt, grads[ix.layer(l, 1)], INV, st, txt_rows);  // in_proj_bias gradient
     if (rc) return rc;
     // ---- in-projections: dgrad dx = dy + [dq|dk|dv] [Wq;Wk;Wv]; wgrad dWqk = [dq|dk]^T (x+pos), dWv = dv^T x ----
     auto qkv_dgrad = [&](GemmProblem& p, int bnn) -> int {
       int r = setup_gemm(p, Mat16{T.dqkv16, M, 3 * d, 3 * d}, 0, Mat16{W16(lp.w_in), 3 * d, d, d}, 1, M, d, 3 * d, bnn);
-      p.a_fmt = FMT_G;
-      p.b_fmt = fmt;
       p.resid = T.dy;
       p.ld_resid = d;
       p.out32 = T.dx;
@@ -609,29 +530,22 @@ int univtg_backward(univtg_plan* P, void* ws, const float* src_txt, const float*
     auto qkv_wgrads = [&](GemmProblem& pqk, GemmProblem& pv, int bnn, int ks) -> int {
       int r = setup_gemm(pqk, Mat16{T.dqkv16, M, 2 * d, 3 * d}, 1, Mat16{T.xpos16[l], M, d, d}, 1, 2 * d, d, M, bnn);
       r |= setup_gemm(pv, Mat16{T.dqkv16 + 2 * d, M, d, 3 * d}, 1, Mat16{T.xin16[l], M, d, d}, 1, d, d, M, bnn);
-      pqk.a_fmt = pv.a_fmt = FMT_G;
-      pqk.b_fmt = pv.b_fmt = fmt;
-      pqk.out32 = G_layer(l, 0);
+      pqk.out32 = grads[ix.layer(l, 0)];
       pqk.ld32 = d;
-      pv.out32 = G_layer(l, 0) + (size_t)2 * d * d;
+      pv.out32 = grads[ix.layer(l, 0)] + (size_t)2 * d * d;
       pv.ld32 = d;
       pqk.alpha = pv.alpha = INV;
       pqk.ksplit = pv.ksplit = ks;
       return r;
     };
     {
-      memset(&g, 0, sizeof(g));
-      g.num = 1;
-      g.fmt = fmt;
+      reset_group(g, txt_pos ? 2 : 1, fmt);
       rc = qkv_dgrad(g.p[0], bn_ddq);
       if (rc) return rc;
       if (txt_pos) {  // d(pos_t) += [dq | dk] [Wq; Wk] over the text rows (the first layer differentiated overwrites)
-        g.num = 2;
         GemmProblem& p = g.p[1];
         rc = setup_gemm(p, Mat16{TP.dqk16, Mt, 2 * d, 2 * d}, 0, Mat16{W16(lp.w_in), 2 * d, d, d}, 1, Mt, d, 2 * d, bn_ddq);
         if (rc) return rc;
-        p.a_fmt = FMT_G;
-        p.b_fmt = fmt;
         p.resid = l == c.enc_layers - 1 ? nullptr : TP.dpos;
         p.ld_resid = d;
         p.out32 = TP.dpos;
@@ -639,12 +553,10 @@ int univtg_backward(univtg_plan* P, void* ws, const float* src_txt, const float*
       }
       rc = gemm_launch(P, g, bn_ddq, sms, st);
       if (rc) return rc;
-      memset(&g, 0, sizeof(g));
-      g.num = 2;
-      g.fmt = fmt;
-      rc = qkv_wgrads(g.p[0], g.p[1], bn_wq, t_wq.ksplit);
+      reset_group(g, 2, fmt);
+      rc = qkv_wgrads(g.p[0], g.p[1], t_wq.bn, t_wq.ksplit);
       if (rc) return rc;
-      rc = gemm_launch(P, g, bn_wq, sms, st);
+      rc = gemm_launch(P, g, t_wq.bn, sms, st);
       if (rc) return rc;
     }
     stage_done(1 + (c.enc_layers - 1 - l));  // encoder layer l
@@ -652,7 +564,7 @@ int univtg_backward(univtg_plan* P, void* ws, const float* src_txt, const float*
 
   // ================================================ projectors ================================================
   if (txt_pos) {  // LayerNorm (+ dropout) backward of pos_t: its three parameter gradients, and du into the text rows of dx
-    const int base = univtg_num_params(&c);
+    const int base = ix.count();
     TxtPosBwdArgs a;
     memset(&a, 0, sizeof(a));
     a.dpos = TP.dpos;
@@ -679,54 +591,47 @@ int univtg_backward(univtg_plan* P, void* ws, const float* src_txt, const float*
   }
   // gradient w.r.t. the projected tokens = stream gradient rows + direct (saliency-loss) gradients (dxt_pool: written up front)
   // column sums = bias gradient of the last projector layer AND the token-type embedding rows
-  rc = launch_stream_gather(T.dx, L, 0, g_vid_mem_proj, GS, T.dxv16, G_type + d, INV, B, Lv, d, FMT_G, st);
+  float* const g_type = grads[ix.type()];
+  rc = launch_stream_gather(T.dx, L, 0, g_vid_mem_proj, GS, T.dxv16, g_type + d, INV, B, Lv, d, fmt, st);
   if (rc) return rc;
-  rc = launch_stream_gather(T.dx, L, Lv, g_txt_mem_proj ? T.dxt_pool : nullptr, 1.0f, T.dxt16, G_type, INV, B, Lt, d, FMT_G, st);
+  rc = launch_stream_gather(T.dx, L, Lv, g_txt_mem_proj ? T.dxt_pool : nullptr, 1.0f, T.dxt16, g_type, INV, B, Lt, d, fmt, st);
   if (rc) return rc;
-  cudaMemcpyAsync(G_vid(np - 1, 3), G_type + d, (size_t)d * 4, cudaMemcpyDeviceToDevice, st);
-  cudaMemcpyAsync(G_txt(np - 1, 3), G_type, (size_t)d * 4, cudaMemcpyDeviceToDevice, st);
+  cudaMemcpyAsync(grads[ix.vid(np - 1, 3)], g_type + d, (size_t)d * 4, cudaMemcpyDeviceToDevice, st);
+  cudaMemcpyAsync(grads[ix.txt(np - 1, 3)], g_type, (size_t)d * 4, cudaMemcpyDeviceToDevice, st);
   for (int i = np - 1; i >= 0; --i) {
     // wgrad: dW_i = dOut^T a_i   (video + text in one launch)
-    memset(&g, 0, sizeof(g));
-    g.num = 2;
-    g.fmt = fmt;
+    reset_group(g, 2, fmt);
     const int kpv = Lw.vid[i].kpad, kpt = Lw.txt[i].kpad, dinv = Lw.vid[i].din, dint = Lw.txt[i].din;
     // a width like 2818 would force scalar epilogue stores: write rows padded to kpad with 256-bit stores, then a pitched copy
     const bool pad_v = (dinv % 8) != 0;
     const int nv = pad_v ? kpv : dinv;  // the operand a_vid[i] is zero beyond dinv
     const TileChoice t_pw = tile_for(sms, 64, 16, MNK{d, nv, Mv}, MNK{d, dint, Mt});
-    const int bn = t_pw.bn;
     const int bn_pd = tile_for(sms, 64, 1, MNK{Mv, kpv, d}, MNK{Mt, kpt, d}).bn;
-    rc |= setup_gemm(g.p[0], Mat16{T.dxv16, Mv, d, d}, 1, Mat16{T.a_vid[i], Mv, kpv, kpv}, 1, d, nv, Mv, bn);
-    rc |= setup_gemm(g.p[1], Mat16{T.dxt16, Mt, d, d}, 1, Mat16{T.a_txt[i], Mt, kpt, kpt}, 1, d, dint, Mt, bn);
+    rc |= setup_gemm(g.p[0], Mat16{T.dxv16, Mv, d, d}, 1, Mat16{T.a_vid[i], Mv, kpv, kpv}, 1, d, nv, Mv, t_pw.bn);
+    rc |= setup_gemm(g.p[1], Mat16{T.dxt16, Mt, d, d}, 1, Mat16{T.a_txt[i], Mt, kpt, kpt}, 1, d, dint, Mt, t_pw.bn);
     if (rc) return rc;
-    g.p[0].a_fmt = g.p[1].a_fmt = FMT_G;
-    g.p[0].b_fmt = g.p[1].b_fmt = fmt;
-    g.p[0].out32 = pad_v ? T.wtap : G_vid(i, 2);
+    g.p[0].out32 = pad_v ? T.wtap : grads[ix.vid(i, 2)];
     g.p[0].ld32 = nv;
-    g.p[1].out32 = G_txt(i, 2);
+    g.p[1].out32 = grads[ix.txt(i, 2)];
     g.p[1].ld32 = dint;
     g.p[0].alpha = g.p[1].alpha = INV;
     g.p[0].ksplit = g.p[1].ksplit = t_pw.ksplit;
     if (pad_v && t_pw.ksplit > 1) cudaMemsetAsync(T.wtap, 0, (size_t)d * kpv * 4, st);  // split-K accumulates into the padded copy
-    rc = gemm_launch(P, g, bn, sms, st);
+    rc = gemm_launch(P, g, t_pw.bn, sms, st);
     if (rc) return rc;
     if (pad_v)
-      cudaMemcpy2DAsync(G_vid(i, 2), (size_t)dinv * 4, T.wtap, (size_t)kpv * 4, (size_t)dinv * 4, (size_t)d, cudaMemcpyDeviceToDevice, st);
+      cudaMemcpy2DAsync(grads[ix.vid(i, 2)], (size_t)dinv * 4, T.wtap, (size_t)kpv * 4, (size_t)dinv * 4, (size_t)d,
+                        cudaMemcpyDeviceToDevice, st);
     // every projector weight, the later layers' LayerNorm terms and all biases are final here; what follows only produces the
     // first layer's LayerNorm terms - the 11.5 MB video weight gradient need not wait for it to start its exchange
     if (i == 0) stage_done(c.enc_layers + 1);
     // dgrad: dA_i = dOut W_i  (fp32, [rows, kpad_i]: N is padded to the packed weight's K so the epilogue stays on its
     // 128-bit path even for the 2818-wide video features; the padded columns are zeros).  The input-dropout mask is applied
     // by the LayerNorm backward when it loads dA.
-    memset(&g, 0, sizeof(g));
-    g.num = 2;
-    g.fmt = fmt;
+    reset_group(g, 2, fmt);
     rc |= setup_gemm(g.p[0], Mat16{T.dxv16, Mv, d, d}, 0, Mat16{W16(Lw.vid[i].w16), d, kpv, kpv}, 1, Mv, kpv, d, bn_pd);
     rc |= setup_gemm(g.p[1], Mat16{T.dxt16, Mt, d, d}, 0, Mat16{W16(Lw.txt[i].w16), d, kpt, kpt}, 1, Mt, kpt, d, bn_pd);
     if (rc) return rc;
-    g.p[0].a_fmt = g.p[1].a_fmt = FMT_G;
-    g.p[0].b_fmt = g.p[1].b_fmt = fmt;
     g.p[0].out32 = T.dA_v;
     g.p[0].ld32 = kpv;
     g.p[1].out32 = T.dA_t;
@@ -753,15 +658,15 @@ int univtg_backward(univtg_plan* P, void* ws, const float* src_txt, const float*
       a.gamma = F32(pp.ln_w);
       a.rows = s == 0 ? Mv : Mt;
       a.d = pp.din;
-      a.dgamma = s == 0 ? G_vid(i, 0) : G_txt(i, 0);
-      a.dbeta = s == 0 ? G_vid(i, 1) : G_txt(i, 1);
+      a.dgamma = grads[s == 0 ? ix.vid(i, 0) : ix.txt(i, 0)];
+      a.dbeta = grads[s == 0 ? ix.vid(i, 1) : ix.txt(i, 1)];
       a.pgrad_scale = INV;
       if (i > 0) {
         a.relu_mask_y = 1;
         a.dbr16 = s == 0 ? T.dxv16 : T.dxt16;
         a.ld16 = d;
-        a.fmt16 = FMT_G;
-        a.colsum = s == 0 ? G_vid(i - 1, 3) : G_txt(i - 1, 3);
+        a.fmt16 = fmt;
+        a.colsum = grads[s == 0 ? ix.vid(i - 1, 3) : ix.txt(i - 1, 3)];
       }
       rc = launch_layernorm_bwd(a, st);
       if (rc) return rc;
@@ -778,30 +683,28 @@ int univtg_backward(univtg_plan* P, void* ws, const float* src_txt, const float*
 }
 
 int univtg_backward_stages(const univtg_config* cfg, int32_t* ranges, int32_t max_stages) {
-  const int n_params = univtg_num_params(cfg);
-  if (n_params < 0) return -1;
-  const int np = cfg->n_input_proj, nl = cfg->enc_layers;
+  if (univtg_num_params(cfg) < 0) return -1;
+  const ParamIndex ix(*cfg);
+  const int nl = cfg->enc_layers;
   const int n = nl + 3;
   if (ranges == nullptr) return n;
   if (max_stages < n) {
     set_error("univtg_backward_stages: need room for %d stages", n);
     return -1;
   }
-  const int hb = 8 * np + 1 + 12 * nl;
   auto put = [&](int k, int a0, int a1, int b0, int b1) {
     ranges[4 * k + 0] = a0;
     ranges[4 * k + 1] = a1;
     ranges[4 * k + 2] = b0;
     ranges[4 * k + 3] = b1;
   };
-  put(0, hb, hb + 13, 0, 0);  // span_embed + class_embed, weightedpool.weight
+  put(0, ix.span(0), ix.count(), 0, 0);  // span_embed + class_embed, weightedpool.weight
   for (int k = 0; k < nl; ++k) {
     const int l = nl - 1 - k;
-    put(1 + k, 8 * np + 1 + 12 * l, 8 * np + 1 + 12 * (l + 1), 0, 0);
+    put(1 + k, ix.layer(l, 0), ix.layer(l + 1, 0), 0, 0);
   }
-  // projector parameters are [ln.weight, ln.bias, W, b] per layer, video layers first, then text, then token_type_embeddings
-  put(nl + 1, 2, 4 * np, 4 * np + 2, 8 * np + 1);  // everything but the first layers' LayerNorm terms
-  put(nl + 2, 0, 2, 4 * np, 4 * np + 2);           // those (final only after the last LayerNorm backward)
+  put(nl + 1, ix.vid(0, 2), ix.txt(0, 0), ix.txt(0, 2), ix.type() + 1);  // everything but the first layers' LayerNorm terms
+  put(nl + 2, ix.vid(0, 0), ix.vid(0, 2), ix.txt(0, 0), ix.txt(0, 2));   // those (final only after the last LayerNorm backward)
   return n;
 }
 
@@ -865,26 +768,10 @@ int univtg_op_attention_bwd(const void* qkv, const void* dO, const void* O, cons
   }
   if (refuse_fmt2(fmt_act, "univtg_op_attention_bwd")) return 1;
   cudaStream_t st = (cudaStream_t)stream;
-  const int d = H * dh;
   int rc = launch_attn_delta(reinterpret_cast<const uint16_t*>(dO), fmt_act, reinterpret_cast<const uint16_t*>(O), fmt_act,
                              delta_ws, B, L, H, dh, st);
   if (rc) return rc;
-  AttnBwdArgs a;
-  memset(&a, 0, sizeof(a));
-  a.qkv = reinterpret_cast<const uint16_t*>(qkv);
-  a.dO = reinterpret_cast<const uint16_t*>(dO);
-  a.key_mask = key_mask;
-  a.lse = lse;
-  a.delta = delta_ws;
-  a.dqkv32 = dqkv32;
-  a.scale = 1.0f / sqrtf((float)dh);
-  a.B = B;
-  a.L = L;
-  a.H = H;
-  a.dh = dh;
-  a.d = d;
-  a.fmt_act = fmt_act;
-  a.fmt_grad = fmt_act;
+  AttnBwdArgs a = attention_bwd_args(qkv, dO, key_mask, lse, delta_ws, dqkv32, B, L, H, dh, fmt_act);
   return attention_bwd_route(a, impl == 0, nullptr, st, nullptr);
 }
 
@@ -921,22 +808,7 @@ int univtg_op_attention_bwd_full(const univtg_attn_bwd* q, const univtg_rng* rng
     const int max_L = attention_bwd_simt_max_L();
     UV_REQ(q->L <= max_L, "%s: SIMT backward stages 32 L bytes of shared memory: L %d exceeds %d", fn, q->L, max_L);
   }
-  AttnBwdArgs a;
-  memset(&a, 0, sizeof(a));
-  const int d = q->H * q->dh;
-  a.qkv = reinterpret_cast<const uint16_t*>(q->qkv);
-  a.dO = reinterpret_cast<const uint16_t*>(q->dO);
-  a.key_mask = q->key_mask;
-  a.lse = q->lse;
-  a.delta = q->delta;
-  a.dqkv32 = q->dqkv32;
-  a.scale = 1.0f / sqrtf((float)q->dh);
-  a.B = q->B;
-  a.L = q->L;
-  a.H = q->H;
-  a.dh = q->dh;
-  a.d = d;
-  a.fmt_act = a.fmt_grad = q->fmt;
+  AttnBwdArgs a = attention_bwd_args(q->qkv, q->dO, q->key_mask, q->lse, q->delta, q->dqkv32, q->B, q->L, q->H, q->dh, q->fmt);
   if (p > 0.f) a.drop = make_drop_spec(rng->seed, (unsigned int)layer, p);
   if (kernel_used) *kernel_used = -1;
   return attention_bwd_route(a, q->impl == 0, reinterpret_cast<uint16_t*>(q->dqkv16), (cudaStream_t)stream, dq_mode, kernel_used);
@@ -955,9 +827,7 @@ int univtg_op_gemm_group(univtg_gemm_problem* problems, int32_t num, int32_t fmt
   UV_REQ(bn >= 32 && bn <= 256 && bn % 16 == 0, "%s: bn %d (multiple of 16 in [32, 256])", fn, bn);
   UV_REQ(cluster == 1 || cluster == 2, "%s: cluster %d (1 or 2)", fn, cluster);
   GemmGroup g;
-  memset(&g, 0, sizeof(g));
-  g.num = num;
-  g.fmt = fmt;
+  reset_group(g, num, fmt);
   g.cluster = cluster;
   for (int i = 0; i < num; ++i) {
     const univtg_gemm_problem& q = problems[i];
@@ -985,25 +855,21 @@ int univtg_op_gemm_group(univtg_gemm_problem* problems, int32_t num, int32_t fmt
     UV_REQ(al_(q.out32, 4) && al_(q.out32_id, 4) && al_(q.resid, 4) && al_(q.addtab, 4) && al_(q.colsum, 4) && al_(q.out16, 2) &&
                al_(q.out16p, 2) && al_(q.mask16, 2) && al_(q.dact16, 2),
            "%s: problem %d: misaligned epilogue pointer", fn, i);
-    const int fg = q.a_fmt < 0 ? fmt : q.a_fmt, fw = q.b_fmt < 0 ? fmt : q.b_fmt;
     int rc = 0;
     if (q.conv == 1) {
       UV_REQ(!q.a_mn && q.b_mn && q.K % 64 == 0, "%s: problem %d: conv dgrad needs a_mn = 0, b_mn = 1 and K %% 64 == 0", fn, i);
       UV_REQ(q.ldb == 3 * q.N, "%s: problem %d: conv dgrad weight pitch ldb must be 3 N", fn, i);
-      rc = conv_dgrad_problem(p, q.M, reinterpret_cast<const uint16_t*>(q.a), q.lda, q.K, reinterpret_cast<const uint16_t*>(q.b), q.N, bn,
-                              fg, fw);
+      rc = conv_dgrad_problem(p, q.M, reinterpret_cast<const uint16_t*>(q.a), q.lda, q.K, reinterpret_cast<const uint16_t*>(q.b), q.N, bn);
     } else if (q.conv == 2) {
       UV_REQ(q.a_mn && q.b_mn && q.tap >= 0 && q.tap <= 2, "%s: problem %d: conv wgrad needs a_mn = b_mn = 1 and tap in 0..2", fn, i);
       rc = conv_wgrad_problem(p, q.K, reinterpret_cast<const uint16_t*>(q.a), q.lda, q.M, reinterpret_cast<const uint16_t*>(q.b), q.ldb,
-                              q.N, q.tap, bn, fg, fw);
+                              q.N, q.tap, bn);
     } else if (q.conv == 3) {
       UV_REQ(!q.a_mn && !q.b_mn && q.K % 192 == 0, "%s: problem %d: forward conv needs a_mn = b_mn = 0 and K = 3 Cin with Cin %% 64 == 0",
              fn, i);
       UV_REQ(q.lda >= q.K / 3 && q.ldb == q.K, "%s: problem %d: forward conv needs lda >= Cin and weight pitch ldb = K", fn, i);
       UV_REQ(cluster == 1, "%s: problem %d: forward conv runs without clusters", fn, i);
       rc = conv_fwd_problem(p, q.M, reinterpret_cast<const uint16_t*>(q.a), q.lda, q.K / 3, reinterpret_cast<const uint16_t*>(q.b), q.N, bn);
-      p.a_fmt = q.a_fmt;
-      p.b_fmt = q.b_fmt;
     } else {
       UV_REQ(q.conv == 0, "%s: problem %d: conv %d (0 plain, 1 dgrad, 2 wgrad, 3 forward)", fn, i, q.conv);
       const Mat16 A = q.a_mn ? Mat16{reinterpret_cast<const uint16_t*>(q.a), q.K, q.M, q.lda}
@@ -1012,10 +878,10 @@ int univtg_op_gemm_group(univtg_gemm_problem* problems, int32_t num, int32_t fmt
                               : Mat16{reinterpret_cast<const uint16_t*>(q.b), q.N, q.K, q.ldb};
       UV_REQ(A.ld >= A.cols && Bm.ld >= Bm.cols, "%s: problem %d: lda / ldb smaller than the operand's row length", fn, i);
       rc = setup_gemm(p, A, q.a_mn, Bm, q.b_mn, q.M, q.N, q.K, cluster == 2 && !q.b_mn ? bn / 2 : bn);
-      p.a_fmt = q.a_fmt;
-      p.b_fmt = q.b_fmt;
     }
     if (rc) return rc;
+    p.a_fmt = q.a_fmt;
+    p.b_fmt = q.b_fmt;
     p.ksplit = q.ksplit;
     p.out_fmt = q.out_fmt;
     p.bias = q.bias;
