@@ -134,6 +134,15 @@ int univtg_droppath_scales(const univtg_rng* rng, int32_t n_sites, int32_t batch
  * plan; 0 = off (default).  The masks come from rng->seed (Philox, csrc/philox.cuh); p > 0 with rng == NULL is an error.
  * The value in effect at univtg_backward must be the one its forward ran with.  univtg_forward never applies it. */
 int univtg_plan_set_attention_dropout(univtg_plan* plan, float p);
+/* Seed source of the train-mode randomness of the following univtg_forward_train / univtg_backward calls on this plan (input
+ * dropout, text-position dropout, attention dropout, DropPath): seed_dev = device uint64 read by every kernel that draws (once,
+ * at its start) in place of rng->seed; NULL (default) = rng->seed.  The other rng fields (rates) still come from rng.  A CUDA
+ * graph captured with a seed source draws new masks on every replay when univtg_rng_advance runs ahead of the step. */
+int univtg_plan_set_seed_source(univtg_plan* plan, const uint64_t* seed_dev);
+/* One-thread kernel: *counter_dev += 1; *seed_dev = univtg_rng_seed_at(base, *counter_dev) (splitmix64 sequence). */
+int univtg_rng_advance(uint64_t base, uint64_t* counter_dev, uint64_t* seed_dev, void* stream);
+/* HOST function: the k-th seed of the sequence of univtg_rng_advance (replay k of a graph with counter 0 before replay 1). */
+uint64_t univtg_rng_seed_at(uint64_t base, uint64_t k);
 /* The multipliers (0 or 1/(1-p)) the kernels apply in encoder layer `layer`: out [B, H, L, L] f32, row = query, column = key
  * (the reference's [B*H, L, L] layout).  Parity tests hand them to the oracle. */
 int univtg_attention_dropout_mask(const univtg_rng* rng, float p, int32_t layer, int32_t B, int32_t H, int32_t L,
@@ -422,6 +431,21 @@ int univtg_debug_choose_tile(const int32_t* Ms, const int32_t* Ns, const int32_t
 int univtg_adamw_step(float* params, float* grads, float* exp_avg, float* exp_avg_sq, size_t n, float lr, float beta1,
                       float beta2, float eps, float weight_decay, int32_t step, float max_grad_norm,
                       int32_t write_clipped_grads, float* scratch3, const univtg_config* cfg, void* packed, void* stream);
+/* univtg_adamw_step with the optimizer state in device memory, for CUDA-graph replay: lr_dev = device fp32 learning rate;
+ * step_dev = device int32 count of completed updates - this update runs at step *step_dev + 1 and writes that value back only
+ * when it was not skipped (scratch3[2] == 0); bc_table = device fp32 [table_len][2] holding (bc1, bc2_sqrt) of steps 1 ..
+ * table_len as univtg_adamw_bias_table writes them (steps past table_len reuse the last row: build it with
+ * univtg_adamw_bias_table_len rows, after which both terms are 1.0f for good).  With that table the update is bit-identical to
+ * univtg_adamw_step at the same step.  scratch3[3] is used as well (the staged step). */
+int univtg_adamw_step_dev(float* params, float* grads, float* exp_avg, float* exp_avg_sq, size_t n, const float* lr_dev,
+                          float beta1, float beta2, float eps, float weight_decay, int32_t* step_dev, float max_grad_norm,
+                          int32_t write_clipped_grads, float* scratch3, const univtg_config* cfg, void* packed,
+                          const float* bc_table, int32_t table_len, void* stream);
+/* HOST functions: rows t = 1 .. len of the bias-correction table, out_host [len][2] = ((float)(1 - beta1^t),
+ * (float)sqrt(1 - beta2^t)) in double precision (univtg_adamw_step's expressions); and the number of rows after which both
+ * terms stay 1.0f (0 with an error message for betas outside [0, 1) or a table longer than 2^26 rows). */
+int univtg_adamw_bias_table(float beta1, float beta2, int32_t len, float* out_host);
+int32_t univtg_adamw_bias_table_len(float beta1, float beta2);
 /* univtg_pack_weights restricted to the fp32 vectors and the two tiny last-conv tensors (everything that is not a 16-bit matrix). */
 int univtg_pack_vectors(const univtg_config* cfg, const float* const* params, int32_t n_params, void* packed, void* stream);
 

@@ -176,6 +176,14 @@ SIGNATURES = {
     "univtg_adamw_step": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, ctypes.c_size_t, c_float, c_float, c_float, c_float,
                                   c_float, c_int, c_float, c_int, c_void_p, ctypes.POINTER(Config), c_void_p, c_void_p]),
     "univtg_pack_vectors": (c_int, [ctypes.POINTER(Config), ctypes.POINTER(c_void_p), c_int, c_void_p, c_void_p]),
+    "univtg_adamw_step_dev": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, ctypes.c_size_t, c_void_p, c_float, c_float, c_float,
+                                      c_float, c_void_p, c_float, c_int, c_void_p, ctypes.POINTER(Config), c_void_p, c_void_p, c_int,
+                                      c_void_p]),
+    "univtg_adamw_bias_table": (c_int, [c_float, c_float, c_int, c_void_p]),
+    "univtg_adamw_bias_table_len": (c_int, [c_float, c_float]),
+    "univtg_plan_set_seed_source": (c_int, [c_void_p, c_void_p]),
+    "univtg_rng_advance": (c_int, [ctypes.c_uint64, c_void_p, c_void_p, c_void_p]),
+    "univtg_rng_seed_at": (ctypes.c_uint64, [ctypes.c_uint64, ctypes.c_uint64]),
     "univtg_plan_set_profiling": (c_int, [c_void_p, c_int]),
     "univtg_plan_set_input_format": (c_int, [c_void_p, c_int]),
     "univtg_plan_read_profile": (c_int, [c_void_p, c_void_p, c_void_p, c_int]),

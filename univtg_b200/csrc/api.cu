@@ -195,6 +195,58 @@ int univtg_adamw_step(float* params, float* grads, float* exp_avg, float* exp_av
                              write_clipped_grads, scratch3, &t, stream);
 }
 
+int univtg_adamw_step_dev(float* params, float* grads, float* exp_avg, float* exp_avg_sq, size_t n, const float* lr_dev,
+                          float beta1, float beta2, float eps, float weight_decay, int32_t* step_dev, float max_grad_norm,
+                          int32_t write_clipped_grads, float* scratch3, const univtg_config* cfg, void* packed,
+                          const float* bc_table, int32_t table_len, void* stream) {
+  const char* fn = "univtg_adamw_step_dev";
+  UV_REQ(params && grads && exp_avg && exp_avg_sq && scratch3, "%s: null params, grads, exp_avg, exp_avg_sq or scratch3", fn);
+  UV_REQ(lr_dev && step_dev && bc_table, "%s: null lr_dev, step_dev or bc_table", fn);
+  UV_REQ(n % 4 == 0, "%s: n %zu must be a multiple of 4", fn, n);
+  UV_REQ(table_len >= 1, "%s: table_len %d must be >= 1", fn, (int)table_len);
+  UV_REQ(al_(params, 16) && al_(grads, 16) && al_(exp_avg, 16) && al_(exp_avg_sq, 16), "%s: flat buffers must be 16-byte aligned", fn);
+  UV_REQ(al_(lr_dev, 4) && al_(step_dev, 4) && al_(bc_table, 4) && al_(scratch3, 4), "%s: misaligned lr_dev, step_dev, bc_table or scratch3", fn);
+  UV_REQ((cfg == nullptr) == (packed == nullptr), "%s: cfg and packed must both be given or both be NULL", fn);
+  uv::AdamDevState dev{lr_dev, step_dev, bc_table, table_len};
+  if (cfg == nullptr)
+    return uv::adamw_step_impl(params, grads, exp_avg, exp_avg_sq, n, 0.f, beta1, beta2, eps, weight_decay, 1, max_grad_norm,
+                               write_clipped_grads, scratch3, nullptr, stream, &dev);
+  if (!check_cfg(cfg) || refuse_split(*cfg, fn)) return 1;
+  PackSegTable t;
+  const int total = make_pack_segments(*cfg, packed, t);
+  if (total < 0) return 1;
+  UV_REQ((size_t)total <= n, "%s: flat buffer has %zu floats, the config's parameters need %d", fn, n, total);
+  return uv::adamw_step_impl(params, grads, exp_avg, exp_avg_sq, n, 0.f, beta1, beta2, eps, weight_decay, 1, max_grad_norm,
+                             write_clipped_grads, scratch3, &t, stream, &dev);
+}
+
+int univtg_adamw_bias_table(float beta1, float beta2, int32_t len, float* out_host) {
+  const char* fn = "univtg_adamw_bias_table";
+  UV_REQ(out_host != nullptr, "%s: null out_host", fn);
+  UV_REQ(len >= 1, "%s: len %d must be >= 1", fn, (int)len);
+  UV_REQ(beta1 >= 0.f && beta1 < 1.f && beta2 >= 0.f && beta2 < 1.f, "%s: betas (%g, %g) must be in [0, 1)", fn, (double)beta1,
+         (double)beta2);
+  for (int32_t t = 1; t <= len; ++t) uv::adamw_bias_row(beta1, beta2, t, out_host + 2 * (size_t)(t - 1), out_host + 2 * (size_t)(t - 1) + 1);
+  return 0;
+}
+
+int32_t univtg_adamw_bias_table_len(float beta1, float beta2) {
+  if (!(beta1 >= 0.f && beta1 < 1.f && beta2 >= 0.f && beta2 < 1.f)) {
+    set_error("univtg_adamw_bias_table_len: betas (%g, %g) must be in [0, 1)", (double)beta1, (double)beta2);
+    return 0;
+  }
+  // both terms are non-decreasing in t (pow of a base in [0, 1) falls, and the float rounding is monotone): the first t where
+  // both are 1.0f is where the table may end
+  for (int32_t t = 1; t <= (1 << 26); ++t) {
+    float b1, b2;
+    uv::adamw_bias_row(beta1, beta2, t, &b1, &b2);
+    if (b1 == 1.f && b2 == 1.f) return t;
+  }
+  set_error("univtg_adamw_bias_table_len: the bias corrections of betas (%g, %g) do not reach 1.0f within 2^26 steps", (double)beta1,
+            (double)beta2);
+  return 0;
+}
+
 }  // extern "C"
 
 extern "C" {
@@ -285,6 +337,13 @@ int univtg_plan_set_attention_dropout(univtg_plan* plan, float p) {
     return 1;
   }
   plan->attn_dropout = p;
+  return 0;
+}
+
+int univtg_plan_set_seed_source(univtg_plan* plan, const uint64_t* seed_dev) {
+  UV_REQ(plan != nullptr, "univtg_plan_set_seed_source: null plan");
+  UV_REQ(al_(seed_dev, 8), "univtg_plan_set_seed_source: seed_dev must be 8-byte aligned");
+  plan->seed_dev = reinterpret_cast<const unsigned long long*>(seed_dev);
   return 0;
 }
 
@@ -379,7 +438,8 @@ int run_forward(univtg_plan* P, const FwdBufs& W, const float* src_txt, const fl
   const TxtPosWs TP = P->txt_pos_on ? make_txt_pos_ws(c, P->shp, P->txt_pos.scratch) : TxtPosWs{};
   prof_begin(P, st);
   rc = launch_sine_pos(src_vid_mask, src_txt_mask, P->dim_t, W.pos, W.key_mask, P->B, Lv, Lt, d, st, dp_rng ? W.dp_scale : nullptr,
-                       W.dp_scale ? 2 * c.enc_layers : 0, rng ? rng->seed : 0ull, rng ? 1.0f - rng->droppath : 1.f);
+                       W.dp_scale ? 2 * c.enc_layers : 0, rng ? rng->seed : 0ull, rng ? 1.0f - rng->droppath : 1.f,
+                       rng ? P->seed_dev : nullptr);
   rc = marked(rc, 0);
   if (rc) return rc;
   if (dp_rng) droppath_scale = W.dp_scale;
@@ -407,7 +467,7 @@ int run_forward(univtg_plan* P, const FwdBufs& W, const float* src_txt, const fl
       a.out16 = s == 0 ? W.a_vid[i] : W.a_txt[i];
       a.ld16 = pp.kpad;
       a.mul32 = drop_masks ? drop_masks[s * c.n_input_proj + i] : nullptr;
-      if (drop_rng) a.drop = make_drop_spec(rng->seed, (unsigned int)(s * c.n_input_proj + i), rng->input_dropout);
+      if (drop_rng) a.drop = plan_drop_spec(P, rng, (unsigned int)(s * c.n_input_proj + i), rng->input_dropout);
       a.mean_out = s == 0 ? W.pmean_v[i] : W.pmean_t[i];
       a.rstd_out = s == 0 ? W.prstd_v[i] : W.prstd_t[i];
       rc = marked(launch_layernorm(a, st), 0);
@@ -459,7 +519,7 @@ int run_forward(univtg_plan* P, const FwdBufs& W, const float* src_txt, const fl
     if (training) {
       a.mul32 = P->txt_pos.drop_mul;
       if (!a.mul32 && rng != nullptr && rng->input_dropout > 0.f)
-        a.drop = make_drop_spec(rng->seed, (unsigned int)(2 * c.n_input_proj), rng->input_dropout);
+        a.drop = plan_drop_spec(P, rng, (unsigned int)(2 * c.n_input_proj), rng->input_dropout);
       a.mean_out = TP.mean;
       a.rstd_out = TP.rstd;
     }
@@ -508,7 +568,7 @@ int run_forward(univtg_plan* P, const FwdBufs& W, const float* src_txt, const fl
       a.fmt = fmt;
       a.split = split;
       a.lo_qkv = a.lo_out = ws_lo;
-      if (attn_rng) a.drop = make_drop_spec(rng->seed, (unsigned int)l, P->attn_dropout);
+      if (attn_rng) a.drop = plan_drop_spec(P, rng, (unsigned int)l, P->attn_dropout);
       if (P->dh == 64 || P->dh == 128) {
         if (make_tmap_op(&a.tm_qkv, W.qkv16[l], (uint64_t)M, (uint64_t)3 * d, (uint64_t)3 * d, 128, 64, ws_lo)) return 1;
         rc = launch_attention(a, st);

@@ -79,6 +79,7 @@ __device__ __forceinline__ void attention_tile(const AttnArgs& a) {
   __syncthreads();
   pdl_launch_dependents();
   pdl_wait();  // barriers are set up; from here on the kernel reads what the previous kernels wrote
+  const DropSpec drop = drop_resolve(a.drop);  // (the seed is read after the PDL wait: a preceding kernel may write it)
 
   auto load_kv = [&](int j) {
     const int s = j & 1;
@@ -131,13 +132,13 @@ __device__ __forceinline__ void attention_tile(const AttnArgs& a) {
       const unsigned int bh = (unsigned int)(b * a.H + h), i0 = (unsigned int)(q0 + wg * 64 + fr);
 #pragma unroll
       for (int kc = 0; kc < 8; ++kc) {
-        const uint4 rr = attn_drop_block(a.drop, bh, i0, (unsigned int)(j * 128 + 16 * kc + fc));
+        const uint4 rr = attn_drop_block(drop, bh, i0, (unsigned int)(j * 128 + 16 * kc + fc));
         const uint32_t w[4] = {rr.x, rr.y, rr.z, rr.w};
 #pragma unroll
         for (int q = 0; q < 4; ++q) {
           const uint32_t wq = w[2 * (q & 1) + (q >> 1)];  // row bit 3 = q & 1, key bit 3 = q >> 1
-          mb[kc >> 2] |= ((wq & 0xffffu) >= a.drop.thresh ? 1u : 0u) << (8 * (kc & 3) + 2 * q);
-          mb[kc >> 2] |= ((wq >> 16) >= a.drop.thresh ? 1u : 0u) << (8 * (kc & 3) + 2 * q + 1);
+          mb[kc >> 2] |= ((wq & 0xffffu) >= drop.thresh ? 1u : 0u) << (8 * (kc & 3) + 2 * q);
+          mb[kc >> 2] |= ((wq >> 16) >= drop.thresh ? 1u : 0u) << (8 * (kc & 3) + 2 * q + 1);
         }
       }
     }
@@ -180,7 +181,7 @@ __device__ __forceinline__ void attention_tile(const AttnArgs& a) {
         psum[r] += p0 + p1;
         if constexpr (DROP != 0) {
           const uint32_t bits = mb[kc >> 2] >> (8 * (kc & 3) + 2 * q);
-          pf[kc][q] = cvt16x2((bits & 1u) ? p0 * a.drop.scale : 0.f, (bits & 2u) ? p1 * a.drop.scale : 0.f, BF);
+          pf[kc][q] = cvt16x2((bits & 1u) ? p0 * drop.scale : 0.f, (bits & 2u) ? p1 * drop.scale : 0.f, BF);
         } else {
           pf[kc][q] = cvt16x2(p0, p1, BF);
         }
@@ -438,6 +439,7 @@ struct AttnSimtArgs {
 template <int DROP, bool SPLIT = false>
 __global__ void __launch_bounds__(128) attention_simt_kernel(const AttnSimtArgs a) {
   pdl_prologue();
+  const DropSpec drop = drop_resolve(a.drop);
   extern __shared__ float s_sc[];  // [4 warps][L]
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int gw = blockIdx.x * 4 + warp;
@@ -471,7 +473,7 @@ __global__ void __launch_bounds__(128) attention_simt_kernel(const AttnSimtArgs 
     const float p = expf(sc[j] - m_use);
     sum += p;
     float pm = p;
-    if constexpr (DROP != 0) pm = p * attn_drop_mul1(a.drop, (unsigned int)(b * a.H + h), (unsigned int)i, (unsigned int)j);
+    if constexpr (DROP != 0) pm = p * attn_drop_mul1(drop, (unsigned int)(b * a.H + h), (unsigned int)i, (unsigned int)j);
     if constexpr (SPLIT) sc[j] = ld16x3(cvt16(pm, 0), cvt16_lo(pm));
     else sc[j] = ld16(cvt16(pm, a.fmt), a.fmt);  // same operand rounding as the tensor-core path
   }
@@ -604,8 +606,9 @@ int launch_attention(const AttnArgs& a, cudaStream_t stream, int* kernel_used) {
 }
 
 // The attention-dropout multipliers of `spec` as dense [B, H, L, L] (parity tests; the kernels above never store them).
-__global__ void __launch_bounds__(256) attention_dropout_mask_kernel(const DropSpec spec, int L, size_t n, float* __restrict__ out) {
+__global__ void __launch_bounds__(256) attention_dropout_mask_kernel(const DropSpec spec_in, int L, size_t n, float* __restrict__ out) {
   pdl_prologue();
+  const DropSpec spec = drop_resolve(spec_in);
   for (size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x; idx < n; idx += (size_t)gridDim.x * blockDim.x) {
     const unsigned int j = (unsigned int)(idx % L), i = (unsigned int)((idx / L) % L), bh = (unsigned int)(idx / ((size_t)L * L));
     out[idx] = attn_drop_mul1(spec, bh, i, j);

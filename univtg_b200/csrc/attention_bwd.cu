@@ -66,6 +66,7 @@ __global__ void __launch_bounds__(256, 1) attention_bwd_wgmma_kernel(const __gri
   __syncthreads();
   pdl_launch_dependents();
   pdl_wait();  // setup done; everything below reads the previous kernels' outputs
+  const DropSpec drop = drop_resolve(a.drop);  // (the seed is read after the PDL wait: a preceding kernel may write it)
   if (threadIdx.x == 0) {
     mbar_arrive_expect_tx(kv_full, 2 * Cfg::kTile);
 #pragma unroll
@@ -119,14 +120,14 @@ __global__ void __launch_bounds__(256, 1) attention_bwd_wgmma_kernel(const __gri
         for (int cp = 0; cp < 4; ++cp) {
 #pragma unroll
           for (int e = 0; e < 2; ++e) {
-            const uint4 rr = attn_drop_block(a.drop, bh, (unsigned int)(i * 128 + hq * 64 + 16 * cp + fc + e), key0 & ~9u);
+            const uint4 rr = attn_drop_block(drop, bh, (unsigned int)(i * 128 + hq * 64 + 16 * cp + fc + e), key0 & ~9u);
             const uint32_t w[4] = {rr.x, rr.y, rr.z, rr.w};
 #pragma unroll
             for (int cq = 0; cq < 2; ++cq)
 #pragma unroll
               for (int r = 0; r < 2; ++r) {  // word 2 (query bit 3 = cq) + (key bit 3 = r), lane half = key bit 0
                 const uint32_t v = half ? (w[2 * cq + r] >> 16) : (w[2 * cq + r] & 0xffffu);
-                mb |= (v >= a.drop.thresh ? 1u : 0u) << (4 * (2 * cp + cq) + 2 * r + e);
+                mb |= (v >= drop.thresh ? 1u : 0u) << (4 * (2 * cp + cq) + 2 * r + e);
               }
           }
         }
@@ -166,8 +167,8 @@ __global__ void __launch_bounds__(256, 1) attention_bwd_wgmma_kernel(const __gri
             p[e] = exp2f(st[4 * c + 2 * r + e] * sc2 + kb2[r] - s_lse2[col]);
             if constexpr (DROP != 0) {
               const bool keep = (mb >> (4 * c + 2 * r + e)) & 1u;
-              d[e] = p[e] == 0.f ? 0.f : p[e] * ((keep ? dpt[4 * c + 2 * r + e] * a.drop.scale : 0.f) - s_dlt[col]) * a.scale;
-              p[e] = keep ? p[e] * a.drop.scale : 0.f;  // P o M feeds the dV product
+              d[e] = p[e] == 0.f ? 0.f : p[e] * ((keep ? dpt[4 * c + 2 * r + e] * drop.scale : 0.f) - s_dlt[col]) * a.scale;
+              p[e] = keep ? p[e] * drop.scale : 0.f;  // P o M feeds the dV product
             } else {
               d[e] = p[e] == 0.f ? 0.f : p[e] * (dpt[4 * c + 2 * r + e] - s_dlt[col]) * a.scale;
             }

@@ -17,6 +17,7 @@ namespace uv {
 template <int EPT>
 __global__ void __launch_bounds__(128) layernorm_bwd_kernel(const LnBwdArgs a) {
   pdl_prologue();
+  const DropSpec drop = drop_resolve(a.drop);
   __shared__ float s_red[2][4];
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   float acc_g[EPT], acc_b[EPT], acc_c[EPT];
@@ -38,7 +39,7 @@ __global__ void __launch_bounds__(128) layernorm_bwd_kernel(const LnBwdArgs a) {
       if (j < a.d) {
         float dj = dout[j];
         if (a.dout_mul) dj *= a.dout_mul[(size_t)row * a.d + j];
-        else if (a.drop.on) dj *= drop_mul1(a.drop, (unsigned int)row, (unsigned int)j);
+        else if (drop.on) dj *= drop_mul1(drop, (unsigned int)row, (unsigned int)j);
         xh[i] = (y[j] - mean) * rstd;
         g[i] = dj * a.gamma[j];
         acc_g[i] += dj * xh[i];
@@ -90,6 +91,7 @@ __global__ void __launch_bounds__(128) layernorm_bwd_kernel(const LnBwdArgs a) {
 template <int NV>
 __global__ void __launch_bounds__(128) layernorm_bwd_vec_kernel(const LnBwdArgs a) {
   pdl_prologue();
+  const DropSpec drop = drop_resolve(a.drop);
   __shared__ float s_red[2][4];
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   float4 acc_g[NV], acc_b[NV], acc_c[NV], gam[NV];
@@ -112,8 +114,8 @@ __global__ void __launch_bounds__(128) layernorm_bwd_vec_kernel(const LnBwdArgs 
         if (a.dout_mul) {
           const float4 m = __ldg(reinterpret_cast<const float4*>(a.dout_mul + (size_t)row * a.d + j));
           nd[i].x *= m.x, nd[i].y *= m.y, nd[i].z *= m.z, nd[i].w *= m.w;
-        } else if (a.drop.on) {
-          const float4 m = drop_mul4(a.drop, (unsigned int)row, (unsigned int)j);
+        } else if (drop.on) {
+          const float4 m = drop_mul4(drop, (unsigned int)row, (unsigned int)j);
           nd[i].x *= m.x, nd[i].y *= m.y, nd[i].z *= m.z, nd[i].w *= m.w;
         }
       }
@@ -202,6 +204,7 @@ __global__ void __launch_bounds__(128) layernorm_bwd_vec_kernel(const LnBwdArgs 
 template <int NV>
 __global__ void __launch_bounds__(256) layernorm_bwd_warp_kernel(const LnBwdArgs a) {
   pdl_prologue();
+  const DropSpec drop = drop_resolve(a.drop);
   extern __shared__ float s_part[];  // [8 warps][NV * 128] floats, reused for the three column accumulators
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   constexpr int D = NV * 128;
@@ -228,8 +231,8 @@ __global__ void __launch_bounds__(256) layernorm_bwd_warp_kernel(const LnBwdArgs
       if (a.dout_mul) {
         const float4 m = __ldg(reinterpret_cast<const float4*>(a.dout_mul + (size_t)row * D + j));
         g[i].x *= m.x, g[i].y *= m.y, g[i].z *= m.z, g[i].w *= m.w;
-      } else if (a.drop.on) {
-        const float4 m = drop_mul4(a.drop, (unsigned int)row, (unsigned int)j);
+      } else if (drop.on) {
+        const float4 m = drop_mul4(drop, (unsigned int)row, (unsigned int)j);
         g[i].x *= m.x, g[i].y *= m.y, g[i].z *= m.z, g[i].w *= m.w;
       }
       const float4 gam = __ldg(reinterpret_cast<const float4*>(a.gamma + j));
@@ -294,6 +297,7 @@ __global__ void __launch_bounds__(256) layernorm_bwd_warp_kernel(const LnBwdArgs
 constexpr int kLnParamRows = 16;  // all 2 x 16 loads of a thread are issued before the first use (the loop is fully unrolled)
 __global__ void __launch_bounds__(256) layernorm_bwd_params_kernel(const LnBwdArgs a) {
   pdl_prologue();
+  const DropSpec drop = drop_resolve(a.drop);
   const int jj = blockIdx.x * 256 + threadIdx.x;
   const bool in = jj < a.d;         // threads past the row end stay in the loop: the Philox words travel by warp shuffle
   const int j = in ? jj : a.d - 1;  // (their loads hit a valid column, their sums are dropped)
@@ -306,15 +310,15 @@ __global__ void __launch_bounds__(256) layernorm_bwd_params_kernel(const LnBwdAr
     if (r >= r1) break;  // warp-uniform
     float dj = __ldg(a.dout + (size_t)r * a.ld_dout + j);
     if (a.dout_mul) dj *= __ldg(a.dout_mul + (size_t)r * a.d + j);
-    else if (a.drop.on) {  // the eight threads of an aligned column group share ONE Philox call (thread = column here)
+    else if (drop.on) {  // the eight threads of an aligned column group share ONE Philox call (thread = column here)
       uint4 blk = make_uint4(0u, 0u, 0u, 0u);
-      if ((threadIdx.x & 7) == 0) blk = drop_block(a.drop, (unsigned int)r, (unsigned int)(jj >> 3));
+      if ((threadIdx.x & 7) == 0) blk = drop_block(drop, (unsigned int)r, (unsigned int)(jj >> 3));
       const int src = (threadIdx.x & 31) & ~7;
       blk.x = __shfl_sync(0xffffffffu, blk.x, src);
       blk.y = __shfl_sync(0xffffffffu, blk.y, src);
       blk.z = __shfl_sync(0xffffffffu, blk.z, src);
       blk.w = __shfl_sync(0xffffffffu, blk.w, src);
-      dj *= drop_pick(a.drop, blk, (unsigned int)(j & 7));
+      dj *= drop_pick(drop, blk, (unsigned int)(j & 7));
     }
     const float yv = a.y16 ? ld16(__ldg(a.y16 + (size_t)r * a.ld_y + j), a.y_fmt) : __ldg(a.y + (size_t)r * a.ld_y + j);
     const float xh = (yv - __ldg(a.mean + r)) * __ldg(a.rstd + r);
@@ -579,6 +583,7 @@ int launch_attn_delta(const uint16_t* dO, int fmt_do, const uint16_t* O, int fmt
 template <int DROP>
 __global__ void __launch_bounds__(128) attention_bwd_simt_kernel(const AttnBwdArgs a) {
   pdl_prologue();
+  const DropSpec drop = drop_resolve(a.drop);
   extern __shared__ float s_buf[];  // [4 warps][2][L]: p and ds
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int gw = blockIdx.x * 4 + warp;
@@ -605,7 +610,7 @@ __global__ void __launch_bounds__(128) attention_bwd_simt_kernel(const AttnBwdAr
       }
       p = expf(s * a.scale - lse);
       if constexpr (DROP != 0) {
-        const float m = attn_drop_mul1(a.drop, (unsigned int)(b * a.H + h), (unsigned int)i, (unsigned int)j);
+        const float m = attn_drop_mul1(drop, (unsigned int)(b * a.H + h), (unsigned int)i, (unsigned int)j);
         ds = p * (m * dp - dlt) * a.scale;
         p *= m;
       } else {
@@ -940,6 +945,7 @@ int launch_stream_gather(const float* dx_stream, int L, int off, const float* ex
 template <int EPT>
 __global__ void __launch_bounds__(128) txt_pos_bwd_kernel(const TxtPosBwdArgs a) {
   pdl_prologue();
+  const DropSpec drop = drop_resolve(a.drop);
   __shared__ float s_red[2][2][4];  // [parity of b][sum g, sum g * xhat][warp]
   const int l = blockIdx.x;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -964,7 +970,7 @@ __global__ void __launch_bounds__(128) txt_pos_bwd_kernel(const TxtPosBwdArgs a)
       if (j < a.d) {
         float go = a.dpos[r * a.d + j];
         if (a.mul32) go *= a.mul32[r * a.d + j];
-        else if (a.drop.on) go *= drop_mul1(a.drop, (unsigned int)r, (unsigned int)j);
+        else if (drop.on) go *= drop_mul1(drop, (unsigned int)r, (unsigned int)j);
         xh[i] = (a.xt[r * a.d + j] + pv[i] - mean) * rstd;
         acc_g[i] += go * xh[i];
         acc_b[i] += go;

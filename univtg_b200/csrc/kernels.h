@@ -158,9 +158,17 @@ struct PackSegTable {
   PackSeg s[kMaxPackSegs];
 };
 
+// device-resident optimizer state of univtg_adamw_step_dev (null: lr / step by value)
+struct AdamDevState {
+  const float* lr;         // device fp32 scalar
+  int32_t* step;           // device int32: completed updates; advanced by the kernel when the step is not skipped
+  const float* bc_table;   // device fp32 [table_len][2]: (bc1, bc2_sqrt) of steps 1 .. table_len (adamw_bias_row)
+  int32_t table_len;
+};
+void adamw_bias_row(float beta1, float beta2, int32_t step, float* bc1, float* bc2_sqrt);
 int adamw_step_impl(float* params, float* grads, float* exp_avg, float* exp_avg_sq, size_t n, float lr, float beta1, float beta2,
                     float eps, float weight_decay, int32_t step, float max_grad_norm, int32_t write_clipped_grads, float* scratch3,
-                    const PackSegTable* segs, void* stream);
+                    const PackSegTable* segs, void* stream, const AdamDevState* dev = nullptr);
 
 
 }  // namespace uv

@@ -16,11 +16,30 @@ namespace uv {
 
 struct DropSpec {
   unsigned long long seed;
+  const unsigned long long* seed_ptr;  // non-null: the seed lives in device memory (read once per kernel, see drop_resolve)
   unsigned int stream;  // which mask of the step (projector layer / modality)
   unsigned int thresh;  // element kept iff its 16-bit lane >= thresh (thresh = round(p * 65536))
   float scale;          // 1 / (1 - p)
   int on;               // 0: no dropout
 };
+
+// A captured CUDA graph replays its kernels with the arguments of the capture, so a seed passed by value would draw the same
+// masks on every replay.  With seed_ptr set the seed is read from device memory instead (written ahead of the step by
+// univtg_rng_advance): once per kernel, after the PDL wait, never inside the Philox loops.
+__device__ __forceinline__ unsigned long long drop_seed(const DropSpec& s) { return s.seed_ptr != nullptr ? *s.seed_ptr : s.seed; }
+__device__ __forceinline__ DropSpec drop_resolve(const DropSpec& s) {
+  DropSpec r = s;
+  if (s.on) r.seed = drop_seed(s);
+  return r;
+}
+__device__ __forceinline__ DropSpec drop_with_seed(const DropSpec& s, unsigned long long seed) {
+  DropSpec r = s;
+  r.seed = seed;
+  return r;
+}
+__device__ __forceinline__ unsigned long long dp_seed_of(unsigned long long seed, const unsigned long long* seed_ptr) {
+  return seed_ptr != nullptr ? *seed_ptr : seed;
+}
 
 __device__ __forceinline__ uint4 philox4x32_10(uint4 ctr, uint2 key) {
 #pragma unroll
@@ -98,9 +117,19 @@ __device__ __forceinline__ float attn_drop_mul1(const DropSpec& s, unsigned int 
   return attn_drop_lane(r, i, j) >= s.thresh ? s.scale : 0.f;
 }
 
+// Seed sequence of univtg_rng_advance / univtg_rng_seed_at: the k-th output of splitmix64 (Steele et al., OOPSLA'14) started at
+// `base`, so consecutive replays get well-separated Philox keys.
+__host__ __device__ __forceinline__ unsigned long long rng_seed_at(unsigned long long base, unsigned long long k) {
+  unsigned long long z = base + k * 0x9E3779B97F4A7C15ull;
+  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+  return z ^ (z >> 31);
+}
+
 inline DropSpec make_drop_spec(unsigned long long seed, unsigned int stream, float p) {
   DropSpec s;
   s.seed = seed;
+  s.seed_ptr = nullptr;
   s.stream = stream;
   s.on = p > 0.f ? 1 : 0;
   const float pc = p < 0.f ? 0.f : (p > 0.999f ? 0.999f : p);

@@ -359,6 +359,9 @@ struct univtg_plan {
   int in_fmt;       // src_vid / src_txt element type: 0 f32 (reference collate), 1 fp16, 2 bf16 (packed feature shards)
   int num_sms_bwd;  // SM budget of the backward's GEMM launches (0: num_sms); see univtg_plan_set_backward_sm_budget
   float attn_dropout;  // p of the attention dropout of univtg_forward_train / univtg_backward (0: off); univtg_forward ignores it
+  // device seed of the train-mode randomness (univtg_plan_set_seed_source; null: rng->seed).  Kernels read it at their start, so a
+  // CUDA graph captured with it set draws the masks of whatever seed univtg_rng_advance wrote ahead of each replay.
+  const unsigned long long* seed_dev = nullptr;
   int txt_pos_on;           // learned text positions (univtg_plan_set_txt_pos); 0: off
   long long pk_lo, ws_lo;   // fp16x3: elements from a 16-bit weight / workspace buffer to its lo plane (0: one plane)
   univtg_txt_pos txt_pos;
@@ -377,6 +380,13 @@ struct univtg_plan {
 };
 
 namespace {
+// dropout spec of the forward / backward of plan P: rng->seed, or the plan's device seed when one is set
+inline uv::DropSpec plan_drop_spec(const univtg_plan* P, const univtg_rng* rng, unsigned int stream, float p) {
+  uv::DropSpec s = uv::make_drop_spec(rng->seed, stream, p);
+  s.seed_ptr = P->seed_dev;
+  return s;
+}
+
 inline void prof_begin(univtg_plan* P, cudaStream_t st) {
   if (!P->profiling) return;
   P->n_marks = 0;

@@ -23,10 +23,11 @@ namespace uv {
 template <bool TXT = false, bool SPLIT = false>
 struct LnStore {
   const LnArgs& a;
+  const unsigned long long seed;  // a.drop's seed, resolved once per row (drop_seed); only the seed is held, not a spec copy
   int row, b, l;
   bool has_pos;
   size_t prow, crow, trow;
-  __device__ LnStore(const LnArgs& a_, int row_) : a(a_), row(row_) {
+  __device__ LnStore(const LnArgs& a_, int row_) : a(a_), seed(a_.drop.on ? drop_seed(a_.drop) : 0ull), row(row_) {
     b = 0;
     l = row;
     if (a.L > 0) {
@@ -44,7 +45,7 @@ struct LnStore {
       const float4 m = *reinterpret_cast<const float4*>(a.mul32 + (size_t)row * a.d + j);
       v.x *= m.x; v.y *= m.y; v.z *= m.z; v.w *= m.w;
     } else if (a.drop.on) {
-      const float4 m = drop_mul4(a.drop, (unsigned int)row, (unsigned int)j);
+      const float4 m = drop_mul4(drop_with_seed(a.drop, seed), (unsigned int)row, (unsigned int)j);
       v.x *= m.x; v.y *= m.y; v.z *= m.z; v.w *= m.w;
     }
     uint2 pk, pkl = make_uint2(0u, 0u);
@@ -82,7 +83,7 @@ struct LnStore {
   __device__ __forceinline__ void store1(int j, float v) const {
     if (a.out32) a.out32[(size_t)row * a.d + j] = v;
     if (a.mul32) v *= a.mul32[(size_t)row * a.d + j];
-    else if (a.drop.on) v *= drop_mul1(a.drop, (unsigned int)row, (unsigned int)j);
+    else if (a.drop.on) v *= drop_mul1(drop_with_seed(a.drop, seed), (unsigned int)row, (unsigned int)j);
     if constexpr (SPLIT) {
       const uint16_t h = cvt16(v, a.fmt), hl = cvt16_lo(v);
       if (a.out16) {
@@ -282,6 +283,7 @@ __global__ void __launch_bounds__(128) layernorm_rows_block_kernel(const LnArgs 
 template <int EPT2, bool SPLIT = false>
 __global__ void __launch_bounds__(128) layernorm_rows_block2_kernel(const LnArgs a) {
   pdl_prologue();
+  const DropSpec drop = drop_resolve(a.drop);
   __shared__ float s_red[4];
   __shared__ float s_stat[2];
   const int row = blockIdx.x;
@@ -334,8 +336,8 @@ __global__ void __launch_bounds__(128) layernorm_rows_block2_kernel(const LnArgs
   for (int st = 0; st < STEPS; ++st) {
     const int j0 = 8 * (tid + 128 * st);
     float m8[8];
-    const bool rnd = a.mul32 == nullptr && a.drop.on && j0 < a.d;
-    if (rnd) drop_mul8(a.drop, (unsigned int)row, (unsigned int)(j0 >> 3), m8);
+    const bool rnd = a.mul32 == nullptr && drop.on && j0 < a.d;
+    if (rnd) drop_mul8(drop, (unsigned int)row, (unsigned int)(j0 >> 3), m8);
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
       const int i = st * 4 + k, j = j0 + 2 * k;
@@ -437,6 +439,7 @@ constexpr int kTxtPosMaxPairs = 16;  // d <= 64 * 16
 template <bool SPLIT = false>
 __global__ void __launch_bounds__(256) txt_pos_rows_kernel(const TxtPosArgs a) {
   pdl_prologue();
+  const DropSpec drop = drop_resolve(a.drop);
   const int row = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   if (row >= a.B * a.Lt) return;
@@ -483,9 +486,9 @@ __global__ void __launch_bounds__(256) txt_pos_rows_kernel(const TxtPosArgs a) {
         const float2 m = *reinterpret_cast<const float2*>(a.mul32 + (size_t)row * a.d + j);
         ox *= m.x;
         oy *= m.y;
-      } else if (a.drop.on) {
-        ox *= drop_mul1(a.drop, (unsigned int)row, (unsigned int)j);
-        oy *= drop_mul1(a.drop, (unsigned int)row, (unsigned int)(j + 1));
+      } else if (drop.on) {
+        ox *= drop_mul1(drop, (unsigned int)row, (unsigned int)j);
+        oy *= drop_mul1(drop, (unsigned int)row, (unsigned int)(j + 1));
       }
       *reinterpret_cast<float2*>(a.pos + (size_t)row * a.d + j) = make_float2(ox, oy);
       const float2 xv = *reinterpret_cast<const float2*>(x + j);
@@ -516,10 +519,13 @@ int launch_txt_pos(const TxtPosArgs& a, cudaStream_t stream) {
 __global__ void __launch_bounds__(256) sine_pos_table_kernel(const float* __restrict__ mask, const float* __restrict__ txt_mask,
                                                             const float* __restrict__ dim_t, float* __restrict__ pos,
                                                             float* __restrict__ key_mask, int Lv, int Lt, int d,
-                                                            float* __restrict__ dp_out, int dp_n, unsigned long long dp_seed, float dp_keep) {
+                                                            float* __restrict__ dp_out, int dp_n, unsigned long long dp_seed,
+                                                            const unsigned long long* __restrict__ dp_seed_ptr, float dp_keep) {
   pdl_prologue();
-  if (dp_out != nullptr && blockIdx.x == 0 && blockIdx.y == 0)  // DropPath scales of this step ([sites, B], a few hundred values)
-    for (int i = threadIdx.x; i < dp_n; i += 256) dp_out[i] = droppath_scale(dp_seed, (unsigned int)i, dp_keep);
+  if (dp_out != nullptr && blockIdx.x == 0 && blockIdx.y == 0) {  // DropPath scales of this step ([sites, B], a few hundred values)
+    const unsigned long long seed = dp_seed_of(dp_seed, dp_seed_ptr);
+    for (int i = threadIdx.x; i < dp_n; i += 256) dp_out[i] = droppath_scale(seed, (unsigned int)i, dp_keep);
+  }
   extern __shared__ float s_e[];  // [Lv] cumulative position, then the normalised angle
   __shared__ float s_part[256];
   const int b = blockIdx.x;
@@ -571,25 +577,44 @@ __global__ void __launch_bounds__(256) sine_pos_table_kernel(const float* __rest
 }
 
 int launch_sine_pos(const float* mask, const float* txt_mask, const float* dim_t, float* pos, float* key_mask, int B, int Lv,
-                    int Lt, int d, cudaStream_t stream, float* dp_out, int dp_sites, unsigned long long dp_seed, float dp_keep) {
+                    int Lt, int d, cudaStream_t stream, float* dp_out, int dp_sites, unsigned long long dp_seed, float dp_keep,
+                    const unsigned long long* dp_seed_ptr) {
   int chunks = (Lv * d + 4095) / 4096;
   if (chunks < 1) chunks = 1;
   if (chunks > 128) chunks = 128;
   launch_k(sine_pos_table_kernel, dim3(dim3(B, chunks)), dim3(256), Lv * sizeof(float), stream, mask, txt_mask, dim_t, pos, key_mask, Lv, Lt, d,
-           dp_out, dp_sites * B, dp_seed, dp_keep);
+           dp_out, dp_sites * B, dp_seed, dp_seed_ptr, dp_keep);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) set_error("sine_pos launch failed: %s", cudaGetErrorString(e));
   return (int)e;
 }
 
-__global__ void __launch_bounds__(256) dropout_mask_kernel(const DropSpec spec, size_t n, size_t cols, float* __restrict__ out) {
+__global__ void __launch_bounds__(256) dropout_mask_kernel(const DropSpec spec_in, size_t n, size_t cols, float* __restrict__ out) {
   pdl_prologue();
+  const DropSpec spec = drop_resolve(spec_in);
   for (size_t i = (size_t)blockIdx.x * 256 + threadIdx.x; i < n; i += (size_t)gridDim.x * 256)
     out[i] = spec.on ? drop_mul1(spec, (unsigned int)(i / cols), (unsigned int)(i % cols)) : 1.f;
 }
-__global__ void __launch_bounds__(256) droppath_scales_kernel(unsigned long long seed, int n, float keep, float* __restrict__ out) {
+__global__ void __launch_bounds__(256) droppath_scales_kernel(unsigned long long seed_in, const unsigned long long* __restrict__ seed_ptr,
+                                                             int n, float keep, float* __restrict__ out) {
   pdl_prologue();
+  const unsigned long long seed = dp_seed_of(seed_in, seed_ptr);
   for (int i = blockIdx.x * 256 + threadIdx.x; i < n; i += gridDim.x * 256) out[i] = droppath_scale(seed, (unsigned int)i, keep);
+}
+__global__ void __launch_bounds__(32) rng_advance_kernel(unsigned long long base, unsigned long long* __restrict__ counter,
+                                                         unsigned long long* __restrict__ seed) {
+  pdl_prologue();
+  if (threadIdx.x == 0) {
+    const unsigned long long k = *counter + 1ull;
+    *counter = k;
+    *seed = rng_seed_at(base, k);
+  }
+}
+int launch_rng_advance(unsigned long long base, unsigned long long* counter, unsigned long long* seed, cudaStream_t stream) {
+  launch_k(rng_advance_kernel, dim3(1), dim3(32), 0, stream, base, counter, seed);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) set_error("rng_advance launch failed: %s", cudaGetErrorString(e));
+  return (int)e;
 }
 int launch_dropout_mask(const DropSpec& spec, size_t n, size_t cols, float* out, cudaStream_t stream) {
   if (n == 0) return 0;
@@ -600,9 +625,9 @@ int launch_dropout_mask(const DropSpec& spec, size_t n, size_t cols, float* out,
   if (e != cudaSuccess) set_error("dropout_mask launch failed: %s", cudaGetErrorString(e));
   return (int)e;
 }
-int launch_droppath_scales(unsigned long long seed, int n, float keep, float* out, cudaStream_t stream) {
+int launch_droppath_scales(unsigned long long seed, int n, float keep, float* out, cudaStream_t stream, const unsigned long long* seed_ptr) {
   if (n <= 0) return 0;
-  launch_k(droppath_scales_kernel, dim3((n + 255) / 256), dim3(256), 0, stream, seed, n, keep, out);
+  launch_k(droppath_scales_kernel, dim3((n + 255) / 256), dim3(256), 0, stream, seed, seed_ptr, n, keep, out);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) set_error("droppath_scales launch failed: %s", cudaGetErrorString(e));
   return (int)e;

@@ -68,10 +68,13 @@ int launch_txt_pos(const TxtPosArgs& a, cudaStream_t stream);
 // dp_out (optional): [dp_sites, B] DropPath scales floor(keep + u) / keep drawn in-kernel from (dp_seed, site * B + b)
 int launch_sine_pos(const float* mask, const float* txt_mask, const float* dim_t, float* pos, float* key_mask, int B, int Lv,
                     int Lt, int d, cudaStream_t stream, float* dp_out = nullptr, int dp_sites = 0, unsigned long long dp_seed = 0,
-                    float dp_keep = 1.f);
+                    float dp_keep = 1.f, const unsigned long long* dp_seed_ptr = nullptr);  // dp_seed_ptr: device seed (null: dp_seed)
 // standalone generators (parity tests read the in-kernel draws back through them)
 int launch_dropout_mask(const DropSpec& spec, size_t n, size_t cols, float* out, cudaStream_t stream);  // [n / cols, cols] row-major
-int launch_droppath_scales(unsigned long long seed, int n, float keep, float* out, cudaStream_t stream);
+int launch_droppath_scales(unsigned long long seed, int n, float keep, float* out, cudaStream_t stream,
+                           const unsigned long long* seed_ptr = nullptr);
+// *counter += 1; *seed = rng_seed_at(base, *counter)  (one thread; the head of a captured train step)
+int launch_rng_advance(unsigned long long base, unsigned long long* counter, unsigned long long* seed, cudaStream_t stream);
 
 struct PoolSalArgs {
   const float* x_txt;     // [B, Lt, d] projected text tokens (incl. token-type embedding)

@@ -507,7 +507,7 @@ int univtg_backward(univtg_plan* P, void* ws, const float* src_txt, const float*
     bool fused16 = false;
     {
       AttnBwdArgs a = attention_bwd_args(T.qkv16[l], T.dO16, T.key_mask, T.lse[l], T.delta, T.dqkv32, B, L, P->H, P->dh, fmt);
-      if (P->attn_dropout > 0.f) a.drop = make_drop_spec(rng->seed, (unsigned int)l, P->attn_dropout);  // the forward's masks
+      if (P->attn_dropout > 0.f) a.drop = plan_drop_spec(P, rng, (unsigned int)l, P->attn_dropout);  // the forward's masks
       // one key tile on tensor cores: the kernel emits the 16-bit operands itself (the in_proj_bias column sums are a separate pass)
       int dq_mode = 2;
       rc = attention_bwd_route(a, P->dh == 64 || P->dh == 128, T.dqkv16, st, &dq_mode, nullptr, P);
@@ -575,7 +575,7 @@ int univtg_backward(univtg_plan* P, void* ws, const float* src_txt, const float*
     a.rstd = TP.rstd;
     a.mul32 = P->txt_pos.drop_mul;
     if (!a.mul32 && rng != nullptr && rng->input_dropout > 0.f)
-      a.drop = make_drop_spec(rng->seed, (unsigned int)(2 * np), rng->input_dropout);
+      a.drop = plan_drop_spec(P, rng, (unsigned int)(2 * np), rng->input_dropout);
     a.dx = T.dx;
     a.dtable = grads[base];
     a.dgamma = grads[base + 1];
@@ -646,7 +646,7 @@ int univtg_backward(univtg_plan* P, void* ws, const float* src_txt, const float*
       a.dout = s == 0 ? T.dA_v : T.dA_t;
       a.ld_dout = pp.kpad;
       a.dout_mul = drop_masks ? drop_masks[s * np + i] : nullptr;
-      if (drop_rng) a.drop = make_drop_spec(rng->seed, (unsigned int)(s * np + i), rng->input_dropout);
+      if (drop_rng) a.drop = plan_drop_spec(P, rng, (unsigned int)(s * np + i), rng->input_dropout);
       a.y = i == 0 ? (s == 0 ? src_vid : src_txt) : (s == 0 ? T.p_vid32[i - 1] : T.p_txt32[i - 1]);
       if (i == 0 && P->in_fmt != 0) {
         a.y16 = reinterpret_cast<const uint16_t*>(a.y);
@@ -1123,7 +1123,6 @@ int univtg_op_txt_pos_bwd(const univtg_txt_pos_bwd* q, const univtg_rng* rng, in
   a.d = q->d;
   return launch_txt_pos_bwd(a, (cudaStream_t)stream);
 }
-#undef UV_REQ
 
 int univtg_dropout_mask(const univtg_rng* rng, int32_t mask_index, size_t rows, size_t cols, float* out, void* stream) {
   if (!rng || !out || mask_index < 0 || cols == 0) {
@@ -1141,6 +1140,17 @@ int univtg_attention_dropout_mask(const univtg_rng* rng, float p, int32_t layer,
     return 1;
   }
   return launch_attention_dropout_mask(make_drop_spec(rng->seed, (unsigned int)layer, p), B, H, L, out, (cudaStream_t)stream);
+}
+
+uint64_t univtg_rng_seed_at(uint64_t base, uint64_t k) { return (uint64_t)rng_seed_at(base, k); }
+
+int univtg_rng_advance(uint64_t base, uint64_t* counter_dev, uint64_t* seed_dev, void* stream) {
+  const char* fn = "univtg_rng_advance";
+  UV_REQ(counter_dev && seed_dev, "%s: null counter_dev or seed_dev", fn);
+  UV_REQ(al_(counter_dev, 8) && al_(seed_dev, 8), "%s: counter_dev and seed_dev must be 8-byte aligned", fn);
+  UV_REQ(counter_dev != seed_dev, "%s: counter_dev and seed_dev must be distinct", fn);
+  return launch_rng_advance(base, reinterpret_cast<unsigned long long*>(counter_dev), reinterpret_cast<unsigned long long*>(seed_dev),
+                            (cudaStream_t)stream);
 }
 
 int univtg_droppath_scales(const univtg_rng* rng, int32_t n_sites, int32_t batch, float* out, void* stream) {
@@ -1338,3 +1348,5 @@ int univtg_qfvs_loss_backward(const float* w5, const float* vid_mem_proj, const 
 }
 
 }  // extern "C"
+
+#undef UV_REQ

@@ -45,7 +45,9 @@ class FlatAdamW(torch.optim.Optimizer):
         self.dynamic_loss_scale = bool(dynamic_loss_scale) and model.operand_format == 0
         self.growth_interval, self.max_loss_scale = int(growth_interval), float(max_loss_scale)
         self.skipped_steps, self._good_streak = 0, 0
-        self._flag_host, self._flag_event = None, None
+        self._flag_host, self._flag_event = None, None  # the flag the next step consumes (this optimizer's or a graph replay's)
+        self._flag_buf = self._flag_evt = None            # this optimizer's own pinned flag and event
+        self._layout_version = 0  # bumped when the flat buffers are re-seated or the state is replaced (captured graphs bake them)
         self._flat_p = None
         self._views = None
         self._m = self._v = self._scratch = None
@@ -103,6 +105,7 @@ class FlatAdamW(torch.optim.Optimizer):
                 off += (n + 3) // 4 * 4
         keep = self._m is not None and self._m.numel() == flat_p.numel() and self._m.device == flat_p.device
         self._flat_p, self._views = flat_p, views
+        self._layout_version = getattr(self, "_layout_version", 0) + 1
         if not keep:
             self._m = torch.zeros_like(flat_p)
             self._v = torch.zeros_like(flat_p)
@@ -117,6 +120,7 @@ class FlatAdamW(torch.optim.Optimizer):
         """The next backward writes the flat gradient buffer from scratch (it zero-fills it itself); without a zero_grad() in
         between, further backwards accumulate into it like torch's .grad (univtg_b200/autograd.py)."""
         self.model.__dict__["_flat_grad_dirty"] = False
+        self.model.__dict__["_flat_grad_unstepped"] = False
         return None  # (with zero_grad_after_step the buffer is already being cleared; the backward waits for that fill)
 
     @torch.no_grad()
@@ -131,6 +135,7 @@ class FlatAdamW(torch.optim.Optimizer):
         lib = _lib.load_library()
         self._consume_overflow_flag()
         self.step_count += 1
+        model.__dict__["_flat_grad_unstepped"] = False
         with torch.cuda.device(flat_g.device):
             # The update kernel also refreshes the 16-bit GEMM operand copies of the weight matrices it has just computed (the
             # packed buffer of the training format), so the next forward needs no re-packing pass over the 43 M fp32 weights;
@@ -166,11 +171,12 @@ class FlatAdamW(torch.optim.Optimizer):
                 model.__dict__["_flat_grad_prezeroed"] = (flat_g.data_ptr(), self._zero_event)
                 model.__dict__["_flat_grad_dirty"] = False
             if self.dynamic_loss_scale:
-                if self._flag_host is None:
-                    self._flag_host = torch.zeros(1, dtype=torch.float32).pin_memory()
-                    self._flag_event = torch.cuda.Event()
-                self._flag_host.copy_(self._scratch[2:3], non_blocking=True)
-                self._flag_event.record()
+                if self._flag_buf is None:
+                    self._flag_buf = torch.zeros(1, dtype=torch.float32).pin_memory()
+                    self._flag_evt = torch.cuda.Event()
+                self._flag_buf.copy_(self._scratch[2:3], non_blocking=True)
+                self._flag_evt.record()
+                self._flag_host, self._flag_event = self._flag_buf, self._flag_evt
         return self._scratch[1]
 
     def _consume_overflow_flag(self):
@@ -259,3 +265,4 @@ class FlatAdamW(torch.optim.Optimizer):
             self.skipped_steps = int(ls.get("skipped_steps", 0))
             self.max_grad_norm = float(ls.get("max_grad_norm", self.max_grad_norm))
         self._flag_event = None  # a pending overflow flag belongs to the state that was just replaced
+        self._layout_version += 1

@@ -349,6 +349,9 @@ class Model(nn.Module):
         """Check a training workspace out of the pool (univtg_b200.plugin._WorkspaceLease).  Buffers are sized for the largest
         shape seen so far and shared between shapes; a buffer that last served another shape gets its zero rows re-established
         (univtg_prepare_workspace) - no per-shape allocation and no full-buffer memset in steady state."""
+        pinned = self.__dict__.get("_graph_train_ws")
+        if pinned is not None:  # a CUDA-graph capture (univtg_b200.graphs): the graphs' own buffer, prepared by their owner
+            return _WorkspaceLease([], pinned, plan)
         lib = _lib.load_library()
         dev = self._device()
         nbytes = lib.univtg_train_workspace_bytes(ctypes.byref(self._cfg), ctypes.byref(plan.shape))
