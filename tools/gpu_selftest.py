@@ -73,6 +73,14 @@ def case_gemm_timeline(M, N, K, act, want32, want16, bn, cluster=False, a_mn=0, 
     def run():
         _lib.check(fn(_lib.ptr(A), _lib.ptr(Bm), M, N, K, a_mn, b_mn, 0, bn, 1, _lib.ptr(bias), act, 1.0, _lib.ptr(out32),
                       _lib.ptr(out16), _lib.stream_ptr()), "op_gemm")
+    return _timeline(run, sms, buf)
+
+
+def _timeline(run, sms, buf):
+    """Warm up, then record the per-CTA %globaltimer stamps of one launch (stamps of a CTA's last tile) and its event time."""
+    import torch
+    from univtg_b200 import _lib
+    lib = _lib.load_library()
     for _ in range(3):
         run()
     torch.cuda.synchronize()
@@ -86,14 +94,83 @@ def case_gemm_timeline(M, N, K, act, want32, want16, bn, cluster=False, a_mn=0, 
     t = buf.view(sms, 8).cpu()
     used = t[:, 0] > 0
     t = t[used]
-    t0 = int(t[:, 0].min())
-    rel = (t - t0).float() / 1000.0  # us
+    rel = (t - int(t[:, 0].min())).float() / 1000.0  # us
     names = ["entry", "setup", "tma_issued", "first_stage", "last_mma", "unused", "epi_done", "exit"]
     res = {"event_us": e0.elapsed_time(e1) * 1e3, "ctas": int(used.sum()), "ok": True}
     for i, n in enumerate(names):
         col = rel[:, i][t[:, i] > 0]  # CTA-pair mode: only the leader CTA stamps the MMA-side events
         res[n] = [round(float(col.min()), 2), round(float(col.median()), 2), round(float(col.max()), 2)] if col.numel() else None
+    both = (t[:, 4] > 0) & (t[:, 6] > 0)
+    res["epi_us"] = round(float(((t[both, 6] - t[both, 4]).float() / 1000.0).median()), 2)  # stamp 4 -> 6, median over CTAs
+    # the same launch without the timeline buffer: mean of 50 back-to-back launches
+    e0.record()
+    for _ in range(50):
+        run()
+    e1.record()
+    torch.cuda.synchronize()
+    res["mean_us"] = round(e0.elapsed_time(e1) * 1e3 / 50, 2)
     return res
+
+
+def case_group_timeline(kind, bn):
+    """Phase timeline of one launch of the train step's backward, with the plan's epilogue options (train.cu, cfg2 sizes):
+    ffn2_dgrad: 16-bit out * saved GELU' (mask16) + column sums;  ffn1_dgrad / qkv_dgrad: fp32 out + fp32 residual;
+    out_dgrad: 16-bit out;  qkv_wgrad: [2d | d] x d weight gradients, both operands MN-major, split-K 4 into fp32."""
+    import torch
+    from univtg_b200 import _lib
+    lib = _lib.load_library()
+    M, d = 3424, 1024
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    buf = torch.zeros(sms * 8, dtype=torch.int64, device="cuda")
+    keep = []
+
+    def h(*shape):
+        x = (torch.randn(*shape, device="cuda") * 0.1).half()
+        keep.append(x)
+        return x
+
+    def f(*shape):
+        x = torch.randn(*shape, device="cuda")
+        keep.append(x)
+        return x
+
+    def dgrad(K):
+        p = _lib.GemmProblem()
+        a, b = h(M, K), h(K, d)
+        p.a, p.lda, p.a_mn, p.b, p.ldb, p.b_mn = _lib.ptr(a), K, 0, _lib.ptr(b), d, 1
+        p.M, p.N, p.K, p.ksplit, p.a_fmt, p.b_fmt, p.out_fmt, p.alpha = M, d, K, 1, -1, -1, -1, 1.0
+        return p
+
+    if kind == "qkv_wgrad":
+        probs = []
+        dq = h(M, 3 * d)
+        for N, off in ((2 * d, 0), (d, 2 * d)):
+            p = _lib.GemmProblem()
+            x = h(M, d)
+            out = f(N, d)
+            p.a, p.lda, p.a_mn, p.b, p.ldb, p.b_mn = dq.data_ptr() + 2 * off, 3 * d, 1, x.data_ptr(), d, 1  # columns [off, off + N)
+            p.M, p.N, p.K, p.ksplit, p.a_fmt, p.b_fmt, p.out_fmt, p.alpha = N, d, M, 4, -1, -1, -1, 1.0 / 1024
+            p.out32, p.ld32 = _lib.ptr(out), d
+            probs.append(p)
+    else:
+        p = dgrad(3 * d if kind == "qkv_dgrad" else d)
+        if kind.startswith("ffn2_dgrad"):  # _nomask / _nocolsum: the same launch without one of its two extra options
+            if kind != "ffn2_dgrad_nomask":
+                p.mask16, p.ld_mask, p.mask_mul = _lib.ptr(h(M, d)), d, 1
+            p.out16, p.ld16 = _lib.ptr(h(M, d)), d
+            if kind != "ffn2_dgrad_nocolsum":
+                p.colsum, p.colsum_scale = _lib.ptr(f(d)), 1.0 / 1024
+        elif kind in ("ffn1_dgrad", "qkv_dgrad"):
+            p.resid, p.ld_resid = _lib.ptr(f(M, d)), d
+            p.out32, p.ld32 = _lib.ptr(f(M, d)), d
+        else:
+            p.out16, p.ld16 = _lib.ptr(h(M, d)), d
+        probs = [p]
+    arr = (_lib.GemmProblem * len(probs))(*probs)
+
+    def run():
+        _lib.check(lib.univtg_op_gemm_group(arr, len(probs), 0, bn, 1, None, _lib.stream_ptr()), "op_gemm_group")
+    return _timeline(run, sms, buf)
 
 
 def case_layernorm(rows, d, ld16, fmt):
@@ -236,6 +313,13 @@ CASES = {
     "tl_outproj": (case_gemm_timeline, (3424, 1024, 1024, 0, True, False, 256)),
     "tl_qkv_bn256": (case_gemm_timeline, (3424, 3072, 1024, 0, False, True, 256)),
     "tl_ffn1_bn128": (case_gemm_timeline, (3424, 1024, 1024, 2, False, True, 128)),
+    "tl_ffn2_dgrad": (case_group_timeline, ("ffn2_dgrad", 256)),
+    "tl_ffn2_dgrad_nomask": (case_group_timeline, ("ffn2_dgrad_nomask", 256)),
+    "tl_ffn2_dgrad_nocolsum": (case_group_timeline, ("ffn2_dgrad_nocolsum", 256)),
+    "tl_ffn1_dgrad": (case_group_timeline, ("ffn1_dgrad", 256)),
+    "tl_out_dgrad": (case_group_timeline, ("out_dgrad", 256)),
+    "tl_qkv_dgrad": (case_group_timeline, ("qkv_dgrad", 256)),
+    "tl_qkv_wgrad": (case_group_timeline, ("qkv_wgrad", 256)),
     "ln_1024": (case_layernorm, (3424, 1024, 1024, 0)),
     "ln_256_bf16": (case_layernorm, (77, 256, 256, 1)),
     "ln_2818": (case_layernorm, (300, 2818, 2880, 0)),

@@ -237,23 +237,23 @@ __device__ __forceinline__ void epi_step(const GemmProblem& pr, const EpiRow& r,
     }
   }
   if (FULL && act == ACT_GELU && r.dact_row != nullptr) {  // training forward: activation and its derivative in one pass
-    float dg[16];
+    uint32_t w8[8];  // the derivative, packed to 16 bits as it is formed (8 registers rather than 16 next to v)
 #pragma unroll
-    for (int j = 0; j < 16; ++j) {
-      float gj;
-      gelu_erf_both(v[j], gj, dg[j]);
-      v[j] = gj * rsc;
+    for (int q = 0; q < 8; ++q) {
+      float g0, d0, g1, d1;
+      gelu_erf_both(v[2 * q], g0, d0);
+      gelu_erf_both(v[2 * q + 1], g1, d1);
+      v[2 * q] = g0 * rsc;
+      v[2 * q + 1] = g1 * rsc;
+      w8[q] = cvt16x2(d0, d1, ofmt);
     }
     if (r.valid) {
       if (vec) {
-        uint32_t w8[8];
-#pragma unroll
-        for (int q = 0; q < 8; ++q) w8[q] = cvt16x2(dg[2 * q], dg[2 * q + 1], ofmt);
         st_global_256(r.dact_row + n0, w8);
       } else {
 #pragma unroll
         for (int j = 0; j < 16; ++j)
-          if (n0 + j < pN) r.dact_row[n0 + j] = cvt16(dg[j], ofmt);
+          if (n0 + j < pN) r.dact_row[n0 + j] = (uint16_t)(w8[j / 2] >> (16 * (j & 1)));
       }
     }
   } else if (act == ACT_GELU) {
@@ -481,7 +481,9 @@ __device__ __forceinline__ void consumer_tiles(const GemmGroup& g, Ring& ring, f
       }
       named_bar_sync(1 + cw, 128);
     }
-    if (tid == 0 && cw == 1) stamp(g.dbg, 6);  // epilogue of the tile done (second warpgroup)
+    // epilogue of the tile done (second warpgroup's first thread; threadIdx.x is read again rather than a predicate kept
+    // across the tile, which keeps the FULL variant free of spills)
+    if (threadIdx.x == 128) stamp(g.dbg, 6);
   }
 }
 

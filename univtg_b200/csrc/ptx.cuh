@@ -189,19 +189,26 @@ UV_DEVINL void ld_global_256f(const float* p, float* v) {
 UV_DEVINL void red_add_f32x4(float* addr, float4 v) {
   asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(addr), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w) : "memory");
 }
+// one halving step of warp_colsum16.  OFF is a template parameter so that every index into v is a compile-time constant: with
+// a loop over OFF the compiler left the inner loop rolled in the GEMM's FULL epilogue, and the dynamic index put v (and with it
+// every value of the epilogue) in local memory.
+template <int OFF>
+UV_DEVINL void colsum16_step(float (&v)[16], int lane) {
+  const bool hi = (lane & OFF) != 0;
+#pragma unroll
+  for (int k = 0; k < OFF; ++k) {
+    const float send = hi ? v[k] : v[k + OFF];
+    const float keep = hi ? v[k + OFF] : v[k];
+    v[k] = keep + __shfl_xor_sync(0xffffffffu, send, OFF);
+  }
+}
 // Transposing reduction of 16 values per lane across the warp (16 shuffles instead of 16 x 5): on return every lane l holds
 // the sum over all 32 lanes of their v[l & 15] (v is clobbered).
 UV_DEVINL float warp_colsum16(float (&v)[16], int lane) {
-#pragma unroll
-  for (int off = 8; off >= 1; off >>= 1) {
-    const bool hi = (lane & off) != 0;
-#pragma unroll
-    for (int k = 0; k < off; ++k) {
-      const float send = hi ? v[k] : v[k + off];
-      const float keep = hi ? v[k + off] : v[k];
-      v[k] = keep + __shfl_xor_sync(0xffffffffu, send, off);
-    }
-  }
+  colsum16_step<8>(v, lane);
+  colsum16_step<4>(v, lane);
+  colsum16_step<2>(v, lane);
+  colsum16_step<1>(v, lane);
   return v[0] + __shfl_xor_sync(0xffffffffu, v[0], 16);
 }
 UV_DEVINL float warp_max(float v) {
