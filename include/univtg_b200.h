@@ -481,6 +481,24 @@ int univtg_decode_mr(const float* pred_logits, const float* pred_spans, const fl
 int univtg_temporal_nms(const double* windows, int32_t B, int32_t n, int32_t max_before_nms, double nms_thd, int32_t max_after_nms,
                         double* out, int32_t* counts, void* stream);
 
+/* The evaluation epoch's variants (main/inference_mr.py:101-222): one ragged row pool per epoch, query q owning the Lv rows of its
+ * batch (each batch is padded to its own maximum) from pool row offsets[q].
+ * univtg_decode_mr_pool = univtg_decode_mr writing the rounded rows of sample b to rows [*,3] f64 at row row_offset + b * Lv, and:
+ *   hl (with saliency_scores [B,Lv]): the highlight value of every clip at hl[row_offset + b * Lv + l], fp32(fp16(saliency)), or with
+ *     add_prob != 0 (eval_mode "add", :124-125) fp32(fp16(saliency)) + prob, prob being pred_logits with 0 where timestamp_mask == 0;
+ *   valid_len (with src_vid_mask [B,Lv]): src_vid_mask.sum(1) as int at valid_len[sample_offset + b];
+ *   round_multiple > 0 (eval/postprocessing.py:26-51): st / ed become double(rintf(fp32(x) / clip_length) * clip_length) in fp32
+ *     (IEEE division, ties to even) and the score float(f"{fp32(score):.4f}").  clip_length > 0.
+ * univtg_temporal_nms_pool = univtg_temporal_nms over that pool: query q's rows are row_offsets[q] .. row_offsets[q + 1] - 1
+ *   (row_offsets [Q+1] i64 on the device, at most max_rows each); with sort != 0 the first max_before_nms rows are first sorted by
+ *   score (descending, ties in row order) as temporal_nms does for clip-order (--no_sort_results) rows. */
+int univtg_decode_mr_pool(const float* pred_logits, const float* pred_spans, const float* timestamp, const float* timestamp_mask,
+                          const float* duration, const float* saliency_scores, const float* src_vid_mask, int32_t B, int32_t Lv,
+                          int32_t sort, int32_t add_prob, int32_t round_multiple, float clip_length, int64_t row_offset,
+                          int64_t sample_offset, double* rows, float* hl, int32_t* valid_len, void* stream);
+int univtg_temporal_nms_pool(const double* rows, const int64_t* row_offsets, int32_t Q, int32_t max_rows, int32_t max_before_nms,
+                             double nms_thd, int32_t max_after_nms, int32_t sort, double* out, int32_t* counts, void* stream);
+
 /* Per-query metrics of the reference's eval_submission (eval/eval.py:20-289, eval/utils.py:17-211), IEEE double, equal to numpy's
  * values bit for bit; univtg_b200/metrics.py does the packing and the means over queries.
  * univtg_eval_mr: pred [Q,10,3] f64 = the first n_pred[q] (1..10) rows [st, ed, score] of each query in submission order;

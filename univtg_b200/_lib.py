@@ -169,6 +169,9 @@ SIGNATURES = {
     "univtg_decode_mr": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
                                  c_void_p]),
     "univtg_temporal_nms": (c_int, [c_void_p, c_int, c_int, c_int, ctypes.c_double, c_int, c_void_p, c_void_p, c_void_p]),
+    "univtg_decode_mr_pool": (c_int, [c_void_p] * 7 + [c_int] * 5 + [c_float, ctypes.c_int64, ctypes.c_int64] + [c_void_p] * 4),
+    "univtg_temporal_nms_pool": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, ctypes.c_double, c_int, c_int, c_void_p, c_void_p,
+                                         c_void_p]),
     "univtg_eval_mr": (c_int, [c_void_p] * 4 + [c_int, c_int] + [c_void_p] * 5),
     "univtg_eval_hl": (c_int, [c_void_p] * 4 + [c_int, c_int, c_int] + [c_void_p] * 4),
     "univtg_eval_hl_topk": (c_int, [c_void_p] * 5 + [c_int] * 5 + [c_void_p, c_void_p]),

@@ -61,9 +61,17 @@ def temporal_nms(windows_r4, nms_thd, max_before_nms=10, max_after_nms=10):
     return out, counts
 
 
-def compose_submission(query_meta, outputs, targets, model_inputs, nms_thd=-1, max_before_nms=10, max_after_nms=10, sort=True):
+def compose_submission(query_meta, outputs, targets, model_inputs, nms_thd=-1, max_before_nms=10, max_after_nms=10, sort=True, *,
+                       eval_mode=None, round_multiple=0, clip_length=1.0):
     """The list of dicts `compute_mr_results` appends to `mr_res` (main/inference_mr.py:158-165), for one batch; with
-    nms_thd != -1 `pred_relevant_windows` is what post_processing_mr_nms would leave (:31-40)."""
+    nms_thd != -1 `pred_relevant_windows` is what post_processing_mr_nms would leave (:31-40).
+
+    eval_mode "add" gives pred_saliency_scores = fp32(fp16(saliency)) + prob (:124-125; None, "add_mr" and other values: the fp16
+    saliency), and round_multiple > 0 applies PostProcessorDETR's round_multiple with clip_length (:184-192) before the NMS, as
+    eval_epoch does.  For a whole evaluation epoch use univtg_b200.evaluation.eval_epoch, which also writes the files."""
+    if eval_mode is not None or round_multiple > 0:
+        return _compose_pool(query_meta, outputs, targets, model_inputs, nms_thd, max_before_nms, max_after_nms, sort, eval_mode,
+                             round_multiple, clip_length)
     durations = [m["duration"] for m in query_meta]
     dec = decode_mr(outputs, targets, durations, sort=sort, rounded=True)
     rows = dec["windows_r4"]
@@ -79,4 +87,31 @@ def compose_submission(query_meta, outputs, targets, model_inputs, nms_thd=-1, m
     for b, meta in enumerate(query_meta):
         res.append(dict(qid=meta["qid"], query=meta["query"], vid=meta["vid"], pred_relevant_windows=windows[b],
                         pred_saliency_scores=sal[b, :int(lens[b])].tolist()))
+    return res
+
+
+def _compose_pool(query_meta, outputs, targets, model_inputs, nms_thd, max_before_nms, max_after_nms, sort, eval_mode, round_multiple,
+                  clip_length):
+    from types import SimpleNamespace
+
+    from .evaluation import EpochState
+
+    dev = outputs["pred_logits"].device
+    if dev.type != "cuda":
+        raise RuntimeError("univtg_b200: compose_submission runs on CUDA tensors only (no CPU path)")
+    opt = SimpleNamespace(no_sort_results=not sort, eval_mode=eval_mode, round_multiple=round_multiple, clip_length=clip_length,
+                          nms_thd=nms_thd, max_before_nms=max_before_nms, max_after_nms=max_after_nms)
+    with torch.cuda.device(dev):
+        state = EpochState(dev, len(query_meta), opt)
+        state.add_batch(query_meta, model_inputs, targets, outputs)
+        host = state.finish({})
+    res = []
+    for b, meta in enumerate(query_meta):
+        o = int(host["offsets"][b])
+        if nms_thd != -1:
+            windows = host["kept"][b, :int(host["counts"][b])].tolist()
+        else:
+            windows = host["rows"][o:o + state.n_rows[b]].tolist()
+        res.append(dict(qid=meta["qid"], query=meta["query"], vid=meta["vid"], pred_relevant_windows=windows,
+                        pred_saliency_scores=host["hl"][o:o + int(host["lens"][b])].tolist()))
     return res

@@ -725,3 +725,98 @@ def teacher_case_sha256(case):
         h.update(str(f.shape).encode())
         h.update(f.tobytes())
     return h.hexdigest()
+
+
+# ---- moment-retrieval evaluation epoch (main/inference_mr.py eval_epoch) ------------------------------------------------
+EPOCH_TS_DEN = 256.0  # clip i of a fake video sits at timestamp (2 i + 1) / 256: dyadic, so planted windows are exact in fp32
+EPOCH_PLANTS = (2, 3, 4, 6, 9, 10, 12, 15, 20, 25, 36, 51, 100, 127, 200)  # (timestamp + span) = k / 256 at planted clips
+EPOCH_SCORE_TIES = (0.03125, 0.09375, 0.15625, 0.5, 0.5)  # exact fp32 values on a 4-decimal tie, and a repeated score
+
+
+def eval_epoch_opt(**over):
+    """The fields of the reference's TestOptions that eval_epoch reads, at the defaults of main/config.py."""
+    opt = dict(eval_bsz=8, num_workers=0, pin_memory=False, device="cuda", span_loss_type="l1", model_id="univtg", eval_mode=None,
+               no_sort_results=False, debug=False, clip_length=2.0, round_multiple=1, results_dir=".", eval_split_name="val",
+               nms_thd=-1, max_before_nms=10, max_after_nms=10)
+    opt.update(over)
+    return Namespace(**opt)
+
+
+class EvalEpochDataset:
+    """Items in the format of main/dataset.py DatasetMR.__getitem__ for eval (load_labels=True) and the ground truth list `data`.
+
+    Ragged clip and token counts, durations that are seldom multiples of the clip length (and a few dyadic ones - 40, 64, 128 -
+    on which the planted windows land exactly on 4-decimal and half-clip-length ties), one gt window per query (so no two gt
+    windows tie in the metrics' IoU order) and 3-annotator saliency labels on the 2 s clip grid."""
+
+    def __init__(self, seed, n_queries=37, lv=(6, 75), lt=(3, 32), dv=8, dt=8, load_labels=True):
+        rng = random.Random(seed)
+        g = torch.Generator().manual_seed(seed)
+        self.load_labels = load_labels
+        self.items, self.data = [], []
+        for q in range(n_queries):
+            Lv, Lt = rng.randint(*lv), rng.randint(*lt)
+            dur = rng.choice((40.0, 64.0, 128.0)) if rng.random() < 0.3 else round(rng.uniform(12.0, 150.0), 2)
+            n_clips = max(1, int(dur / 2))
+            st = 2 * rng.randint(0, max(0, n_clips - 2))
+            ed = min(2 * n_clips, st + 2 * rng.randint(1, 6))
+            ids = list(range(st // 2, ed // 2))
+            meta = {"qid": 1000 + q, "query": f"query {q}", "vid": f"video_{q % 11}", "duration": dur}
+            ts = ((2 * torch.arange(Lv, dtype=torch.float32) + 1) / EPOCH_TS_DEN)[:, None].expand(Lv, 2).contiguous()
+            window = torch.zeros(Lv)
+            c0 = min(Lv - 1, int(st / dur * Lv))
+            window[c0:max(c0 + 1, min(Lv, int(ed / dur * Lv)))] = 1.0
+            span_nn = torch.tensor([st / dur, ed / dur], dtype=torch.float32).expand(Lv, 2).contiguous()
+            sal = torch.randint(0, 5, (Lv,), generator=g).float() / 4.0
+            pos = int(torch.randint(0, Lv, (1,), generator=g))
+            sal[pos] = 1.0
+            mi = {"query_feat": torch.randn(Lt, dt, generator=g), "video_feat": torch.randn(Lv, dv, generator=g), "timestamp": ts,
+                  "timestamp_window": window, "span_labels_nn": span_nn, "saliency_scores": sal, "saliency_pos_labels": [pos],
+                  "saliency_neg_labels": [(pos + 1) % Lv]}
+            self.items.append({"meta": meta, "model_inputs": mi})
+            self.data.append({"qid": meta["qid"], "query": meta["query"], "vid": meta["vid"], "duration": dur,
+                              "relevant_windows": [[st, ed]], "relevant_clip_ids": ids,
+                              "saliency_scores": [[rng.randint(0, 4) for _ in range(3)] for _ in ids]})
+
+    def __len__(self):
+        return len(self.items)
+
+    def __getitem__(self, idx):
+        return self.items[idx]
+
+
+class ReplayEvalModel(torch.nn.Module):
+    """Stands in for the model in eval_epoch: call k returns outputs drawn from Generator(seed * 1000 + k) for the batch's shape,
+    on the device of its one buffer.  Scores are sigmoid values, a third of them on a 1/16 grid (ties), a few planted on 4-decimal
+    ties; some clips get windows (timestamp + span) = k / 256 (exact for the dyadic durations); saliency is fp32 with a few values
+    half way between fp16 neighbours.  n_classes=2 gives two-class logits (refused by the device evaluation)."""
+
+    def __init__(self, seed, d=16, n_classes=1):
+        super().__init__()
+        self.seed, self.d, self.n_classes, self.calls = seed, d, n_classes, 0
+        self.register_buffer("anchor", torch.zeros(1))
+
+    def forward(self, src_txt, src_txt_mask, src_vid, src_vid_mask):
+        B, Lv = src_vid.shape[:2]
+        g = torch.Generator().manual_seed(self.seed * 1000 + self.calls)
+        self.calls += 1
+        logits = torch.sigmoid(2.0 * torch.randn(B, Lv, generator=g))
+        grid = torch.rand(B, Lv, generator=g) < 0.33
+        logits = torch.where(grid, (logits * 16).round() / 16, logits)
+        spans = torch.stack([-0.3 * torch.rand(B, Lv, generator=g), 0.3 * torch.rand(B, Lv, generator=g)], -1)
+        idx = torch.arange(Lv, dtype=torch.float32)
+        for b in range(B):
+            for j, k in enumerate(EPOCH_PLANTS[:Lv]):
+                c = (7 * j + b) % Lv
+                spans[b, c, 0] = (k - 2 * idx[c] - 1) / EPOCH_TS_DEN
+                spans[b, c, 1] = (min(255, k + 4 * (j + 1)) - 2 * idx[c] - 1) / EPOCH_TS_DEN
+            for j, v in enumerate(EPOCH_SCORE_TIES[:Lv]):
+                logits[b, (5 * j + 2 * b + 1) % Lv] = v
+        sal = torch.randn(B, Lv, generator=g)
+        half = torch.rand(B, Lv, generator=g) < 0.2  # midpoints of fp16 neighbours: ties of __float2half_rn
+        sal = torch.where(half, torch.round(sal * 1024) / 1024 + 1.0 / 2048, sal)
+        out = {"pred_logits": logits[..., None].repeat(1, 1, self.n_classes), "pred_spans": spans, "saliency_scores": sal,
+               "vid_mem_proj": torch.randn(B, Lv, self.d, generator=g), "txt_mem_proj": torch.randn(B, 1, self.d, generator=g),
+               "src_vid_mask": src_vid_mask}
+        dev = self.anchor.device
+        return {k: v.to(dev) for k, v in out.items()}
