@@ -14,8 +14,9 @@ graph launch.  What the eager step fixes on the host at every step is read from 
   * AdamW's lr and step: univtg_adamw_step_dev reads lr from a device scalar (refreshed outside the graph when
     optimizer.lr changes, e.g. by a scheduler), reads the step from a device counter it advances only when the update was not
     skipped, and takes the bias corrections from a host-built table - bit-identical to the eager univtg_adamw_step;
-  * the overflow flag of dynamic loss scaling is copied to pinned memory inside the graph and consumed one call later, exactly
-    where the eager FlatAdamW.step consumes it; a new grad_scale selects (or captures) another graph.
+  * the skip flag of the update (non-finite gradients) is copied to pinned memory inside the graph and consumed one call later,
+    exactly where the eager FlatAdamW.step consumes it: a skipped update is not counted, and with dynamic loss scaling the
+    scale backs off; a new grad_scale selects (or captures) another graph.
 
 One graph per (B, Lv, Lt, input dtypes, target keys and shapes, grad_scale, dropout rates, optimizer constants), kept in an
 LRU of `max_graphs`.  All graphs of one GraphedTrainStep share one training workspace and one text-position scratch (sized for
@@ -194,11 +195,10 @@ class GraphedTrainStep:
             # ago), then this step
             opt._consume_overflow_flag()
             opt.step_count += 1
-            if opt.dynamic_loss_scale:
-                slot = self.replays % _FLAG_SLOTS
-                ev = self._events[slot]
-                ev.record()
-                opt._flag_host, opt._flag_event = self._flags_host[slot:slot + 1], ev
+            slot = self.replays % _FLAG_SLOTS
+            ev = self._events[slot]
+            ev.record()
+            opt._flag_host, opt._flag_event = self._flags_host[slot:slot + 1], ev
             self._last_count, self._last_event = opt.step_count, opt._flag_event
             opt._opt_called = True  # (what torch's step wrapper records: lr schedulers then know an update has run)
             model.__dict__["_flat_grad_dirty"] = True
@@ -215,7 +215,7 @@ class GraphedTrainStep:
             self._lr_host = lr
         if opt.step_count != self._last_count or opt._flag_event is not self._last_event:
             self._step.fill_(opt.step_count)
-            if opt.dynamic_loss_scale and opt._flag_event is not None and opt._flag_event is opt._flag_evt:
+            if opt._flag_event is not None and opt._flag_event is opt._flag_evt:
                 # the last eager step's flag is not consumed yet: if it was skipped, step_count counts one update too many
                 self._step.sub_(opt._scratch[2:3].ne(0).to(torch.int32))
 
@@ -288,10 +288,9 @@ class GraphedTrainStep:
         params = model._packed_params()
         arr = (ctypes.c_void_p * len(params))(*[p.data_ptr() for p in params])
         _lib.check(lib.univtg_pack_vectors(ctypes.byref(cfg), arr, len(arr), _lib.ptr(packed), _lib.stream_ptr()), "univtg_pack_vectors")
-        if opt.dynamic_loss_scale:
-            slot = torch.remainder(self._counter, _FLAG_SLOTS)
-            self._flags_dev.index_copy_(0, slot, opt._scratch[2:3])
-            self._flags_host.copy_(self._flags_dev, non_blocking=True)
+        slot = torch.remainder(self._counter, _FLAG_SLOTS)
+        self._flags_dev.index_copy_(0, slot, opt._scratch[2:3])
+        self._flags_host.copy_(self._flags_dev, non_blocking=True)
 
     def _capture(self, key, inputs, targets, mask_GT):
         model = self.model

@@ -39,9 +39,10 @@ class FlatAdamW(torch.optim.Optimizer):
         self.max_grad_norm = float(max_grad_norm) if max_grad_norm is not None else 0.0
         self.write_clipped_grads = bool(write_clipped_grads)
         self.step_count = 0
-        # dynamic loss scale of the fp16 backward (model.grad_scale): a step whose gradients are not finite is skipped ON THE
-        # DEVICE (univtg_adamw_step); the flag is read back one step later (no host synchronisation in the step), the scale is
-        # halved and the step counter corrected; after `growth_interval` good steps in a row the scale doubles again.
+        # A step whose gradients are not finite is skipped ON THE DEVICE (univtg_adamw_step), in every format; its flag is read
+        # back one step later (no host synchronisation in the step) and the skipped update is taken off step_count, so the bias
+        # correction, state_dict()'s 'step' and skipped_steps count real updates only.  With the dynamic loss scale of the fp16
+        # backward (model.grad_scale) a skipped step also halves the scale, and `growth_interval` good steps in a row double it.
         self.dynamic_loss_scale = bool(dynamic_loss_scale) and model.operand_format == 0
         self.growth_interval, self.max_loss_scale = int(growth_interval), float(max_loss_scale)
         self.skipped_steps, self._good_streak = 0, 0
@@ -133,7 +134,12 @@ class FlatAdamW(torch.optim.Optimizer):
         if flat_g.numel() != self._flat_p.numel():
             raise RuntimeError("FlatAdamW: gradient / parameter buffer size mismatch")
         lib = _lib.load_library()
-        self._consume_overflow_flag()
+        # Inside a torch.cuda.graph capture of the whole training step the step number is baked into the graph and the host
+        # cannot wait for a flag: the skip flag is neither read nor staged there.  The update itself still skips non-finite
+        # gradients on the device.
+        capturing = torch.cuda.is_current_stream_capturing()
+        if not capturing:
+            self._consume_overflow_flag()
         self.step_count += 1
         model.__dict__["_flat_grad_unstepped"] = False
         with torch.cuda.device(flat_g.device):
@@ -170,7 +176,7 @@ class FlatAdamW(torch.optim.Optimizer):
                     self._zero_event.record()
                 model.__dict__["_flat_grad_prezeroed"] = (flat_g.data_ptr(), self._zero_event)
                 model.__dict__["_flat_grad_dirty"] = False
-            if self.dynamic_loss_scale:
+            if not capturing:
                 if self._flag_buf is None:
                     self._flag_buf = torch.zeros(1, dtype=torch.float32).pin_memory()
                     self._flag_evt = torch.cuda.Event()
@@ -180,13 +186,19 @@ class FlatAdamW(torch.optim.Optimizer):
         return self._scratch[1]
 
     def _consume_overflow_flag(self):
-        """Outcome of the PREVIOUS step (its flag copy finished long ago: no stall): back off / grow the loss scale."""
-        if not self.dynamic_loss_scale or self._flag_event is None:
+        """Outcome of the PREVIOUS step (its flag copy finished long ago: no stall): a skipped update is not counted; with the
+        dynamic loss scale, back off / grow the scale."""
+        if self._flag_event is None:
             return
         self._flag_event.synchronize()
-        if float(self._flag_host[0]) != 0.0:
+        skipped = float(self._flag_host[0]) != 0.0
+        self._flag_host = self._flag_event = None  # consumed once
+        if skipped:
             self.step_count -= 1  # that update never happened
             self.skipped_steps += 1
+        if not self.dynamic_loss_scale:
+            return
+        if skipped:
             self._good_streak = 0
             self.model.grad_scale = max(1.0, self.model.grad_scale * 0.5)
         else:
@@ -206,7 +218,9 @@ class FlatAdamW(torch.optim.Optimizer):
     @torch.no_grad()
     def state_dict(self):
         """{'state': {i: {'step', 'exp_avg', 'exp_avg_sq'}}, 'param_groups': [...]} exactly as torch.optim.AdamW writes it
-        (parameters numbered in group order = named_parameters() order), plus a 'loss_scale' entry torch ignores."""
+        (parameters numbered in group order = named_parameters() order), plus a 'loss_scale' entry torch ignores.  The last
+        step's skip flag is consumed first, so a checkpoint taken right after a skipped step counts real updates only."""
+        self._consume_overflow_flag()
         group = self._group()
         offs = self._offsets()
         state = {}
