@@ -411,6 +411,17 @@ int univtg_debug_gemm_timeline(void* buf);
  * M x N with kblocks 64-wide k-blocks each; step 16 for K-major B, 64 for MN-major B).  Testing / tuning aid. */
 int univtg_debug_choose_tile(const int32_t* Ms, const int32_t* Ns, const int32_t* kblocks, int32_t num, int32_t num_sms, int32_t step,
                              int32_t max_split, int32_t* bn, int32_t* ksplit);
+/* Host-only, the same with a split limit per problem (powers of two; 1 for a problem whose epilogue cannot accumulate): the
+ * launch's one tile width and each problem's split-K factor (ksplit[num]).  univtg_debug_choose_tile gives every problem the
+ * limit max_split and reports the largest factor. */
+int univtg_debug_choose_tile_group(const int32_t* Ms, const int32_t* Ns, const int32_t* kblocks, const int32_t* max_split, int32_t num,
+                                   int32_t num_sms, int32_t step, int32_t* bn, int32_t* ksplit);
+/* Host-only: the static deal of a grouped GEMM launch's work units (output tile x k-split) over its persistent CTAs, walked as
+ * the kernel's CTAs walk it.  Units are numbered problem by problem (tiles n fastest, then m, then the split); cta[u] receives
+ * the CTA that runs unit u, -1 if none does and -2 if more than one does.  Returns the number of units (cap bounds what is
+ * written), or -1 for bad arguments. */
+int32_t univtg_debug_gemm_deal(const int32_t* Ms, const int32_t* Ns, const int32_t* kblocks, const int32_t* ksplit, int32_t num,
+                               int32_t num_sms, int32_t bn, int32_t* cta, int32_t cap);
 /* Parameter update of the reference's training loop (main/train_vlp_ddp.py:66-68 = main/train_mr.py:64-66; optimizer built at
  * main/config.py:350 as torch.optim.AdamW(lr, weight_decay)) over ONE flat fp32 buffer of n floats (n % 4 == 0, 16-byte
  * aligned; the plugin lays every parameter and its gradient out at the same offsets):

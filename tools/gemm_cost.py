@@ -12,6 +12,8 @@ Two views, both with CUDA events:
     row remapping, residual / mask / column-sum options and the training forward's pre-activation and GELU' stores.
     Reported: us per launch, TFLOP/s, share of the data-sheet 989 TFLOP/s (dense fp16, H100 SXM at 700 W), and the sum of
     count x us per step next to the plan's own GEMM time.
+  * merged: each backward launch that runs a data gradient together with the weight gradients reading the same operand, against
+    the separate launches it replaces (one encoder layer and projector layer 1 at cfg2), both at the plan's widths and splits.
   * plan: the summed GEMM launch times of one cfg2 and cfg5 forward and one cfg2 train step, from the plan's per-launch event
     timeline.
 
@@ -65,9 +67,10 @@ def forward_groups(cfg_name):
     ]
 
 
-def backward_groups(cfg_name):
+def backward_groups(cfg_name, separate=False):
     """the backward's launches (train.cu: univtg_backward): data gradients A K-major x B MN-major, weight gradients both
-    MN-major with split-K into a pre-zeroed fp32 output."""
+    MN-major with split-K into a pre-zeroed fp32 output.  The last entry of each tuple is the weight gradients' split limit.
+    separate: the earlier plan, in which data and weight gradients had launches of their own."""
     c = synth.CONFIGS[cfg_name]
     B, Lv, Lt, d, ff, n = c["batch"], c["l_vid"], c["l_txt"], c["hidden_dim"], c["dim_feedforward"], c["enc_layers"]
     M, Mv, Mt, Mh = B * (Lv + Lt), B * Lv, B * Lt, B * (Lv + 1)
@@ -79,6 +82,19 @@ def backward_groups(cfg_name):
         (f"{f} conv wgrad (3 taps)", 2, [P(d, d, Mh, **wg)] * 3, 64, 8),
         (f"{f} conv2 dgrad (class + span)", 1, [P(Mh, d, 3 * d, **dg)] * 2, 64, 1),
         (f"{f} conv1 dgrad", 1, [P(Mh, d, 6 * d, **dg)], 64, 1),
+    ]
+    if not separate:
+        g += [
+            (f"{f} ffn2 dgrad + w2 wgrad", n, [P(M, ff, d, **dg), P(d, ff, M, **wg)], 64, 4),
+            (f"{f} ffn1 dgrad + w1 wgrad", n, [P(M, d, ff, **dg), P(ff, d, M, **wg)], 64, 4),
+            (f"{f} out-proj dgrad + wgrad", n, [P(M, d, d, **dg), P(d, d, M, **wg)], 64, 4),
+            (f"{f} qkv dgrad + wgrad (2d + d)", n, [P(M, d, 3 * d, **dg), P(2 * d, d, M, **wg), P(d, d, M, **wg)], 64, 4),
+            (f"{f} proj0 wgrad (vid + txt)", 1, [P(d, kv, Mv, **wg), P(d, kt, Mt, **wg)], 64, 16),
+            (f"{f} proj0 dgrad (vid + txt)", 1, [P(Mv, kv, d, **dg), P(Mt, kt, d, **dg)], 64, 1),
+            (f"{f} proj1 wgrad + dgrad (vid + txt)", 1, [P(d, d, Mv, **wg), P(d, d, Mt, **wg), P(Mv, d, d, **dg), P(Mt, d, d, **dg)], 64, 4),
+        ]
+        return g
+    g += [
         (f"{f} ffn2 dgrad", n, [P(M, ff, d, **dg)], 64, 1),
         (f"{f} ffn wgrad (w2 + w1)", n, [P(d, ff, M, **wg), P(ff, d, M, **wg)], 64, 16),
         (f"{f} ffn1 dgrad", n, [P(M, d, ff, **dg)], 64, 1),
@@ -94,14 +110,16 @@ def backward_groups(cfg_name):
 
 
 def choose(probs, num_sms, step, max_split):
+    """width and per-problem split-K factors (problems without split-K accumulation: limit 1)"""
     lib = _lib.load_library()
     n = len(probs)
     Ms = (ctypes.c_int32 * n)(*[p["M"] for p in probs])
     Ns = (ctypes.c_int32 * n)(*[p["N"] for p in probs])
     Ks = (ctypes.c_int32 * n)(*[(p["K"] + 63) // 64 for p in probs])
-    bn, ks = ctypes.c_int32(0), ctypes.c_int32(0)
-    _lib.check(lib.univtg_debug_choose_tile(Ms, Ns, Ks, n, num_sms, step, max_split, ctypes.byref(bn), ctypes.byref(ks)), "choose_tile")
-    return bn.value, ks.value
+    lim = (ctypes.c_int32 * n)(*[max_split if p.get("acc") else 1 for p in probs])
+    bn, ks = ctypes.c_int32(0), (ctypes.c_int32 * n)()
+    _lib.check(lib.univtg_debug_choose_tile_group(Ms, Ns, Ks, lim, n, num_sms, step, ctypes.byref(bn), ks), "choose_tile")
+    return bn.value, list(ks)
 
 
 def time_group(probs, bn, ksplit, launches):
@@ -115,7 +133,7 @@ def time_group(probs, bn, ksplit, launches):
         p = arr[i]
         p.a, p.lda, p.a_mn = a.data_ptr(), (M if q["a_mn"] else K), q["a_mn"]
         p.b, p.ldb, p.b_mn = b.data_ptr(), (N if q["b_mn"] else K), q["b_mn"]
-        p.M, p.N, p.K, p.ksplit = M, N, K, (ksplit if q.get("acc") else 1)
+        p.M, p.N, p.K, p.ksplit = M, N, K, (ksplit[i] if q.get("acc") else 1)
         p.a_fmt, p.b_fmt, p.out_fmt, p.alpha, p.colsum_scale = -1, -1, -1, 1.0, 1.0
         p.act = q.get("act", 0)
         keep += [a, b]
@@ -149,6 +167,34 @@ def time_group(probs, bn, ksplit, launches):
     us = e0.elapsed_time(e1) / launches * 1e3
     tf = sum(2.0 * q["M"] * q["N"] * q["K"] for q in probs) / (us * 1e-6) / 1e12
     return dict(us=round(us, 3), tflops=round(tf, 1), peak_share=round(tf / PEAK_TFLOPS, 4), full=full.value)
+
+
+def merged_comparison(num_sms, launches):
+    """each merged backward launch of cfg2 against the separate launches it replaces (per encoder layer: the FFN pair of launches
+    against FFN2 dgrad, the FFN weight-gradient launch and FFN1 dgrad)"""
+    new = {name.split(" bwd ")[1]: (probs, step, ms) for name, _, probs, step, ms in backward_groups("cfg2")}
+    old = {name.split(" bwd ")[1]: (probs, step, ms) for name, _, probs, step, ms in backward_groups("cfg2", separate=True)}
+
+    def t(entry):
+        probs, step, ms = entry
+        bn, ks = choose(probs, num_sms, step, ms)
+        return time_group(probs, bn, ks, launches)["us"], bn, ks
+
+    pairs = [("ffn (two launches)", ["ffn2 dgrad + w2 wgrad", "ffn1 dgrad + w1 wgrad"], ["ffn2 dgrad", "ffn wgrad (w2 + w1)", "ffn1 dgrad"]),
+             ("out-proj", ["out-proj dgrad + wgrad"], ["out-proj dgrad", "out-proj wgrad"]),
+             ("qkv", ["qkv dgrad + wgrad (2d + d)"], ["qkv dgrad", "qkv wgrad (2d + d)"]),
+             ("proj1", ["proj1 wgrad + dgrad (vid + txt)"], ["proj1 wgrad (vid + txt)", "proj1 dgrad (vid + txt)"])]
+    rows = []
+    for name, merged, separate in pairs:
+        m = [t(new[k]) for k in merged]
+        s = [t(old[k]) for k in separate]
+        mu, su = sum(x[0] for x in m), sum(x[0] for x in s)
+        rows.append(dict(name=name, merged_us=round(mu, 3), separate_us=round(su, 3),
+                         merged=[dict(launch=k, us=round(x[0], 3), bn=x[1], ksplit=x[2]) for k, x in zip(merged, m)],
+                         separate=[dict(launch=k, us=round(x[0], 3), bn=x[1], ksplit=x[2]) for k, x in zip(separate, s)]))
+        print(f"merged {name:20s} {mu:8.2f} us  separate {su:8.2f} us ({mu / su - 1:+.1%})  "
+              f"merged {[(x[1], x[2]) for x in m]} separate {[(x[1], x[2]) for x in s]}", flush=True)
+    return rows
 
 
 def plan_gemm_ms(cfg_name, train):
@@ -225,12 +271,13 @@ def main():
                   flush=True)
         per_step[set_name] = round(total / 1e3, 4)
     print("sum of count x us at the chosen widths, ms:", per_step)
+    merged = merged_comparison(sms, args.launches)
     plan = {}
     if not args.no_plan:
         plan = {"cfg2_fwd": plan_gemm_ms("cfg2", False), "cfg5_fwd": plan_gemm_ms("cfg5", False), "cfg2_train": plan_gemm_ms("cfg2", True)}
         print("plan GEMM time per step:", plan)
     res = dict(gpu=gpu_info(), lib=os.environ.get("UNIVTG_LIB", "default"), launches=args.launches, peak_tflops=PEAK_TFLOPS,
-               groups=rows, modelled_ms=per_step, plan=plan)
+               groups=rows, modelled_ms=per_step, merged=merged, plan=plan)
     os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
     with open(args.out, "w") as f:
         json.dump(res, f, indent=1)

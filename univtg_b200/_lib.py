@@ -206,6 +206,8 @@ SIGNATURES = {
     "univtg_op_txt_pos_bwd": (c_int, [ctypes.POINTER(TxtPosBwd), ctypes.POINTER(Rng), c_int, c_void_p]),
     "univtg_debug_gemm_timeline": (c_int, [c_void_p]),
     "univtg_debug_choose_tile": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
+    "univtg_debug_choose_tile_group": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
+    "univtg_debug_gemm_deal": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_int]),
     "univtg_op_layernorm": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_float, c_int, c_void_p, c_void_p, c_int,
                                     c_void_p]),
     "univtg_op_attention": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int,

@@ -303,13 +303,13 @@ int univtg_plan_create(const univtg_config* cfg, const univtg_shape* shape, cons
   // per-launch tile widths: fill the SMs with as little wave quantisation as possible (fp16x3 walks every K three times)
   const int sms = P->num_sms, M = P->M, Mh = P->Mh, kx = is_split(*cfg) ? 3 : 1;
   for (int i = 0; i < cfg->n_input_proj; ++i)
-    P->bn_proj[i] = tile_for(sms, 16, 1, MNK{P->Mv, d, kx * P->lay.vid[i].kpad}, MNK{P->Mt, d, kx * P->lay.txt[i].kpad}).bn;
-  P->bn_qkv = tile_for(sms, 16, 1, MNK{M, 2 * d, kx * d}, MNK{M, d, kx * d}).bn;
-  P->bn_out = tile_for(sms, 16, 1, MNK{M, d, kx * d}).bn;
-  P->bn_ffn1 = tile_for(sms, 16, 1, MNK{M, ff, kx * d}).bn;
-  P->bn_ffn2 = tile_for(sms, 16, 1, MNK{M, d, kx * ff}).bn;
-  P->bn_conv1 = tile_for(sms, 16, 1, MNK{Mh, 2 * d, kx * 3 * d}).bn;
-  P->bn_conv2 = tile_for(sms, 16, 1, MNK{Mh, d, kx * 3 * d}, MNK{Mh, d, kx * 3 * d}).bn;
+    P->bn_proj[i] = tile_for(sms, 16, MNK{P->Mv, d, kx * P->lay.vid[i].kpad}, MNK{P->Mt, d, kx * P->lay.txt[i].kpad}).bn;
+  P->bn_qkv = tile_for(sms, 16, MNK{M, 2 * d, kx * d}, MNK{M, d, kx * d}).bn;
+  P->bn_out = tile_for(sms, 16, MNK{M, d, kx * d}).bn;
+  P->bn_ffn1 = tile_for(sms, 16, MNK{M, ff, kx * d}).bn;
+  P->bn_ffn2 = tile_for(sms, 16, MNK{M, d, kx * ff}).bn;
+  P->bn_conv1 = tile_for(sms, 16, MNK{Mh, 2 * d, kx * 3 * d}).bn;
+  P->bn_conv2 = tile_for(sms, 16, MNK{Mh, d, kx * 3 * d}, MNK{Mh, d, kx * 3 * d}).bn;
   P->launches = 1 + 3 * cfg->n_input_proj + 7 * cfg->enc_layers + 6;
   *out = P;
   return 0;
@@ -817,10 +817,32 @@ int univtg_debug_choose_tile(const int32_t* Ms, const int32_t* Ns, const int32_t
     set_error("univtg_debug_choose_tile: bad argument");
     return 1;
   }
-  const uv::TileChoice t = uv::choose_tile(Ms, Ns, kblocks, num, num_sms, step, max_split);
+  const int32_t limits[GEMM_MAX_GROUP] = {max_split, max_split, max_split, max_split};
+  const uv::TileChoice t = uv::choose_tile(Ms, Ns, kblocks, limits, num, num_sms, step);
   *bn = t.bn;
   *ksplit = t.ksplit;
   return 0;
+}
+
+int univtg_debug_choose_tile_group(const int32_t* Ms, const int32_t* Ns, const int32_t* kblocks, const int32_t* max_split, int32_t num,
+                                   int32_t num_sms, int32_t step, int32_t* bn, int32_t* ksplit) {
+  bool ok = Ms && Ns && kblocks && max_split && bn && ksplit && num >= 1 && num <= GEMM_MAX_GROUP && num_sms >= 1 && (step == 16 || step == 64);
+  for (int p = 0; ok && p < num; ++p) ok = max_split[p] >= 1 && (max_split[p] & (max_split[p] - 1)) == 0;
+  if (!ok) {
+    set_error("univtg_debug_choose_tile_group: bad argument");
+    return 1;
+  }
+  const uv::TileChoice t = uv::choose_tile(Ms, Ns, kblocks, max_split, num, num_sms, step);
+  *bn = t.bn;
+  for (int p = 0; p < num; ++p) ksplit[p] = t.ks[p];
+  return 0;
+}
+
+int32_t univtg_debug_gemm_deal(const int32_t* Ms, const int32_t* Ns, const int32_t* kblocks, const int32_t* ksplit, int32_t num,
+                               int32_t num_sms, int32_t bn, int32_t* cta, int32_t cap) {
+  const int n = (Ms && Ns && kblocks && ksplit && (cta || cap == 0) && cap >= 0) ? uv::gemm_deal_ctas(Ms, Ns, kblocks, ksplit, num, num_sms, bn, cta, cap) : -1;
+  if (n < 0) set_error("univtg_debug_gemm_deal: bad argument");
+  return n;
 }
 
 int univtg_debug_gemm_timeline(void* buf) {

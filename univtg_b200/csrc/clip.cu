@@ -350,7 +350,7 @@ int clip_gemm(const uint16_t* A, int M, int K, const uint16_t* Wt, int N, int fm
   memset(&g, 0, sizeof(g));
   g.num = 1;
   g.fmt = fmt;
-  const int bn = tile_for(sms, 16, 1, MNK{M, N, K}).bn;
+  const int bn = tile_for(sms, 16, MNK{M, N, K}).bn;
   if (setup_linear(g.p[0], A, M, K, K, Wt, N, K, bn)) return 1;
   epi(g.p[0]);
   return launch_gemm_group(g, bn, sms, st);

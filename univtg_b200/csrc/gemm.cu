@@ -7,7 +7,7 @@
 // in-projections + out-projection (torch MHA called at model/transformer_encoder_droppath.py:118), the FFN
 // (:122) and the k=3 Conv1d heads (model/univtg.py:378-382) expressed as three row-shifted K segments.
 //
-// Roles (384 threads = 3 warpgroups, 1 CTA / SM, persistent over a static round-robin tile schedule of 128 x BN tiles):
+// Roles (384 threads = 3 warpgroups, 1 CTA / SM, persistent over a static, longest-first deal of 128 x BN tiles):
 //   warpgroup 2 (one elected lane of warp 8): TMA producer (cp.async.bulk.tensor -> 128B-swizzled smem ring, mbarrier
 //                    expect_tx); it gives most of its registers to the consumers (setmaxnreg)
 //   warpgroups 0, 1: consumers.  Each issues wgmma m64 x BN x k16 for its 64 rows of the tile (accumulators in registers),
@@ -52,10 +52,11 @@ struct TileInfo {
   int p, m_blk, n_blk, kb0, kb1, split;
 };
 
-// CL = 1: `t` is this CTA's tile index.  CL = 2: `t` indexes a 256-row PAIR tile made of two vertically adjacent 128-row tiles
+// `t` is a unit index of the deal (gemm_deal_unit, kernels.h): problems in order (launch_gemm_group put them in deal order),
+// then tile order inside the problem.  CL = 1: a unit is one tile.  CL = 2: a unit is a 256-row PAIR tile made of two vertically adjacent 128-row tiles
 // (m_blk = 2*pair + rank, same n_blk).  The odd tail tile of a problem is a phantom whose rows are all out of range.
 template <int CL, bool SPLIT>
-__device__ __forceinline__ bool decode_tile(const GemmGroup& g, int bn, int t, int rank, TileInfo& ti) {
+__host__ __device__ __forceinline__ bool decode_tile(const GemmGroup& g, int bn, int t, int rank, TileInfo& ti) {
   for (int p = 0; p < g.num; ++p) {
     const GemmProblem& pr = g.p[p];
     const int tm_real = (pr.M + GEMM_BM - 1) / GEMM_BM;
@@ -69,9 +70,9 @@ __device__ __forceinline__ bool decode_tile(const GemmGroup& g, int bn, int t, i
       ti.m_blk = (rest % tm) * CL + rank;
       ti.split = rest / tm;
       const int total_kb = pr.taps * pr.kblk_per_tap * (SPLIT ? 3 : 1);
-      const int per = (total_kb + pr.ksplit - 1) / pr.ksplit;
+      const int per = gemm_unit_kblocks(pr, SPLIT);
       ti.kb0 = ti.split * per;
-      ti.kb1 = min(total_kb, ti.kb0 + per);
+      ti.kb1 = total_kb < ti.kb0 + per ? total_kb : ti.kb0 + per;
       return true;
     }
     t -= cnt;
@@ -398,8 +399,7 @@ __device__ __forceinline__ void epi_step(const GemmProblem& pr, const EpiRow& r,
 // ---- one consumer warpgroup: every tile of its schedule at tile width BN ----
 // Each width has its own accumulator array, k-loops and epilogue read-out; the kernel picks the width once, before the first tile.
 template <int CL, bool FULL, bool SPLIT, int BN>
-__device__ __forceinline__ void consumer_tiles(const GemmGroup& g, Ring& ring, float* epi_buf, int tile0, int tstep, int crank, int cw,
-                                               int lane) {
+__device__ __forceinline__ void consumer_tiles(const GemmGroup& g, Ring& ring, float* epi_buf, int crank, int cw, int lane) {
   using Cfg = GemmCfg<CL>;
   const int tid = threadIdx.x & 127;
   const int fr = 16 * (tid >> 5) + (lane >> 2);  // accumulator fragment: rows fr, fr + 8; columns 8 i + fc, + 1
@@ -412,7 +412,8 @@ __device__ __forceinline__ void consumer_tiles(const GemmGroup& g, Ring& ring, f
   for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
   TileInfo ti;
   bool first_tile = true;
-  for (int t = tile0; decode_tile<CL, SPLIT>(g, BN, t, crank, ti); t += tstep) {
+  // the CTA's place in the deal is re-read from blockIdx / gridDim rather than kept in registers across the tile
+  for (int rnd = 0; decode_tile<CL, SPLIT>(g, BN, gemm_deal_unit(gridDim.x / CL, blockIdx.x / CL, rnd), crank, ti); ++rnd) {
     const GemmProblem& pr = g.p[ti.p];
     const int bf = pr.a_fmt < 0 ? fmt : pr.a_fmt;  // both operands share it (checked on the host)
     if (first_tile && g.dbg != nullptr && ti.kb0 < ti.kb1) {
@@ -497,8 +498,6 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_wgmma_kernel(const __gri
   const int kStageBytes = Cfg::stage_bytes(BN);
   const int kStages = Cfg::num_stages(BN);
   const int crank = (CL > 1) ? (int)cluster_ctarank() : 0;  // rank inside the cluster
-  const int tile0 = (CL > 1) ? (int)(blockIdx.x / CL) : (int)blockIdx.x;
-  const int tstep = (int)(gridDim.x / CL);
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   const uint32_t raw_addr = smem_u32(smem_raw);
   const uint32_t align_off = (1024u - (raw_addr & 1023u)) & 1023u;  // 0 when the runtime honours the 1024 B alignment
@@ -543,7 +542,7 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_wgmma_kernel(const __gri
       int stage = 0;
       uint32_t phase = 0;
       TileInfo ti;
-      for (int t = tile0; decode_tile<CL, SPLIT>(g, BN, t, crank, ti); t += tstep) {
+      for (int r = 0; decode_tile<CL, SPLIT>(g, BN, gemm_deal_unit(gridDim.x / CL, blockIdx.x / CL, r), crank, ti); ++r) {
         const GemmProblem& pr = g.p[ti.p];
         const int m0 = ti.m_blk * GEMM_BM;
         const int n0 = ti.n_blk * BN;
@@ -607,9 +606,9 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_wgmma_kernel(const __gri
     Ring ring{stage_base, full_bar, empty_bar, kStageBytes, kStages, 0, 0u};
     switch (BN >> 4) {
 #define UV_BN_CASE(k) \
-  case k: consumer_tiles<CL, FULL, SPLIT, 16 * k>(g, ring, epi_buf, tile0, tstep, crank, wg, lane); break;
+  case k: consumer_tiles<CL, FULL, SPLIT, 16 * k>(g, ring, epi_buf, crank, wg, lane); break;
 #define UV_BN_CASE_ODD(k) \
-  case k: if constexpr (CL == 1) consumer_tiles<CL, FULL, SPLIT, 16 * k>(g, ring, epi_buf, tile0, tstep, crank, wg, lane); break;
+  case k: if constexpr (CL == 1) consumer_tiles<CL, FULL, SPLIT, 16 * k>(g, ring, epi_buf, crank, wg, lane); break;
       UV_BN_CASE(2) UV_BN_CASE_ODD(3) UV_BN_CASE(4) UV_BN_CASE_ODD(5) UV_BN_CASE(6) UV_BN_CASE_ODD(7) UV_BN_CASE(8)
       UV_BN_CASE_ODD(9) UV_BN_CASE(10) UV_BN_CASE_ODD(11) UV_BN_CASE(12) UV_BN_CASE_ODD(13) UV_BN_CASE(14) UV_BN_CASE_ODD(15)
       UV_BN_CASE(16)
@@ -874,15 +873,17 @@ int launch_gemm_group(GemmGroup& g, int bn, int num_sms, cudaStream_t stream, in
   if (used_full) *used_full = full ? 1 : 0;
   g.bn = bn;
   g.dbg = g_timeline;
+  GemmGroup gl = g;  // the launched copy, problems in deal order (the caller's order stays as it was)
+  gemm_deal_order(gl, nullptr);
   cudaError_t e;
   if (cl == 1) {
     const int grid = total < num_sms ? total : num_sms;
     if (g.split) {
-      launch_k(gemm_wgmma_kernel<1, false, true>, dim3(grid), dim3(kGemmThreads), Cfg::kSmemBytes, stream, g);
+      launch_k(gemm_wgmma_kernel<1, false, true>, dim3(grid), dim3(kGemmThreads), Cfg::kSmemBytes, stream, gl);
     } else if (full) {
-      launch_k(gemm_wgmma_kernel<1, true>, dim3(grid), dim3(kGemmThreads), Cfg::kSmemBytes, stream, g);
+      launch_k(gemm_wgmma_kernel<1, true>, dim3(grid), dim3(kGemmThreads), Cfg::kSmemBytes, stream, gl);
     } else {
-      launch_k(gemm_wgmma_kernel<1, false>, dim3(grid), dim3(kGemmThreads), Cfg::kSmemBytes, stream, g);
+      launch_k(gemm_wgmma_kernel<1, false>, dim3(grid), dim3(kGemmThreads), Cfg::kSmemBytes, stream, gl);
     }
     e = cudaGetLastError();
   } else {
@@ -904,7 +905,7 @@ int launch_gemm_group(GemmGroup& g, int bn, int num_sms, cudaStream_t stream, in
     cfg.attrs = attr;
     cfg.numAttrs = pdl_enabled() ? 2 : 1;
     ++*launch_counter();
-    e = full ? cudaLaunchKernelEx(&cfg, gemm_wgmma_kernel<2, true>, g) : cudaLaunchKernelEx(&cfg, gemm_wgmma_kernel<2, false>, g);
+    e = full ? cudaLaunchKernelEx(&cfg, gemm_wgmma_kernel<2, true>, gl) : cudaLaunchKernelEx(&cfg, gemm_wgmma_kernel<2, false>, gl);
   }
   if (e != cudaSuccess) {
     set_error("gemm launch failed: %s", cudaGetErrorString(e));
@@ -913,42 +914,152 @@ int launch_gemm_group(GemmGroup& g, int bn, int num_sms, cudaStream_t stream, in
   return 0;
 }
 
-// Tile width (and split-K factor) that minimise the modelled time of one grouped launch on H100.  The constants are a model,
-// not a measurement: a 64-wide k-block of a 128 x bn tile is 128 * bn * 64 multiply-adds at the data-sheet dense fp16 rate of one
-// SM (989 TFLOP/s over 132 SMs, ~0.0018 us per tile column) plus ~0.15 us of TMA / barrier overhead, ~1 us from kernel entry
-// to the first MMA, and an epilogue of ~0.5 us + 2 us x bn/256 (3 us x bn/256 with split-K reductions), of which only a
-// fraction is exposed when a CTA has further tiles to run.
-//   kblocks[p] = 64-wide k-blocks of problem p (taps included); max_split = 1 disables split-K.
-TileChoice choose_tile(const int* Ms, const int* Ns, const int* kblocks, int num, int num_sms, int step, int max_split) {
-  TileChoice best{256, 1};
-  double best_t = -1.0;
-  for (int ks = 1; ks <= max_split; ks *= 2) {
-    bool ok = true;
-    for (int p = 0; p < num; ++p) ok = ok && (ks == 1 || ks * 4 <= kblocks[p]);
-    if (!ok) break;
-    for (int bn = 256; bn >= 64; bn -= step) {
-      // persistent CTAs take whole tiles round-robin (tile t -> CTA t % sms, problems in order): k-blocks of the busiest CTA
-      long tiles = 0;
-      long load[256];
-      const int ncta = num_sms < 256 ? num_sms : 256;
-      for (int i = 0; i < ncta; ++i) load[i] = 0;
-      for (int p = 0; p < num; ++p) {
-        const long t = (long)((Ms[p] + GEMM_BM - 1) / GEMM_BM) * ((Ns[p] + bn - 1) / bn) * ks;
-        const int kb = (kblocks[p] + ks - 1) / ks;
-        for (long i = 0; i < t; ++i) load[(tiles + i) % ncta] += kb;
-        tiles += t;
-      }
-      long kb_cta = 0;
-      for (int i = 0; i < ncta; ++i) kb_cta = load[i] > kb_cta ? load[i] : kb_cta;
-      const long rounds = (tiles + ncta - 1) / ncta;
-      const double epi = 0.5 + bn * (ks > 1 ? 3.0 : 2.0) / 256.0;
-      const double t = 1.0 + (0.15 + 0.0018 * bn) * (double)kb_cta + epi * (1.0 + 0.3 * (double)(rounds - 1));
-      if (best_t < 0 || t < best_t - 1e-9) {
-        best_t = t;
-        best = TileChoice{bn, ks};
-      }
+void gemm_deal_order(GemmGroup& g, int* perm) {
+  const bool split = g.split != 0;
+  int order[GEMM_MAX_GROUP];
+  for (int p = 0; p < g.num; ++p) {  // stable insertion: equal units keep the problem order
+    const int kb = gemm_unit_kblocks(g.p[p], split);
+    int i = p;
+    for (; i > 0 && gemm_unit_kblocks(g.p[order[i - 1]], split) < kb; --i) order[i] = order[i - 1];
+    order[i] = p;
+  }
+  GemmProblem sorted[GEMM_MAX_GROUP];
+  for (int i = 0; i < g.num; ++i) sorted[i] = g.p[order[i]];
+  for (int i = 0; i < g.num; ++i) {
+    g.p[i] = sorted[i];
+    if (perm) perm[i] = order[i];
+  }
+}
+
+// The scheduling fields of a launch of problems M x N x (kblocks 64-wide k-blocks), split ks ways (CL = 1, plain taps).
+static void deal_group(GemmGroup& g, const int* Ms, const int* Ns, const int* kblocks, const int* ks, int num, int* perm = nullptr) {
+  memset(&g, 0, sizeof(g));
+  g.num = num;
+  for (int p = 0; p < num; ++p) {
+    g.p[p].M = Ms[p];
+    g.p[p].N = Ns[p];
+    g.p[p].taps = 1;
+    g.p[p].kblk_per_tap = kblocks[p];
+    g.p[p].ksplit = ks[p];
+  }
+  gemm_deal_order(g, perm);
+}
+
+static int deal_units(const GemmGroup& g, int bn) {
+  int total = 0;
+  for (int p = 0; p < g.num; ++p) total += ((g.p[p].M + GEMM_BM - 1) / GEMM_BM) * ((g.p[p].N + bn - 1) / bn) * g.p[p].ksplit;
+  return total;
+}
+
+int gemm_deal_ctas(const int* Ms, const int* Ns, const int* kblocks, const int* ksplit, int num, int num_sms, int bn, int* cta, int cap) {
+  if (num < 1 || num > GEMM_MAX_GROUP || num_sms < 1 || bn < 16) return -1;
+  for (int p = 0; p < num; ++p)
+    if (Ms[p] < 1 || Ns[p] < 1 || kblocks[p] < 1 || ksplit[p] < 1 || ksplit[p] > kblocks[p]) return -1;
+  GemmGroup g;
+  int perm[GEMM_MAX_GROUP];  // deal position -> problem
+  deal_group(g, Ms, Ns, kblocks, ksplit, num, perm);
+  const int total = deal_units(g, bn);
+  int first[GEMM_MAX_GROUP];  // index of problem p's first unit in `cta` (problem order)
+  for (int p = 0, u = 0; p < num; ++p) {
+    first[p] = u;
+    u += ((Ms[p] + GEMM_BM - 1) / GEMM_BM) * ((Ns[p] + bn - 1) / bn) * ksplit[p];
+  }
+  for (int u = 0; u < total && u < cap; ++u) cta[u] = -1;
+  const int n = total < num_sms ? total : num_sms;  // the grid launch_gemm_group runs
+  for (int c = 0; c < n; ++c) {
+    TileInfo ti;
+    for (int r = 0; decode_tile<1, false>(g, bn, gemm_deal_unit(n, c, r), 0, ti); ++r) {
+      const int p = perm[ti.p];
+      const int tm = (Ms[p] + GEMM_BM - 1) / GEMM_BM, tn = (Ns[p] + bn - 1) / bn;
+      const int u = first[p] + (ti.split * tm + ti.m_blk) * tn + ti.n_blk;
+      if (u < cap) cta[u] = cta[u] == -1 ? c : -2;
     }
   }
+  return total;
+}
+
+// Modelled time (us) of one launch: the busiest CTA of the deal that the kernel runs.  The constants are a model, not a
+// measurement: a 64-wide k-block of a 128 x bn tile is 128 * bn * 64 multiply-adds at the data-sheet dense fp16 rate of one SM
+// (989 TFLOP/s over 132 SMs, ~0.0018 us per tile column) plus ~0.15 us of TMA / barrier overhead, ~1 us from kernel entry to
+// the first MMA, and per unit an epilogue of ~0.5 us + 2 us x bn/256 (3 us x bn/256 for a split-K unit, which reduces into its
+// output), of which only a fraction is exposed when the CTA has further units to run.
+static double model_launch_us(const GemmGroup& g, int bn, int num_sms) {
+  const int total = deal_units(g, bn);
+  const int n = total < num_sms ? total : num_sms;
+  const double kb_us = 0.15 + 0.0018 * bn;
+  double worst = 0.0;
+  for (int c = 0; c < n; ++c) {
+    double busy = 0.0, last_epi = 0.0;
+    TileInfo ti;
+    for (int r = 0; decode_tile<1, false>(g, bn, gemm_deal_unit(n, c, r), 0, ti); ++r) {
+      last_epi = 0.5 + bn * (g.p[ti.p].ksplit > 1 ? 3.0 : 2.0) / 256.0;
+      busy += kb_us * (double)(ti.kb1 - ti.kb0) + 0.3 * last_epi;
+    }
+    busy += 0.7 * last_epi;
+    worst = busy > worst ? busy : worst;
+  }
+  return 1.0 + worst;
+}
+
+// Every combination of per-problem split factors (powers of two up to max_split[p], at least 4 k-blocks per split) at every
+// width; ties keep the smaller splits and the wider tile.  The plan asks the same questions every step: a small cache of
+// answers keeps the search off the host's launch path.
+struct TileQuery {
+  int Ms[GEMM_MAX_GROUP], Ns[GEMM_MAX_GROUP], kb[GEMM_MAX_GROUP], max_split[GEMM_MAX_GROUP];
+  int num, num_sms, step;
+};
+TileChoice choose_tile(const int* Ms, const int* Ns, const int* kblocks, const int* max_split, int num, int num_sms, int step) {
+  TileQuery q;
+  memset(&q, 0, sizeof(q));
+  for (int p = 0; p < num; ++p) {
+    q.Ms[p] = Ms[p];
+    q.Ns[p] = Ns[p];
+    q.kb[p] = kblocks[p];
+    q.max_split[p] = max_split[p];
+  }
+  q.num = num;
+  q.num_sms = num_sms;
+  q.step = step;
+  constexpr int kCache = 32;
+  static thread_local TileQuery cq[kCache];
+  static thread_local TileChoice ca[kCache];
+  static thread_local int cn = 0;
+  for (int i = 0; i < cn && i < kCache; ++i)
+    if (memcmp(&cq[i], &q, sizeof(q)) == 0) return ca[i];
+
+  TileChoice best;
+  memset(&best, 0, sizeof(best));
+  double best_t = -1.0;
+  int ks[GEMM_MAX_GROUP];
+  for (int p = 0; p < num; ++p) ks[p] = 1;
+  GemmGroup g;
+  for (;;) {
+    deal_group(g, Ms, Ns, kblocks, ks, num);
+    for (int bn = 256; bn >= 64; bn -= step) {
+      const double t = model_launch_us(g, bn, num_sms);
+      if (best_t < 0 || t < best_t - 1e-9) {
+        best_t = t;
+        best.bn = bn;
+        best.ksplit = 1;
+        for (int p = 0; p < GEMM_MAX_GROUP; ++p) {
+          best.ks[p] = p < num ? ks[p] : 1;
+          best.ksplit = best.ks[p] > best.ksplit ? best.ks[p] : best.ksplit;
+        }
+      }
+    }
+    int p = 0;  // next combination (mixed radix, problem 0 fastest)
+    for (; p < num; ++p) {
+      if (ks[p] * 2 <= max_split[p] && ks[p] * 2 * 4 <= kblocks[p]) {
+        ks[p] *= 2;
+        break;
+      }
+      ks[p] = 1;
+    }
+    if (p == num) break;
+  }
+  cq[cn % kCache] = q;
+  ca[cn % kCache] = best;
+  ++cn;
   return best;
 }
 

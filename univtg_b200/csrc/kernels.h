@@ -96,14 +96,35 @@ struct GemmGroup {
   GemmProblem p[GEMM_MAX_GROUP];
 };
 
+// ---- static deal of a launch's work units over its persistent CTAs ----
+// A unit is one output tile (CL = 2: tile pair) of one k-split of one problem.  Units are numbered longest first: problems in
+// deal order (k-blocks per unit descending, ties in problem order; launch_gemm_group launches the problems so ordered), a
+// problem's units in tile order.  They are dealt in waves of one unit per CTA whose direction alternates (a snake): the CTA
+// that draws the longest unit of one wave draws the shortest of the next.  Round r of CTA c (of n) runs unit gemm_deal_unit(n, c, r); every unit is run exactly once.
+__host__ __device__ __forceinline__ int gemm_deal_unit(int n, int c, int r) { return r * n + ((r & 1) ? n - 1 - c : c); }
+// k-blocks of one unit of problem `pr` (its last split may be shorter); split: fp16x3 walks every k-block three times.
+__host__ __device__ __forceinline__ int gemm_unit_kblocks(const GemmProblem& pr, bool split) {
+  const int total_kb = pr.taps * pr.kblk_per_tap * (split ? 3 : 1);
+  return (total_kb + pr.ksplit - 1) / pr.ksplit;
+}
+// Puts g's problems in deal order; perm (optional) receives the original index of each.
+void gemm_deal_order(GemmGroup& g, int* perm);
+
 // bn: tile width, multiple of 16 in [32, 256] (multiple of 64 when a problem has an MN-major B).  A and B of a problem must share
 // one 16-bit format.  Returns cudaError_t as int.  used_full (optional): 1 when the FULL epilogue variant was launched, 0 for the lean one.
 int launch_gemm_group(GemmGroup& g, int bn, int num_sms, cudaStream_t stream, int* used_full = nullptr);
-// Tile width minimising waves x tile-time for problems that share a launch (step 16: K-major B, 64: MN-major B).
+// Tile width and per-problem split-K factors that minimise the modelled time of problems sharing one launch (step 16: K-major B,
+// 64: MN-major B).  max_split[p] (a power of two): split limit of problem p, 1 for a problem whose epilogue cannot accumulate.
 struct TileChoice {
-  int bn, ksplit;
+  int bn;
+  int ksplit;                  // the largest of ks
+  int ks[GEMM_MAX_GROUP];      // split-K factor of each problem
 };
-TileChoice choose_tile(const int* Ms, const int* Ns, const int* kblocks, int num, int num_sms, int step, int max_split);
+TileChoice choose_tile(const int* Ms, const int* Ns, const int* kblocks, const int* max_split, int num, int num_sms, int step);
+// The deal of gemm_wgmma_kernel (CL = 1) for problems M x N with kblocks k-blocks split ksplit ways at width bn: cta[u] receives the
+// CTA that runs unit u (units problem by problem, in each problem's tile order; -1 if no CTA runs it, -2 if two do).  Returns the
+// number of units (also when it exceeds cap, in which case nothing past cap is written), or -1 for bad arguments.
+int gemm_deal_ctas(const int* Ms, const int* Ns, const int* kblocks, const int* ksplit, int num, int num_sms, int bn, int* cta, int cap);
 // MN-major B operand [rows = K, cols = N] (N contiguous): a 3-D view {64, K, N/64} lets one TMA instruction fetch the whole
 // 64 x bn tile of a k-block (fewer TMA operations per k-block than one 2-D box per 64-wide block); needs cols % 64 == 0.
 int make_tmap_b_mn(GemmProblem& p, const void* base, uint64_t rows, uint64_t cols, uint64_t ld_elems, int bn);

@@ -593,15 +593,25 @@ inline int setup_linear(GemmProblem& p, const uint16_t* A, int M, int K, int lda
   return setup_gemm(p, Mat16{A, M, K, lda}, 0, Mat16{W, N, K, ldw}, 0, M, N, K, bn, lo_a, lo_w);
 }
 
-// Tile width + split-K factor for one grouped launch (cost model: choose_tile, gemm.cu).  K in elements; step 16 when every B
-// operand is K-major, 64 when one is MN-major; max_split = 1 for launches whose epilogue cannot accumulate.
+// Tile width + split-K factors for one grouped launch (cost model: choose_tile, gemm.cu).  K in elements; step 16 when every B
+// operand is K-major, 64 when one is MN-major; split: split-K limit of the problem (1, the default, for a problem whose epilogue
+// cannot accumulate).
 struct MNK {
   int M, N, K;
+  int split = 1;
 };
-inline TileChoice tile_for(int sms, int step, int max_split, MNK a, MNK b = MNK{0, 0, 0}, MNK c3 = MNK{0, 0, 0}) {
-  const int Ms[3] = {a.M, b.M, c3.M}, Ns[3] = {a.N, b.N, c3.N}, kb[3] = {(a.K + 63) / 64, (b.K + 63) / 64, (c3.K + 63) / 64};
-  const int num = c3.M > 0 ? 3 : (b.M > 0 ? 2 : 1);
-  return choose_tile(Ms, Ns, kb, num, sms, step, max_split);
+inline TileChoice tile_for(int sms, int step, MNK a, MNK b = MNK{0, 0, 0}, MNK c3 = MNK{0, 0, 0}, MNK c4 = MNK{0, 0, 0}) {
+  const MNK all[GEMM_MAX_GROUP] = {a, b, c3, c4};
+  int Ms[GEMM_MAX_GROUP], Ns[GEMM_MAX_GROUP], kb[GEMM_MAX_GROUP], ms[GEMM_MAX_GROUP], num = 0;
+  for (const MNK& x : all) {
+    if (x.M <= 0) break;
+    Ms[num] = x.M;
+    Ns[num] = x.N;
+    kb[num] = (x.K + 63) / 64;
+    ms[num] = x.split;
+    ++num;
+  }
+  return choose_tile(Ms, Ns, kb, ms, num, sms, step);
 }
 
 // Inference workspace: one buffer per role, shared by all layers; LayerNorm 1 works in place on the residual stream.

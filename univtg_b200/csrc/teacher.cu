@@ -467,8 +467,8 @@ extern "C" int univtg_teacher_label(const float* cls, const void* cls_ws, int32_
   int dev = 0, sms = 0;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  const int32_t Ms[1] = {V}, Ns[1] = {Cp}, kb[1] = {Dp / 64};
-  const TileChoice tc = choose_tile(Ms, Ns, kb, 1, sms, 16, 1);
+  const int32_t Ms[1] = {V}, Ns[1] = {Cp}, kb[1] = {Dp / 64}, no_split[1] = {1};
+  const TileChoice tc = choose_tile(Ms, Ns, kb, no_split, 1, sms, 16);
   int rc = univtg_op_gemm(w.planes, cw.planes, V, Cp, Dp, 0, 0, 2, tc.bn, 1, nullptr, 0, 1.0f, w.approx, nullptr, stream);
   if (rc) return rc;
   launch_k(candidates_kernel, dim3(V), dim3(kThreads), 0, st, (const float*)w.approx, (int)C, Cp, w.cand, w.next);

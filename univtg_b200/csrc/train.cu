@@ -279,17 +279,17 @@ int univtg_backward(univtg_plan* P, void* ws, const float* src_txt, const float*
                           int Cin, int bnn) -> int { return conv_dgrad_problem(p, Mh, dY, ldy, Kc, Wp, Cin, bnn); };
     // wgrad of one tap, written as a tap-major plane of T.wtap (launch_tap_interleave then builds the [N, C, 3] layout with 256-bit
     // stores here instead of stride-3 scalars)
-    const TileChoice t_cw = tile_for(sms, 64, 8, MNK{d, d, Mh}, MNK{d, d, Mh}, MNK{d, d, Mh});
+    const TileChoice t_cw = tile_for(sms, 64, MNK{d, d, Mh, 8}, MNK{d, d, Mh, 8}, MNK{d, d, Mh, 8});
     auto conv_wgrad = [&](GemmProblem& p, const uint16_t* dY, int ldy, int Nc, const uint16_t* X, int ldx, int Cin, int t) -> int {
       const int r = conv_wgrad_problem(p, Mh, dY, ldy, Nc, X, ldx, Cin, t, t_cw.bn);
       p.out32 = T.wtap + (size_t)t * Nc * Cin;
       p.ld32 = Cin;
       p.alpha = INV;
-      p.ksplit = t_cw.ksplit;
+      p.ksplit = t_cw.ks[t];
       return r;
     };
-    const int bn_c2d = tile_for(sms, 64, 1, MNK{Mh, d, 3 * d}, MNK{Mh, d, 3 * d}).bn;
-    const int bn_c1d = tile_for(sms, 64, 1, MNK{Mh, d, 6 * d}).bn;
+    const int bn_c2d = tile_for(sms, 64, MNK{Mh, d, 3 * d}, MNK{Mh, d, 3 * d}).bn;
+    const int bn_c1d = tile_for(sms, 64, MNK{Mh, d, 6 * d}).bn;
     // (splitting the k-blocks of the layer-1 dgrad - 76 tiles of 96 k-blocks - over idle SMs saves ~8 us but reduces into the stream
     // gradient with atomics, which makes every gradient upstream of the heads order-dependent in its last bits: not taken)
     // ---- conv layer 2 (two heads): dgrad -> dh1 [Mh+2, 2d] (class cols [0,d), span cols [d,2d)), ReLU mask of h1 ----
@@ -400,22 +400,27 @@ int univtg_backward(univtg_plan* P, void* ws, const float* src_txt, const float*
     a.pgrad_scale = INV;
     return launch_layernorm_bwd(a, st);
   };
+  // Each data gradient shares one launch with the weight gradients that read the same gradient operand.  A d-wide data gradient
+  // is a single wave that leaves SMs idle, and a weight gradient is a few long output tiles: dealt together longest first, the
+  // weight gradients' units fill the SMs the data gradient leaves, with fewer split-K reductions (choose_tile picks each weight
+  // gradient's split), and the launch ramps and tails of separate launches go away (DESIGN §5.1).  Every operand of a launch is
+  // complete when it starts; no buffer is written by one problem of a launch and read or written by another.
+  const TileChoice t_f2 = tile_for(sms, 64, MNK{M, ff, d}, MNK{d, ff, M, 4});  // FFN2 dgrad + linear2.weight
+  const TileChoice t_f1 = tile_for(sms, 64, MNK{M, d, ff}, MNK{ff, d, M, 4});  // FFN1 dgrad + linear1.weight
+  const TileChoice t_o = tile_for(sms, 64, MNK{M, d, d}, MNK{d, d, M, 4});     // out-proj dgrad + out_proj.weight
+  // QKV dgrad (+ text-position dgrad) + the q|k and v rows of in_proj_weight
+  const TileChoice t_q = txt_pos ? tile_for(sms, 64, MNK{M, d, 3 * d}, MNK{Mt, d, 2 * d}, MNK{2 * d, d, M, 4}, MNK{d, d, M, 4})
+                                 : tile_for(sms, 64, MNK{M, d, 3 * d}, MNK{2 * d, d, M, 4}, MNK{d, d, M, 4});
   for (int l = c.enc_layers - 1; l >= 0; --l) {
     const LayerPacked& lp = Lw.layer[l];
     const float* s1 = droppath_scale ? droppath_scale + (size_t)(2 * l) * B : nullptr;
     const float* s2 = droppath_scale ? droppath_scale + (size_t)(2 * l + 1) * B : nullptr;
-    const int bn_dff = tile_for(sms, 64, 1, MNK{M, ff, d}).bn, bn_dd1 = tile_for(sms, 64, 1, MNK{M, d, ff}).bn,
-              bn_ddo = tile_for(sms, 64, 1, MNK{M, d, d}).bn, bn_ddq = tile_for(sms, 64, 1, MNK{M, d, 3 * d}).bn;
-    const TileChoice t_wo = tile_for(sms, 64, 16, MNK{d, d, M}), t_wq = tile_for(sms, 64, 16, MNK{2 * d, d, M}, MNK{d, d, M}),
-                     t_wf = tile_for(sms, 64, 16, MNK{d, ff, M}, MNK{ff, d, M});
     // ---- LN2 backward: dx (grad of the layer output) -> dy (grad of x1 + s2 * F), branch operand s2 * dy ----
     rc = ln_bwd(T.y2[l], T.mean2[l], T.rstd2[l], F32(lp.n2w), s2, grads[ix.layer(l, 10)], grads[ix.layer(l, 11)],
                 grads[ix.layer(l, 7)]);  // linear2.bias
     if (rc) return rc;
     // ---- FFN2: dgrad -> d(hpre) = (dF W2) * gelu'(hpre) (saved 16-bit derivative);  wgrad dW2 = dF^T h ----
     // ---- FFN1: dgrad d(x1) = dhpre W1 + dy (residual);          wgrad dW1 = dhpre^T x1 ----
-    // (the data-gradient and weight-gradient GEMMs that read the same dY are separate launches chained by programmatic
-    //  dependent launch; sharing one launch was slower per step on the earlier GPU generation and has not been re-measured)
     auto ffn2_dgrad = [&](GemmProblem& p, int bnn) -> int {
       int r = setup_gemm(p, Mat16{T.dbr16, M, d, d}, 0, Mat16{W16(lp.w2), d, ff, ff}, 1, M, ff, d, bnn);
       p.mask16 = T.dgelu16[l];  // d(hpre) = (dF W2) * GELU'(hpre), the derivative saved by the forward as a 16-bit operand
@@ -451,23 +456,19 @@ int univtg_backward(univtg_plan* P, void* ws, const float* src_txt, const float*
       p.ksplit = ks;
       return r;
     };
-    {
-      reset_group(g, 1, fmt);
-      rc = ffn2_dgrad(g.p[0], bn_dff);
-      if (rc) return rc;
-      rc = gemm_launch(P, g, bn_dff, sms, st);
-      if (rc) return rc;
-
+    {  // FFN2 launch: reads dbr16, W2, dgelu16, h16; writes dhpre16, linear1.bias (column sums), linear2.weight
       reset_group(g, 2, fmt);
-      rc |= ffn2_wgrad(g.p[0], t_wf.bn, t_wf.ksplit);
-      rc |= ffn1_wgrad(g.p[1], t_wf.bn, t_wf.ksplit);
+      rc |= ffn2_dgrad(g.p[0], t_f2.bn);
+      rc |= ffn2_wgrad(g.p[1], t_f2.bn, t_f2.ks[1]);
       if (rc) return rc;
-      rc = gemm_launch(P, g, t_wf.bn, sms, st);
+      rc = gemm_launch(P, g, t_f2.bn, sms, st);
       if (rc) return rc;
-      reset_group(g, 1, fmt);
-      rc = ffn1_dgrad(g.p[0], bn_dd1);
+      // FFN1 launch: reads dhpre16, W1, dy, x1_16; writes dx, linear1.weight
+      reset_group(g, 2, fmt);
+      rc |= ffn1_dgrad(g.p[0], t_f1.bn);
+      rc |= ffn1_wgrad(g.p[1], t_f1.bn, t_f1.ks[1]);
       if (rc) return rc;
-      rc = gemm_launch(P, g, bn_dd1, sms, st);
+      rc = gemm_launch(P, g, t_f1.bn, sms, st);
       if (rc) return rc;
     }
     // ---- LN1 backward ----
@@ -489,16 +490,12 @@ int univtg_backward(univtg_plan* P, void* ws, const float* src_txt, const float*
       p.ksplit = ks;
       return r;
     };
-    {
-      reset_group(g, 1, fmt);
-      rc = out_dgrad(g.p[0], bn_ddo);
+    {  // reads dbr16, W_out, attn16; writes dO16, out_proj.weight
+      reset_group(g, 2, fmt);
+      rc |= out_dgrad(g.p[0], t_o.bn);
+      rc |= out_wgrad(g.p[1], t_o.bn, t_o.ks[1]);
       if (rc) return rc;
-      rc = gemm_launch(P, g, bn_ddo, sms, st);
-      if (rc) return rc;
-      reset_group(g, 1, fmt);
-      rc = out_wgrad(g.p[0], t_wo.bn, t_wo.ksplit);
-      if (rc) return rc;
-      rc = gemm_launch(P, g, t_wo.bn, sms, st);
+      rc = gemm_launch(P, g, t_o.bn, sms, st);
       if (rc) return rc;
     }
     // ---- attention core backward -> dqkv32 -> dqkv16 (+ in_proj_bias gradient) ----
@@ -527,7 +524,7 @@ int univtg_backward(univtg_plan* P, void* ws, const float* src_txt, const float*
       p.ld32 = d;
       return r;
     };
-    auto qkv_wgrads = [&](GemmProblem& pqk, GemmProblem& pv, int bnn, int ks) -> int {
+    auto qkv_wgrads = [&](GemmProblem& pqk, GemmProblem& pv, int bnn, int ks_qk, int ks_v) -> int {
       int r = setup_gemm(pqk, Mat16{T.dqkv16, M, 2 * d, 3 * d}, 1, Mat16{T.xpos16[l], M, d, d}, 1, 2 * d, d, M, bnn);
       r |= setup_gemm(pv, Mat16{T.dqkv16 + 2 * d, M, d, 3 * d}, 1, Mat16{T.xin16[l], M, d, d}, 1, d, d, M, bnn);
       pqk.out32 = grads[ix.layer(l, 0)];
@@ -535,28 +532,28 @@ int univtg_backward(univtg_plan* P, void* ws, const float* src_txt, const float*
       pv.out32 = grads[ix.layer(l, 0)] + (size_t)2 * d * d;
       pv.ld32 = d;
       pqk.alpha = pv.alpha = INV;
-      pqk.ksplit = pv.ksplit = ks;
+      pqk.ksplit = ks_qk;
+      pv.ksplit = ks_v;
       return r;
     };
-    {
-      reset_group(g, txt_pos ? 2 : 1, fmt);
-      rc = qkv_dgrad(g.p[0], bn_ddq);
+    {  // reads dqkv16, W_in, dy, xpos16, xin16 (text positions: dqk16, and dpos in its own problem's epilogue); writes dx,
+       // in_proj_weight (text positions: dpos)
+      const int w = txt_pos ? 2 : 1;  // first weight-gradient problem (order of t_q's problems)
+      reset_group(g, w + 2, fmt);
+      rc = qkv_dgrad(g.p[0], t_q.bn);
       if (rc) return rc;
       if (txt_pos) {  // d(pos_t) += [dq | dk] [Wq; Wk] over the text rows (the first layer differentiated overwrites)
         GemmProblem& p = g.p[1];
-        rc = setup_gemm(p, Mat16{TP.dqk16, Mt, 2 * d, 2 * d}, 0, Mat16{W16(lp.w_in), 2 * d, d, d}, 1, Mt, d, 2 * d, bn_ddq);
+        rc = setup_gemm(p, Mat16{TP.dqk16, Mt, 2 * d, 2 * d}, 0, Mat16{W16(lp.w_in), 2 * d, d, d}, 1, Mt, d, 2 * d, t_q.bn);
         if (rc) return rc;
         p.resid = l == c.enc_layers - 1 ? nullptr : TP.dpos;
         p.ld_resid = d;
         p.out32 = TP.dpos;
         p.ld32 = d;
       }
-      rc = gemm_launch(P, g, bn_ddq, sms, st);
+      rc = qkv_wgrads(g.p[w], g.p[w + 1], t_q.bn, t_q.ks[w], t_q.ks[w + 1]);
       if (rc) return rc;
-      reset_group(g, 2, fmt);
-      rc = qkv_wgrads(g.p[0], g.p[1], t_wq.bn, t_wq.ksplit);
-      if (rc) return rc;
-      rc = gemm_launch(P, g, t_wq.bn, sms, st);
+      rc = gemm_launch(P, g, t_q.bn, sms, st);
       if (rc) return rc;
     }
     stage_done(1 + (c.enc_layers - 1 - l));  // encoder layer l
@@ -599,24 +596,41 @@ int univtg_backward(univtg_plan* P, void* ws, const float* src_txt, const float*
   cudaMemcpyAsync(grads[ix.vid(np - 1, 3)], g_type + d, (size_t)d * 4, cudaMemcpyDeviceToDevice, st);
   cudaMemcpyAsync(grads[ix.txt(np - 1, 3)], g_type, (size_t)d * 4, cudaMemcpyDeviceToDevice, st);
   for (int i = np - 1; i >= 0; --i) {
-    // wgrad: dW_i = dOut^T a_i   (video + text in one launch)
-    reset_group(g, 2, fmt);
     const int kpv = Lw.vid[i].kpad, kpt = Lw.txt[i].kpad, dinv = Lw.vid[i].din, dint = Lw.txt[i].din;
     // a width like 2818 would force scalar epilogue stores: write rows padded to kpad with 256-bit stores, then a pitched copy
     const bool pad_v = (dinv % 8) != 0;
     const int nv = pad_v ? kpv : dinv;  // the operand a_vid[i] is zero beyond dinv
-    const TileChoice t_pw = tile_for(sms, 64, 16, MNK{d, nv, Mv}, MNK{d, dint, Mt});
-    const int bn_pd = tile_for(sms, 64, 1, MNK{Mv, kpv, d}, MNK{Mt, kpt, d}).bn;
+    // wgrad: dW_i = dOut^T a_i (video + text).  dgrad: dA_i = dOut W_i (fp32, [rows, kpad_i]: N is padded to the packed weight's
+    // K so the epilogue stays on its 128-bit path even for the 2818-wide video features; the padded columns are zeros).  The
+    // input-dropout mask is applied by the LayerNorm backward when it loads dA.  Layer 0's weight gradients end a gradient stage
+    // (the event below), so its data gradients follow in a launch of their own; a later layer's four problems share one launch
+    // (reads dxv16, dxt16, a_vid, a_txt and the packed weights; writes the weight gradients, T.wtap, dA_v and dA_t).
+    const bool merged = i > 0;
+    const TileChoice t_pw = merged ? tile_for(sms, 64, MNK{d, nv, Mv, 4}, MNK{d, dint, Mt, 4}, MNK{Mv, kpv, d}, MNK{Mt, kpt, d})
+                                   : tile_for(sms, 64, MNK{d, nv, Mv, 16}, MNK{d, dint, Mt, 16});
+    const int bn_pd = merged ? t_pw.bn : tile_for(sms, 64, MNK{Mv, kpv, d}, MNK{Mt, kpt, d}).bn;
+    auto proj_dgrads = [&](GemmProblem* p) -> int {
+      int r = setup_gemm(p[0], Mat16{T.dxv16, Mv, d, d}, 0, Mat16{W16(Lw.vid[i].w16), d, kpv, kpv}, 1, Mv, kpv, d, bn_pd);
+      r |= setup_gemm(p[1], Mat16{T.dxt16, Mt, d, d}, 0, Mat16{W16(Lw.txt[i].w16), d, kpt, kpt}, 1, Mt, kpt, d, bn_pd);
+      p[0].out32 = T.dA_v;
+      p[0].ld32 = kpv;
+      p[1].out32 = T.dA_t;
+      p[1].ld32 = kpt;
+      return r;
+    };
+    reset_group(g, merged ? 4 : 2, fmt);
     rc |= setup_gemm(g.p[0], Mat16{T.dxv16, Mv, d, d}, 1, Mat16{T.a_vid[i], Mv, kpv, kpv}, 1, d, nv, Mv, t_pw.bn);
     rc |= setup_gemm(g.p[1], Mat16{T.dxt16, Mt, d, d}, 1, Mat16{T.a_txt[i], Mt, kpt, kpt}, 1, d, dint, Mt, t_pw.bn);
+    if (merged) rc |= proj_dgrads(g.p + 2);
     if (rc) return rc;
     g.p[0].out32 = pad_v ? T.wtap : grads[ix.vid(i, 2)];
     g.p[0].ld32 = nv;
     g.p[1].out32 = grads[ix.txt(i, 2)];
     g.p[1].ld32 = dint;
     g.p[0].alpha = g.p[1].alpha = INV;
-    g.p[0].ksplit = g.p[1].ksplit = t_pw.ksplit;
-    if (pad_v && t_pw.ksplit > 1) cudaMemsetAsync(T.wtap, 0, (size_t)d * kpv * 4, st);  // split-K accumulates into the padded copy
+    g.p[0].ksplit = t_pw.ks[0];
+    g.p[1].ksplit = t_pw.ks[1];
+    if (pad_v && t_pw.ks[0] > 1) cudaMemsetAsync(T.wtap, 0, (size_t)d * kpv * 4, st);  // split-K accumulates into the padded copy
     rc = gemm_launch(P, g, t_pw.bn, sms, st);
     if (rc) return rc;
     if (pad_v)
@@ -625,19 +639,13 @@ int univtg_backward(univtg_plan* P, void* ws, const float* src_txt, const float*
     // every projector weight, the later layers' LayerNorm terms and all biases are final here; what follows only produces the
     // first layer's LayerNorm terms - the 11.5 MB video weight gradient need not wait for it to start its exchange
     if (i == 0) stage_done(c.enc_layers + 1);
-    // dgrad: dA_i = dOut W_i  (fp32, [rows, kpad_i]: N is padded to the packed weight's K so the epilogue stays on its
-    // 128-bit path even for the 2818-wide video features; the padded columns are zeros).  The input-dropout mask is applied
-    // by the LayerNorm backward when it loads dA.
-    reset_group(g, 2, fmt);
-    rc |= setup_gemm(g.p[0], Mat16{T.dxv16, Mv, d, d}, 0, Mat16{W16(Lw.vid[i].w16), d, kpv, kpv}, 1, Mv, kpv, d, bn_pd);
-    rc |= setup_gemm(g.p[1], Mat16{T.dxt16, Mt, d, d}, 0, Mat16{W16(Lw.txt[i].w16), d, kpt, kpt}, 1, Mt, kpt, d, bn_pd);
-    if (rc) return rc;
-    g.p[0].out32 = T.dA_v;
-    g.p[0].ld32 = kpv;
-    g.p[1].out32 = T.dA_t;
-    g.p[1].ld32 = kpt;
-    rc = gemm_launch(P, g, bn_pd, sms, st);
-    if (rc) return rc;
+    if (!merged) {
+      reset_group(g, 2, fmt);
+      rc = proj_dgrads(g.p);
+      if (rc) return rc;
+      rc = gemm_launch(P, g, bn_pd, sms, st);
+      if (rc) return rc;
+    }
     // LayerNorm_i backward: parameter gradients; for i > 0 also the gradient of the previous layer's ReLU output
     for (int s = 0; s < 2; ++s) {
       LnBwdArgs a;
