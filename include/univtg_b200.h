@@ -544,6 +544,18 @@ int univtg_eval_hl_topk(const float* scores, const int32_t* n_score, const int32
  * gets s = NaN, so the caller passes the largest side it packed. */
 int univtg_qfvs_match(const uint64_t* a, const int32_t* a_off, const uint64_t* b, const int32_t* b_off, int32_t Q,
                       int32_t max_side, double* s, void* stream);
+/* Selection step of the QFVS evaluation epoch (main/inference_qfvs.py eval_epoch) for F queries of one video, query f writing
+ * slot q0 + f of the pools.  The model outputs of the three query variants (concept 1, concept 2, both) are [F, N] f32 each,
+ * N = S*Lf, query f's S segments in rows f*S .. f*S+S-1.  pos [n]: the first n kept positions of mask_GT in row-major order
+ * (1 <= n <= min(N, 8192)).  Per kept position i the variant score is logits (mode 0), sal (mode 1) or (0 + logits) + sal
+ * (mode 2), and score[q, i] = score_both, or (score_both + score_1) + score_2 with gather = 1, in fp32.  top[q, 0..k) = the
+ * indices of score.topk(k) as torch.topk on CUDA returns them (descending, NaN first; equal scores by ascending index when
+ * k > 32, in the order of torch's unstable 32-wide bitonic sort of its selection when k <= 32; 1 <= k
+ * <= n), a[q, 0..k) = tags[top[q, j]] (the machine side of univtg_qfvs_match, offsets q*k).  Variants 1 and 2 are read only
+ * with gather = 1; logits only for modes 0 and 2, sal only for modes 1 and 2. */
+int univtg_qfvs_eval_select(const float* logits1, const float* sal1, const float* logits2, const float* sal2, const float* logits_o,
+                            const float* sal_o, const int32_t* pos, const uint64_t* tags, int32_t F, int32_t N, int32_t n, int32_t k,
+                            int32_t mode, int32_t gather, int32_t q0, float* score, int32_t* top, uint64_t* a, void* stream);
 
 /* LayerNorm rows: in [rows,d] f32 -> out32 [rows,d] f32 and/or out16 [rows,ld16] 16-bit (zero padded). */
 int univtg_op_layernorm(const float* in, int32_t rows, int32_t d, const float* gamma, const float* beta, float eps,

@@ -176,6 +176,7 @@ SIGNATURES = {
     "univtg_eval_hl": (c_int, [c_void_p] * 4 + [c_int, c_int, c_int] + [c_void_p] * 4),
     "univtg_eval_hl_topk": (c_int, [c_void_p] * 5 + [c_int] * 5 + [c_void_p, c_void_p]),
     "univtg_qfvs_match": (c_int, [c_void_p] * 4 + [c_int, c_int, c_void_p, c_void_p]),
+    "univtg_qfvs_eval_select": (c_int, [c_void_p] * 8 + [c_int] * 7 + [c_void_p] * 4),
     "univtg_adamw_step": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, ctypes.c_size_t, c_float, c_float, c_float, c_float,
                                   c_float, c_int, c_float, c_int, c_void_p, ctypes.POINTER(Config), c_void_p, c_void_p]),
     "univtg_pack_vectors": (c_int, [ctypes.POINTER(Config), ctypes.POINTER(c_void_p), c_int, c_void_p, c_void_p]),

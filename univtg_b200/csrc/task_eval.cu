@@ -4,6 +4,8 @@
 //   univtg_qfvs_match    eval/qfvs.py calculate_semantic_matching: the total weight of a maximum-weight bipartite matching
 //                        between machine-summary and ground-truth shots, weights the semantic IoU of their tag sets.  One block
 //                        per query.
+//   univtg_qfvs_eval_select  main/inference_qfvs.py eval_epoch: each query's score, its top k and the tag masks of the chosen
+//                        shots, written into the epoch's pools.  One block per query.
 // All arithmetic is IEEE double with explicit _rn intrinsics (no FMA contraction), so univtg_eval_hl_topk's APs equal the
 // reference's Python floats bit for bit.
 #include <math.h>
@@ -398,6 +400,122 @@ __global__ void __launch_bounds__(kMatchThreads) qfvs_match_kernel(const MatchAr
   }
 }
 
+// ---- QFVS evaluation epoch: per-query score, top k and the matching's machine side --------------------------------------
+// main/inference_qfvs.py eval_epoch for the queries of one chunk: the score of each kept position in the reference's fp32
+// order, score.topk(k) as torch.topk on CUDA orders it (descending, NaN above every number; ties by ascending index above 32
+// results, by torch's bitonic network up to 32) and the
+// tag masks of the chosen shots.  One block per query; the top k comes from a bitonic sort of n (<= 8,192) 64-bit keys
+// (order-preserving score << 32 | ~index) in shared memory.
+constexpr int kSelectMaxN = 8192;
+constexpr int kSelectThreads = 1024;
+constexpr int kTopkSmallSort = 32;  // torch.topk results up to this size are sorted by at::native's unstable bitonic network
+
+struct SelectArgs {
+  const float* logits[3];  // [F, N] per variant: concept 1, concept 2, both (NULL when the variant is not read)
+  const float* sal[3];
+  const int32_t* pos;      // [n] kept positions of mask_GT, row-major, cut to n
+  const uint64_t* tags;    // [>= n] tag mask per shot
+  float* score;            // [Q, n]
+  int32_t* top;            // [Q, k]
+  uint64_t* a;             // [Q, k]
+  int N, n, k, mode, gather, q0;
+};
+
+__device__ __forceinline__ float variant_score(const SelectArgs& a, int v, size_t i) {
+  if (a.mode == 0) return a.logits[v][i];
+  if (a.mode == 1) return a.sal[v][i];
+  return __fadd_rn(__fadd_rn(0.0f, a.logits[v][i]), a.sal[v][i]);  // torch.zeros(n) += pred_logits; += saliency_scores
+}
+
+// descending order of torch.topk: NaN first, -0 == +0
+__device__ __forceinline__ uint32_t topk_key(float x) { return isnan(x) ? 0xffffffffu : order_key(x); }
+
+__global__ void __launch_bounds__(kSelectThreads) qfvs_eval_select_kernel(const SelectArgs a) {
+  pdl_prologue();
+  extern __shared__ unsigned long long s_key[];
+  const int f = blockIdx.x, tid = threadIdx.x;
+  const size_t q = (size_t)a.q0 + f;
+  int P = 1;
+  while (P < a.n) P <<= 1;
+  for (int i = tid; i < P; i += kSelectThreads) {
+    unsigned long long key = 0ull;  // below every real key: order_key(-inf) = 0x007fffff
+    if (i < a.n) {
+      const size_t p = (size_t)f * a.N + a.pos[i];
+      float s = variant_score(a, 2, p);
+      if (a.gather) s = __fadd_rn(__fadd_rn(s, variant_score(a, 0, p)), variant_score(a, 1, p));  // score + score1 + score2
+      a.score[q * a.n + i] = s;
+      key = ((unsigned long long)topk_key(s) << 32) | (uint32_t)~(uint32_t)i;
+    }
+    s_key[i] = key;
+  }
+  __syncthreads();
+  for (int size = 2; size <= P; size <<= 1) {
+    for (int stride = size >> 1; stride > 0; stride >>= 1) {
+      for (int t = tid; t < P / 2; t += kSelectThreads) {
+        const int lo = 2 * t - (t & (stride - 1)), hi = lo + stride;
+        const unsigned long long x = s_key[lo], y = s_key[hi];
+        if (((lo & size) == 0) == (x < y)) {  // blocks with (lo & size) == 0 run descending, so the last pass is descending
+          s_key[lo] = y;
+          s_key[hi] = x;
+        }
+      }
+      __syncthreads();
+    }
+  }
+  if (a.k > kTopkSmallSort) {  // torch.topk sorts larger results stably: ties stay in ascending index order
+    for (int j = tid; j < a.k; j += kSelectThreads) {
+      const int i = (int)~(uint32_t)s_key[j];
+      a.top[q * a.k + j] = i;
+      a.a[q * a.k + j] = a.tags[i];
+    }
+    return;
+  }
+  // k <= 32: torch.topk gathers the chosen elements (those above the k-th score by ascending index, then those equal to it by
+  // ascending index) and sorts them with a 32-wide bitonic network that is not stable; warp 0 runs the same network
+  __shared__ unsigned long long s_small[kTopkSmallSort];  // (score key << 32) | index
+  __shared__ bool s_valid[kTopkSmallSort];
+  if (tid >= 32) return;
+  const int lane = tid;
+  const uint32_t kth = (uint32_t)(s_key[a.k - 1] >> 32);
+  const unsigned long long e = lane < a.k ? s_key[lane] : 0ull;
+  const uint32_t hi = (uint32_t)(e >> 32), idx = ~(uint32_t)e;
+  const bool above = lane < a.k && hi > kth;
+  const unsigned above_mask = __ballot_sync(0xffffffffu, above);
+  int before = 0;  // entries above the k-th score with a smaller index
+  for (int j = 0; j < 32; ++j) {
+    const uint32_t other = __shfl_sync(0xffffffffu, idx, j);
+    before += ((above_mask >> j) & 1u) && other < idx;
+  }
+  const int slot = above ? before : lane;  // the equal ones already sit at the end of the first k, by ascending index
+  s_small[slot] = lane < a.k ? (((unsigned long long)hi << 32) | idx) : 0ull;
+  s_valid[slot] = lane < a.k;
+  __syncwarp();
+  // at::native bitonicSort<32> with GTOp: swap = (A > B && validA) || !validB; exchange when swap == dir
+  auto step = [&](int stride, bool dir) {
+    if (lane < kTopkSmallSort / 2) {
+      const int p = 2 * lane - (lane & (stride - 1)), r = p + stride;
+      const bool sw = ((uint32_t)(s_small[p] >> 32) > (uint32_t)(s_small[r] >> 32) && s_valid[p]) || !s_valid[r];
+      if (sw == dir) {
+        const unsigned long long t = s_small[p];
+        s_small[p] = s_small[r];
+        s_small[r] = t;
+        const bool v = s_valid[p];
+        s_valid[p] = s_valid[r];
+        s_valid[r] = v;
+      }
+    }
+    __syncwarp();
+  };
+  for (int size = 2; size < kTopkSmallSort; size *= 2)
+    for (int stride = size / 2; stride > 0; stride /= 2) step(stride, (lane & (size / 2)) != 0);
+  for (int stride = kTopkSmallSort / 2; stride > 0; stride /= 2) step(stride, false);
+  if (lane < a.k) {
+    const int i = (int)(uint32_t)s_small[lane];
+    a.top[q * a.k + lane] = i;
+    a.a[q * a.k + lane] = a.tags[i];
+  }
+}
+
 }  // namespace
 }  // namespace uv
 
@@ -430,5 +548,42 @@ extern "C" int univtg_qfvs_match(const uint64_t* a, const int32_t* a_off, const 
   launch_k(qfvs_match_kernel, dim3(Q), dim3(kMatchThreads), 0, reinterpret_cast<cudaStream_t>(stream), args);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) set_error("univtg_qfvs_match launch failed: %s", cudaGetErrorString(e));
+  return (int)e;
+}
+
+extern "C" int univtg_qfvs_eval_select(const float* logits1, const float* sal1, const float* logits2, const float* sal2,
+                                       const float* logits_o, const float* sal_o, const int32_t* pos, const uint64_t* tags, int32_t F,
+                                       int32_t N, int32_t n, int32_t k, int32_t mode, int32_t gather, int32_t q0, float* score,
+                                       int32_t* top, uint64_t* a, void* stream) {
+  using namespace uv;
+  const bool need_l = mode != 1, need_s = mode != 0;
+  bool ok = pos && tags && score && top && a && F >= 0 && N >= 1 && n >= 1 && n <= N && n <= kSelectMaxN && k >= 1 && k <= n &&
+            mode >= 0 && mode <= 2 && (gather == 0 || gather == 1) && q0 >= 0;
+  const float* lg[3] = {logits1, logits2, logits_o};
+  const float* sl[3] = {sal1, sal2, sal_o};
+  for (int v = gather ? 0 : 2; ok && v < 3; ++v) ok = (!need_l || lg[v]) && (!need_s || sl[v]);
+  if (!ok) {
+    set_error("univtg_qfvs_eval_select: bad argument (n in 1..min(N, %d), k in 1..n, mode 0..2, gather 0 or 1, the outputs the "
+              "mode and gather read non-NULL)", kSelectMaxN);
+    return 1;
+  }
+  if (F == 0) return 0;
+  static bool attr_set = false;
+  if (!attr_set) {
+    cudaError_t e = cudaFuncSetAttribute(qfvs_eval_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         kSelectMaxN * (int)sizeof(unsigned long long));
+    if (e != cudaSuccess) {
+      set_error("cudaFuncSetAttribute(qfvs_eval_select): %s", cudaGetErrorString(e));
+      return (int)e;
+    }
+    attr_set = true;
+  }
+  int P = 1;
+  while (P < n) P <<= 1;
+  SelectArgs args{{logits1, logits2, logits_o}, {sal1, sal2, sal_o}, pos, tags, score, top, a, N, n, k, mode, gather, q0};
+  launch_k(qfvs_eval_select_kernel, dim3(F), dim3(kSelectThreads), (size_t)P * sizeof(unsigned long long),
+           reinterpret_cast<cudaStream_t>(stream), args);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) set_error("univtg_qfvs_eval_select launch failed: %s", cudaGetErrorString(e));
   return (int)e;
 }

@@ -820,3 +820,116 @@ class ReplayEvalModel(torch.nn.Module):
                "src_vid_mask": src_vid_mask}
         dev = self.anchor.device
         return {k: v.to(dev) for k, v in out.items()}
+
+
+# ---- QFVS evaluation epoch (main/inference_qfvs.py eval_epoch) ------------------------------------------------------------
+QFVS_CONCEPTS = ("Beach", "Car", "Cupglass", "Musicalinstrument", "Petsanimal", "Tree", "Sky", "Food", "Water", "Book")
+
+
+def qfvs_eval_config(**over):
+    """The config dict eval_epoch reads (main/train_qfvs.py update_config), at the reference's defaults."""
+    cfg = dict(test_videos=[1], txt_feature="txt_clip", vid_feature="vid_clip", max_segment_num=20, max_frame_num=200,
+               top_percent=0.02, qfvs_score_ensemble=1, qfvs_score_gather=1)
+    cfg.update(over)
+    return cfg
+
+
+def qfvs_eval_opt(**over):
+    """The opt fields eval_epoch reads, at the defaults of main/config.py."""
+    opt = dict(dset_name="qfvs", qfvs_split=1, f_loss_coef=10.0, s_loss_intra_coef=0.1)
+    opt.update(over)
+    return Namespace(**opt)
+
+
+def h5py_stub():
+    """A module standing in for h5py: File(path) reads the npz archive write_qfvs_eval_tree stores at the .h5 path, so
+    file["features"][()] and file["seg_len"][()] give the stored arrays."""
+    import types
+
+    import numpy as np
+
+    mod = types.ModuleType("h5py")
+    mod.File = lambda path, mode="r": np.load(path)
+    return mod
+
+
+def write_qfvs_eval_tree(root, seed, video_id=1, S=4, Lf=16, seg_len=(16, 16, 16, 5), dv=6, dt=8, shots=(60, 60, 60, 60),
+                         files=(("Beach", "Car"), ("Cupglass", "Tree")), tokens=None, gt_sizes=(5, 3), gt_extra=()):
+    """Writes the inputs of eval_epoch under root, in the layout and formats the reference reads: data/qfvs/txt_clip/txt_clip.pkl
+    (concept -> [tokens, dt] float32, tokens from `tokens` or 1..3), data/qfvs/processed/P0<v>_vid_clip.h5 (an npz archive, read
+    through h5py_stub(): features [S', Lf', dv] float32, seg_len), one oracle summary file per (concept 1, concept 2) pair with
+    1-based shot numbers (gt_extra: raw lines added to the file of the same index), eval/Tags.mat with the struct / cell layout of
+    the released one (Tags(v).Bin_Vecs{i} a 1 x 48 uint8 row; `shots` per video) and the plot directory."""
+    import os
+    import pickle
+
+    import numpy as np
+    import scipy.io
+
+    rng = random.Random(seed)
+    g = torch.Generator().manual_seed(seed)
+    tokens = dict(tokens or {})
+    emb = {}
+    for c in sorted(set(QFVS_CONCEPTS) | {"Glass", "Instrument", "Animal"}):
+        emb[c] = torch.randn(tokens.get(c, rng.randint(1, 3)), dt, generator=g).numpy()
+    for d in ("data/qfvs/txt_clip", "data/qfvs/processed", f"{QFVS_SUMMARY_DIR}{video_id}", "eval", "plot/qfvs"):
+        os.makedirs(os.path.join(root, d), exist_ok=True)
+    with open(os.path.join(root, "data/qfvs/txt_clip/txt_clip.pkl"), "wb") as f:
+        pickle.dump(emb, f)
+    seg = np.asarray(seg_len, dtype=np.int64)
+    feats = torch.randn(S, Lf, dv, generator=g).numpy()
+    with open(os.path.join(root, f"data/qfvs/processed/P0{video_id}_vid_clip.h5"), "wb") as f:
+        np.savez(f, features=feats, seg_len=seg)
+    n_shots = shots[video_id - 1]
+    for i, (c1, c2) in enumerate(files):
+        gt = sorted(rng.sample(range(1, n_shots + 1), gt_sizes[i % len(gt_sizes)]))
+        lines = [str(x) for x in gt] + [str(x) for x in (gt_extra[i] if i < len(gt_extra) else ())]
+        with open(os.path.join(root, f"{QFVS_SUMMARY_DIR}{video_id}", f"{c1}_{c2}_oracle.txt"), "w") as f:
+            f.write("\n".join(lines) + "\n")
+    tags = np.empty((1, len(shots)), dtype=[("Bin_Vecs", "O")])
+    for v, n in enumerate(shots):
+        t = make_shot_tags(seed * 10 + v, n)
+        cells = np.empty((n, 1), dtype=object)
+        for i in range(n):
+            cells[i, 0] = t[i:i + 1]
+        tags[0, v]["Bin_Vecs"] = cells
+    scipy.io.savemat(os.path.join(root, "eval/Tags.mat"), {"Tags": tags})
+
+
+QFVS_SUMMARY_DIR = "data/qfvs/metadata/origin_data/Query-Focused_Summaries/Oracle_Summaries/P0"
+
+
+class QFVSReplayModel(torch.nn.Module):
+    """Stands in for the model in the QFVS eval_epoch.  Each sample's outputs are drawn from a generator keyed by the sample's own
+    inputs (its text and video rows) and the seed, so they do not depend on how samples are batched or how often the model is
+    called.  pred_logits and saliency_scores are normal draws; one logit per sample is -0.0 (the ensemble's `0 +` turns it into
+    +0.0).  Outputs land on the device of the model's one buffer."""
+
+    def __init__(self, seed, d=8):
+        super().__init__()
+        self.seed, self.d, self.calls = seed, d, 0
+        self.register_buffer("anchor", torch.zeros(1))
+
+    def forward(self, src_txt, src_txt_mask, src_vid, src_vid_mask):
+        import hashlib
+
+        self.calls += 1
+        B, Lv = src_vid.shape[:2]
+        txt = src_txt.detach().to(torch.float32).cpu().numpy()
+        vid = src_vid.detach().to(torch.float32).cpu().numpy()
+        logits, sal, vm, tm = [], [], [], []
+        for b in range(B):
+            h = hashlib.sha256(struct.pack("<q", self.seed) + txt[b].tobytes() + vid[b].tobytes()).digest()
+            g = torch.Generator().manual_seed(int.from_bytes(h[:8], "little") >> 1)
+            lg = torch.randn(Lv, generator=g)
+            lg[int(torch.randint(0, Lv, (1,), generator=g))] = -0.0
+            logits.append(lg)
+            sal.append(torch.randn(Lv, generator=g))
+            vm.append(torch.randn(Lv, self.d, generator=g))
+            tm.append(torch.randn(1, self.d, generator=g))
+        out = {"pred_logits": torch.stack(logits)[..., None], "pred_spans": torch.zeros(B, Lv, 2), "saliency_scores": torch.stack(sal),
+               "vid_mem_proj": torch.stack(vm), "txt_mem_proj": torch.stack(tm)}
+        dev = self.anchor.device
+        out = {k: v.to(dev) for k, v in out.items()}
+        out["src_vid_mask"] = src_vid_mask
+        return out
